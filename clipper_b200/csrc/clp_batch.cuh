@@ -74,7 +74,7 @@ __host__ __device__ inline BatchSmem batch_smem_plan(int max_m) {
   b.hist = o; o += (nb + 1) * 4; o = (o + 15u) & ~15u;            // counting sort of the rows by length
   b.scan = o; o += 64;                                             // block scan scratch
   b.ring = o; o += kFillWarps * 4 * kRing * (4 + 2);               // item-wise fill rings
-  const unsigned int solve = res_smem_plan(max_m, kBatchWarps, 0, kBatchU, res_chunk_bytes(4, false)).total;
+  const unsigned int solve = res_smem_plan(max_m, kBatchWarps).total;
   b.total = (o > solve ? o : solve) + 128;
   return b;
 }
@@ -353,7 +353,7 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
     if (tid == 0) {
       ResArgs a;
       a.sp.val = val; a.sp.off16 = idx; a.sp.itemptr = itemptr; a.sp.rowid = rowid; a.sp.rows_pad = rows_pad; a.sp.plain = 1;
-      a.sp.cta_first = ctafirst; a.sp.cta_chunk = ctafirst; a.sp.head_chunks = 0u; a.sp.head_where = 0;
+      a.sp.cta_first = ctafirst;
       a.m = m; a.row0 = 0; a.rows = m; a.rows_pad = rows_pad; a.NI = NI; a.G = 1;
       a.prm = ba.prm;
       a.u0 = ba.u0 + P.u_off;
@@ -367,12 +367,12 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
       a.out = ba.out + p;
       a.rank = 0; a.world = 1;
       for (int r = 0; r < kMaxPeers; ++r) { a.peer_ll[r] = nullptr; a.peer_comm[r] = nullptr; }
-      a.comm = nullptr; a.seq0 = 0; a.spin_limit = ba.spin_limit; a.ll_gpu_scope = 0; a.ring_stages = 0; a.pieces_cap = 0u; a.state_cap = 0u; a.redll = nullptr; a.prof_cta = nullptr; a.prof_laps = 0;
+      a.comm = nullptr; a.seq0 = 0; a.spin_limit = ba.spin_limit; a.pieces_cap = 0u; a.state_cap = 0u; a.redll = nullptr; a.prof_cta = nullptr; a.prof_laps = 0;
       sa = a;
     }
     __syncthreads();
     const unsigned long long t_built = global_ns();
-    res_solve_body<float, kBatchThreads, kBatchU, kBatchD, false, false, true, /*coherent loads*/ true>(sa, smem);
+    res_solve_body<float, kBatchThreads, kBatchU, kBatchD, false, true, /*coherent loads*/ true>(sa, smem);
     if (ba.prof && tid == 0) {
       const unsigned long long t_end = global_ns();
       ba.prof[(size_t)p * 4 + 0] = t_scored - t_begin; ba.prof[(size_t)p * 4 + 1] = t_built - t_scored;

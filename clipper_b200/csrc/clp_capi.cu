@@ -61,8 +61,6 @@ struct clp_handle_s {
   int ctas_per_sm = 2;       // dense sweeps (and the user cap set by clp_set_ctas_per_sm)
   int ctas_sparse = 3;       // compact-row sweep: latency-bound, few registers -> 3 CTAs per SM
   int ctas_cap = 3;          // user cap (clp_set_ctas_per_sm)
-  int head_kb = env_int("CLP_HEAD_KB", 0);       // compact sweep: KB per CTA prefetched into L2 during the sync steps
-  int head_where = env_int("CLP_HEAD_WHERE", 1);
   int ctas_for(int mode) const { return std::min(ctas_cap, mode == 3 ? ctas_sparse : ctas_per_sm); }
   int grid_cap = 0;          // > 0: at most this many CTAs in the persistent kernels (clp_set_grid_cap)
   int spin_seconds = env_int("CLP_SPIN_SECONDS", 4);  // bound of every in-kernel wait of the resident solver
@@ -93,14 +91,10 @@ struct clp_handle_s {
   int score_filter = env_int("CLP_SCORE_FILTER", 1);
   // resident-vector solver (clp_resident.cuh): the default whenever the whole trial vector fits shared memory
   int res_enabled = env_int("CLP_RESIDENT", 1);
-  int res_cfg = env_int("CLP_RES_CFG", -1);         // load pipeline of the resident sweep (-1: automatic), see kResCfgs
-  int res_cfg_eff = 0;
   int res_smem_extra = env_int("CLP_RES_SMEM_EXTRA", 1);  // 0: launch with the plan's minimum (piece table / row state in HBM)
   int prof_ctas = env_int("CLP_PROF_CTAS", 0);      // print the per-CTA phase times of every resident solve (stderr)
   int prof_host = env_int("CLP_PROF_HOST", 0);      // print wall-clock marks of the scoring / solve calls (stderr)
   int prof_laps = env_int("CLP_PROF_LAPS", 1);      // in-kernel phase timers (the split reported in clp_solution.prof_*)
-  int stage_bulk = env_int("CLP_STAGE_BULK", 1);    // unsharded resident solver: trial vector staged by cp.async.bulk (0: register loads)
-  int ll_gpu_scope = env_int("CLP_LL_GPU_SCOPE", 1);  // sharded staging: gpu-scope first look at an LL cell (system-scope polls follow)
   int res_G_env = env_int("CLP_RES_G", 0);          // > 0: CTAs of the resident kernels (A/B runs)
   int item_cost = env_int("CLP_ITEM_COST", (int)kItemCost);  // fixed cost of an item in the partition of the sweep (A/B runs)
   DevBuf prof_buf;
@@ -112,7 +106,6 @@ struct clp_handle_s {
   bool score_pending = false;                       // a scoring launch's error flag has not been read back yet
   bool counts_fused = false;                        // sp_ptr4 already holds the counts of the current matrix
   long long counts_m = 0; int counts_rows_pad = 0, counts_nseg = 0, counts_W = 0;  // ... which was this one
-  int fill_items = env_int("CLP_FILL_ITEMS", 1);  // compact copy written item-wise (coalesced) instead of row-wise
   int pack = env_int("CLP_PACK", 1);              // resident layout of plain fp32 matrices with 4-byte entries (0: always 6 bytes)
   bool counts_win = false;                          // the fused counts came with the occupied-window bitmap (sp_win)
 
@@ -138,7 +131,7 @@ struct clp_handle_s {
                           //            4 auto (6 if the vector fits shared memory, else 3, when the graph is sparse enough; else 2 / 0)
   int dense_mode_eff = 2; // effective, decided when the matrix is finalised
   // compact-row copy (clp_sparse.cuh)
-  DevBuf sp_val, sp_col, sp_ptr4, sp_part, sp_item, sp_rowid, sp_rank;  // sp_ptr4: kept entries per (segment, row)
+  DevBuf sp_val, sp_col, sp_ptr4, sp_part, sp_item, sp_rowid;  // sp_ptr4: kept entries per (segment, row)
   DevBuf sp_win, res_wcol;  // packed layout: occupied 16-column windows per row | members' columns where every warp starts
   unsigned long long sp_nnz = 0, sp_nnz_real = 0;
   SparseView sp{};
@@ -148,7 +141,6 @@ struct clp_handle_s {
 
   size_t esize() const { return storage == CLP_STORE_F64 ? 8 : 4; }
   int entry_bytes() const { return sp.packed ? 4 : (int)esize() + 2; }  // compact copy: bytes per stored entry
-  int chunk_bytes() const { return res_chunk_bytes((int)esize(), sp.packed != 0); }
   int wwords() const { return (int)((ld + 511) / 512); }  // 32-bit words of a row's window bitmap
   // the packed layout may be built: whole rows, fp32, one GPU, not switched off
   bool pack_candidate() const { return pack && storage == CLP_STORE_F32 && world == 1; }
@@ -293,52 +285,34 @@ int build_plan2(clp_handle h) {
 
 
 // ------------------------------------------------------------------------------------------
-// resident-vector solver (clp_resident.cuh): load-pipeline configurations, selectable with CLP_RES_CFG for A/B runs
+// resident-vector solver (clp_resident.cuh): one load pipeline per handle type (ResShape)
 // ------------------------------------------------------------------------------------------
-struct ResCfg { int NT, U, D, ring; const char* name; };
-const ResCfg kResCfgs[] = {
-    {768, 2, 3, 0, "768 threads, registers: 3 rounds x 2 chunks per lane"},
-    {768, 3, 2, 0, "768 threads, registers: 2 rounds x 3 chunks per lane"},
-    {512, 2, 4, 0, "512 threads, registers: 4 rounds x 2 chunks per lane"},
-    {768, 1, 3, 1, "768 threads, cp.async.bulk ring: 3 stages x 1 chunk per lane"},
-    {768, 2, 3, 1, "768 threads, cp.async.bulk ring: 3 stages x 2 chunks per lane"},
-    {512, 2, 4, 1, "512 threads, cp.async.bulk ring: 4 stages x 2 chunks per lane"},
-    {512, 2, 6, 1, "512 threads, cp.async.bulk ring: 6 stages x 2 chunks per lane"},
-    {512, 2, 2, 0, "512 threads, registers: 2 rounds x 2 chunks per lane (fp64 storage)"},
-};
-constexpr int kResCfgF64 = 7;
-constexpr int kNumResCfgs = (int)(sizeof(kResCfgs) / sizeof(kResCfgs[0]));
-
-// calls f.template operator()<NT, U, D, RING>() for configuration c
-template <typename F>
-auto res_dispatch(int c, F&& f) {
-  switch (c) {
-    case 1: return f.template operator()<768, 3, 2, false>();
-    case 2: return f.template operator()<512, 2, 4, false>();
-    case 3: return f.template operator()<768, 1, 3, true>();
-    case 4: return f.template operator()<768, 2, 3, true>();
-    case 5: return f.template operator()<512, 2, 4, true>();
-    case 6: return f.template operator()<512, 2, 6, true>();
-    case 7: return f.template operator()<512, 2, 2, false>();
-    default: return f.template operator()<768, 2, 3, false>();
-  }
+struct ResKernels { const void* solver; const void* matvec; int NT; };
+template <typename T>
+ResKernels res_kernels(clp_handle h) {
+  if (h->world > 1)
+    return {(const void*)solver_resident_kernel<T, true>, (const void*)matvec_resident_kernel<T, ResShape<T, true>>, ResShape<T, true>::NT};
+  using S = ResShape<T, false>;
+  if constexpr (sizeof(T) == 4)
+    if (h->sp.packed)
+      return {(const void*)solver_resident_kernel<T, false, true>, (const void*)matvec_resident_kernel<T, S, true>, S::NT};
+  return {(const void*)solver_resident_kernel<T, false>, (const void*)matvec_resident_kernel<T, S>, S::NT};
+}
+int res_warps(clp_handle h) {
+  return (h->storage == CLP_STORE_F64 ? res_kernels<double>(h) : res_kernels<float>(h)).NT / 32;
 }
 
-unsigned int res_smem_bytes(clp_handle h, int c) {  // the plan's minimum
-  const ResCfg& k = kResCfgs[c];
-  return res_smem_plan((int)h->m, k.NT / 32, k.ring ? k.D : 0, k.U, h->chunk_bytes()).total;
-}
 // On-chip tables behind the plan's minimum: the CTA's piece table and per-row solver state, sized for 1.5x the mean
 // CTA (a CTA that exceeds them falls back to the HBM copies on its own).  Kept to a few KB on purpose: launching with
 // all 227 KB leaves no L1 for the streaming sweep.
-void res_pick_caps(clp_handle h, int c, unsigned int* pieces_cap, unsigned int* state_cap) {
+void res_pick_caps(clp_handle h, unsigned int* pieces_cap, unsigned int* state_cap) {
   *pieces_cap = 0; *state_cap = 0;
   if (!h->res_smem_extra || h->res_G < 1) return;
-  const ResCfg& k = kResCfgs[c];
+  const int NW = res_warps(h);
   const unsigned int items = (unsigned int)((h->res_NI + h->res_G - 1) / h->res_G);
   // the partition is balanced by bytes, so CTAs holding short rows hold more items than the mean: 2x the mean + slack
-  unsigned int pc = 2 * items + 8 + (unsigned int)(k.NT / 32), sc = 4 * (2 * items + 8);
-  const unsigned int base = res_smem_plan((int)h->m, k.NT / 32, k.ring ? k.D : 0, k.U, h->chunk_bytes()).total;
+  unsigned int pc = 2 * items + 8 + (unsigned int)NW, sc = 4 * (2 * items + 8);
+  const unsigned int base = res_smem_plan((int)h->m, NW).total;
   const unsigned int budget = std::min<unsigned int>(32u << 10, (unsigned int)std::max(0, h->smem_optin - (int)base - 256));
   if (pc * 64u + sc * 72u > budget) {  // keep the piece table first, then as much row state as fits -- or none
     if (pc * 64u > budget) return;
@@ -346,59 +320,30 @@ void res_pick_caps(clp_handle h, int c, unsigned int* pieces_cap, unsigned int* 
   }
   *pieces_cap = pc; *state_cap = sc;
 }
-unsigned int res_launch_smem(clp_handle h, int c) {
-  const ResCfg& k = kResCfgs[c];
+unsigned int res_launch_smem(clp_handle h) {
   unsigned int pc, sc;
-  res_pick_caps(h, c, &pc, &sc);
-  return res_smem_plan((int)h->m, k.NT / 32, k.ring ? k.D : 0, k.U, h->chunk_bytes(), pc, sc).total_ext;
+  res_pick_caps(h, &pc, &sc);
+  return res_smem_plan((int)h->m, res_warps(h), pc, sc).total_ext;
 }
 
 // can the resident solver take a problem of this size on this handle?
 bool resident_possible(clp_handle h, long long m) {
   if (!h->res_enabled || m > kResMaxM || m > 65535) return false;
   if (!(h->dense_mode == 4 || h->dense_mode == 6)) return false;
-  return (long long)res_smem_plan((int)m, kResThreads / 32, 0, 2, res_chunk_bytes((int)h->esize(), false)).total <= (long long)h->smem_optin;
-}
-
-// the configuration used for the current matrix: the requested one if its shared memory fits, else the register pipeline
-int res_pick_cfg(clp_handle h) {
-  if (h->storage == CLP_STORE_F64) return kResCfgF64;  // 8-byte values: one light register pipeline
-  int c = h->res_cfg;
-  // automatic: on one H100 (sm_90a) the 512-thread 2 x 4 register pipeline gets 128 registers and spills less than the
-  // 768-thread instances, which are capped at 80; it measured 16.8 vs 17.7 ms per c2 solve against 2 x 3 (DESIGN.md
-  // section 6); with the packed layout it is again the fastest (12.4 ms against 13.1-14.8 for the others).
-  // Shards keep 3 x 2 (not measured on several H100s)
-  if (c < 0 || c >= kNumResCfgs || c == kResCfgF64) c = (h->world > 1) ? 0 : 2;
-  if ((long long)res_smem_bytes(h, c) > (long long)h->smem_optin) c = 0;
-  return c;
+  return (long long)res_smem_plan((int)m, kResThreads / 32).total <= (long long)h->smem_optin;
 }
 
 template <typename T>
-cudaError_t res_set_attrs(clp_handle h, int c, bool sharded) {
-  // [storage][configuration][sharded][packed][device]: set once per process (handles may live on different host threads)
-  static std::atomic<bool> done[2][kNumResCfgs][2][2][8];
-  const bool packed = h->sp.packed != 0;
-  std::atomic<bool>& flag = done[sizeof(T) == 8 ? 1 : 0][c][sharded ? 1 : 0][packed ? 1 : 0][h->device & 7];
+cudaError_t res_set_attrs(clp_handle h) {
+  // [storage][sharded][packed][device]: set once per process (handles may live on different host threads)
+  static std::atomic<bool> done[2][2][2][8];
+  std::atomic<bool>& flag = done[sizeof(T) == 8 ? 1 : 0][h->world > 1 ? 1 : 0][h->sp.packed ? 1 : 0][h->device & 7];
   if (flag.load(std::memory_order_acquire)) return cudaSuccess;
   // the attribute is a per-function PERMISSION shared by every handle of the process (two shards in one process ask
   // for different sizes): always the device maximum; the carve-out follows what each launch actually requests
-  const int bytes = h->smem_optin;
-  const cudaError_t rc = res_dispatch(c, [&]<int NT, int U, int D, bool RING>() -> cudaError_t {
-    if constexpr ((sizeof(T) == 8) != (NT == 512 && U == 2 && D == 2 && !RING)) return cudaErrorInvalidValue;
-    else {
-      if (packed) {
-        if constexpr (sizeof(T) == 4) {
-          cudaError_t e = cudaFuncSetAttribute(matvec_resident_kernel<T, NT, U, D, RING, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-          if (e != cudaSuccess) return e;
-          return cudaFuncSetAttribute(solver_resident_kernel<T, NT, U, D, RING, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-        }
-      }
-      cudaError_t e = cudaFuncSetAttribute(matvec_resident_kernel<T, NT, U, D, RING>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-      if (e != cudaSuccess) return e;
-      if (sharded) return cudaFuncSetAttribute(solver_resident_kernel<T, NT, U, D, RING, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-      return cudaFuncSetAttribute(solver_resident_kernel<T, NT, U, D, RING, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-    }
-  });
+  const ResKernels k = res_kernels<T>(h);
+  cudaError_t rc = cudaFuncSetAttribute(k.matvec, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin);
+  if (rc == cudaSuccess) rc = cudaFuncSetAttribute(k.solver, cudaFuncAttributeMaxDynamicSharedMemorySize, h->smem_optin);
   if (rc == cudaSuccess) flag.store(true, std::memory_order_release);
   return rc;
 }
@@ -425,51 +370,27 @@ ResArgs res_args(clp_handle h) {
   a.comm = h->comm.as<CommBlock>();
   for (int r = 0; r < kMaxPeers; ++r) { a.peer_ll[r] = h->peer_ll[r]; a.peer_comm[r] = h->peer_comm[r]; }
   a.spin_limit = (long long)h->spin_seconds * 1900000000LL;
-  a.ll_gpu_scope = h->ll_gpu_scope;
-  a.ring_stages = kResCfgs[h->res_cfg_eff].ring ? kResCfgs[h->res_cfg_eff].D : 0;
-  res_pick_caps(h, h->res_cfg_eff, &a.pieces_cap, &a.state_cap);
+  res_pick_caps(h, &a.pieces_cap, &a.state_cap);
   a.redll = h->res_redll.as<uint4>();
   a.prof_cta = h->prof_ctas ? h->prof_buf.as<double>() : nullptr;
   a.prof_laps = (h->prof_ctas || h->prof_laps) ? 1 : 0;
-  a.stage_bulk = h->stage_bulk;
   a.wcol = h->res_wcol.as<int>();
   return a;
 }
 
 template <typename T>
 cudaError_t launch_resident_solver(clp_handle h, ResArgs& a) {
-  const int c = h->res_cfg_eff;
-  const size_t bytes = res_launch_smem(h, c);
+  const ResKernels k = res_kernels<T>(h);
   void* args[] = {&a};
-  return res_dispatch(c, [&]<int NT, int U, int D, bool RING>() -> cudaError_t {
-    if constexpr ((sizeof(T) == 8) != (NT == 512 && U == 2 && D == 2 && !RING)) return cudaErrorInvalidValue;
-    else {
-      const void* fn = (h->world > 1) ? (const void*)solver_resident_kernel<T, NT, U, D, RING, true>
-                                      : (const void*)solver_resident_kernel<T, NT, U, D, RING, false>;
-      if constexpr (sizeof(T) == 4)
-        if (h->sp.packed) fn = (const void*)solver_resident_kernel<T, NT, U, D, RING, false, true>;
-      return cudaLaunchCooperativeKernel(fn, dim3(a.G), dim3(NT), args, bytes, h->stream);
-    }
-  });
+  return cudaLaunchCooperativeKernel(k.solver, dim3(a.G), dim3(k.NT), args, res_launch_smem(h), h->stream);
 }
 
 template <typename T>
 cudaError_t launch_resident_matvec(clp_handle h, const double* v, double d, double* y, double* Mv, double* Cv) {
-  const int c = h->res_cfg_eff;
-  const size_t bytes = res_launch_smem(h, c);
+  const ResKernels k = res_kernels<T>(h);
   ResArgs a = res_args(h);
-  return res_dispatch(c, [&]<int NT, int U, int D, bool RING>() -> cudaError_t {
-    if constexpr ((sizeof(T) == 8) != (NT == 512 && U == 2 && D == 2 && !RING)) return cudaErrorInvalidValue;
-    else {
-      if constexpr (sizeof(T) == 4)
-        if (h->sp.packed) {
-          matvec_resident_kernel<T, NT, U, D, RING, true><<<a.G, NT, bytes, h->stream>>>(a, v, d, y, Mv, Cv);
-          return cudaGetLastError();
-        }
-      matvec_resident_kernel<T, NT, U, D, RING><<<a.G, NT, bytes, h->stream>>>(a, v, d, y, Mv, Cv);
-      return cudaGetLastError();
-    }
-  });
+  void* args[] = {&a, &v, &d, &y, &Mv, &Cv};
+  return cudaLaunchKernel(k.matvec, dim3(a.G), dim3(k.NT), args, res_launch_smem(h), h->stream);
 }
 
 constexpr int kKeepDense = -1;  // build_sparse: the compact copy would not pay off (NOT an error code)
@@ -519,12 +440,10 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   const int NI = h->rows_pad / 4;
   const long long nitem = (long long)nseg * (NI + 1);
   CLP_CUDA(h, h->sp_rowid.ensure((size_t)nseg * h->rows_pad * sizeof(unsigned int)));
-  CLP_CUDA(h, h->sp_rank.ensure((size_t)nseg * h->rows_pad * sizeof(unsigned int)));
   CLP_CUDA(h, h->sp_item.ensure((size_t)nitem * sizeof(unsigned int)));
   const int nb = p.W / 4 + 2;  // possible slice lengths in chunks
   sell_sort_kernel<<<nseg, 1024, (size_t)(nb + 1) * sizeof(unsigned int), h->stream>>>(
-      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, h->sp_rowid.as<unsigned int>(), h->sp_rank.as<unsigned int>(),
-      fused ? &sb->counts[0] : nullptr, pc);
+      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, h->sp_rowid.as<unsigned int>(), fused ? &sb->counts[0] : nullptr, pc);
   CLP_CUDA(h, cudaGetLastError());
   sell_itemlen_kernel<<<(unsigned)((nitem + 255) / 256), 256, 0, h->stream>>>(h->sp_ptr4.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
                                                                               h->rows_pad, nseg, h->sp_item.as<unsigned int>(), pc);
@@ -563,16 +482,11 @@ int build_sparse(clp_handle h, bool force, bool resident) {
       sparse_fill_items_kernel<T, true><<<(unsigned)((NI + kFillWarps - 1) / kFillWarps), kFillWarps * 32, 0, h->stream>>>(
           M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
           h->sp_val.as<T>(), nullptr, 0, 0u, bias);
-  } else if (resident || (h->fill_items && !std::getenv("CLP_PROBE_NO_CONFLICT"))) {
+  } else {
     const long long nwarp = (long long)nseg * NI;
     sparse_fill_items_kernel<T><<<(unsigned)((nwarp + kFillWarps - 1) / kFillWarps), kFillWarps * 32, 0, h->stream>>>(
         M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
         h->sp_val.as<T>(), h->sp_col.as<unsigned short>(), resident ? 0 : 3, resident ? (unsigned int)h->m : kZeroSlot);
-  } else {
-    sparse_fill_kernel<T><<<blocks, 256, 0, h->stream>>>(M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg,
-                                                         h->sp_item.as<unsigned int>(), h->sp_rank.as<unsigned int>(),
-                                                         h->sp_val.as<T>(), h->sp_col.as<unsigned short>(),
-                                                         std::getenv("CLP_PROBE_NO_CONFLICT") ? 1 : 0);
   }
   CLP_CUDA(h, cudaGetLastError());
   h->sp.val = h->sp_val.p; h->sp.off16 = h->sp.packed ? nullptr : h->sp_col.as<unsigned short>();
@@ -588,31 +502,25 @@ int build_sparse(clp_handle h, bool force, bool resident) {
                                                         std::max<long long>(1, by_bytes)));
     if (h->res_G_env > 0) G = std::max(1, std::min(h->res_G_env, std::min(h->sm_count, std::max(1, NI / 2))));
     h->res_G = G;
-    h->res_cfg_eff = res_pick_cfg(h);
-    CLP_CUDA(h, res_set_attrs<T>(h, h->res_cfg_eff, h->world > 1));
-    const int NW = kResCfgs[h->res_cfg_eff].NT / 32;
+    CLP_CUDA(h, res_set_attrs<T>(h));
+    const int NW = res_warps(h);
     CLP_CUDA(h, h->res_vecs.ensure((size_t)R_SLOTS * h->mpad * sizeof(double)));
     CLP_CUDA(h, h->res_cand.ensure((size_t)4 * h->mpad * sizeof(double)));
     CLP_CUDA(h, h->res_pieces.ensure(((size_t)NI + (size_t)G * NW + 8) * kPieceVals * sizeof(double)));
     CLP_CUDA(h, h->res_redll.ensure((size_t)2 * G * kRedVals * sizeof(uint4)));
   }
-  CLP_CUDA(h, h->sp_part.ensure(2 * ((size_t)G + 1) * sizeof(unsigned int)));
+  CLP_CUDA(h, h->sp_part.ensure(((size_t)G + 1) * sizeof(unsigned int)));
   sparse_partition_kernel<<<(G + 1 + 255) / 256, 256, 0, h->stream>>>(h->sp.itemptr, h->rows_pad, nseg, G, h->sp_part.as<unsigned int>(),
-                                                                      h->sp_part.as<unsigned int>() + G + 1,
                                                                       (unsigned int)std::max(0, h->item_cost));
   CLP_CUDA(h, cudaGetLastError());
   h->sp.cta_first = h->sp_part.as<unsigned int>();
-  h->sp.cta_chunk = h->sp.cta_first + G + 1;
-  if (h->sp.packed) {  // where every warp of the chosen configuration starts: once per build, not per sweep
-    const int NW = kResCfgs[h->res_cfg_eff].NT / 32;
+  if (h->sp.packed) {  // where every warp of the resident kernels starts: once per build, not per sweep
+    const int NW = res_warps(h);
     CLP_CUDA(h, h->res_wcol.ensure((size_t)G * NW * 4 * sizeof(int)));
     res_warp_cols_kernel<<<(unsigned)((G * NW * 32 + 255) / 256), 256, 0, h->stream>>>(h->sp, G, NW, h->res_wcol.as<int>());
     CLP_CUDA(h, cudaGetLastError());
   }
   h->compact_resident = resident;
-  // head of every CTA's range kept warm in L2 across the synchronisation steps: 24 B per chunk (fp32)
-  h->sp.head_chunks = (unsigned int)(std::max(0, h->head_kb) * 1024 / (4 * ((int)sizeof(T) + 2)) / 256 * 256);
-  h->sp.head_where = h->head_where;
   return CLP_OK;
 }
 
@@ -1105,7 +1013,7 @@ int clp_destroy(clp_handle h) {
   for (int r = 0; r < kMaxPeers; ++r)
     if (h->peer_opened[r]) { cudaIpcCloseMemHandle(h->peer_open_ptr[r][0]); cudaIpcCloseMemHandle(h->peer_open_ptr[r][1]); }
   h->comm.release();
-  for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->sp_rank, &h->parts, &h->small,
+  for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf})
     b->release();
   if (h->pinned) cudaFreeHost(h->pinned);

@@ -1142,11 +1142,9 @@ __global__ void __launch_bounds__(kThreads, MODE == 3 ? 3 : 2) solver_kernel(Sol
   else out = block_sum_ordered(a.d2.sumpart, a.plan2.G, red_smem);
 #define CLP_EXCHANGE()                                                                      \
   CLP_LAP(ns_cb);                                                                           \
-  if constexpr (MODE == 3) sparse_prefetch_head<T>(a.sp);                                   \
   if (!exchange_sums(a, loc, vals, red_par, round, seq, red_smem, &smem_flag)) { status = 5; goto finish; } \
   CLP_LAP(ns_ex);
 #define CLP_BAR_CHECK()                                               \
-  if constexpr (MODE == 3) { if (a.sp.head_where == 2) sparse_prefetch_head<T>(a.sp); } \
   ++round;                                                            \
   grid_barrier(a.bar, round, &smem_flag);                             \
   if (*reinterpret_cast<volatile int*>(errp) != 0) { status = 5; goto finish; } \

@@ -25,9 +25,8 @@
 // of item boundaries: a warp adds up the part of an item it covers (a "piece") and the per-row epilogue adds the
 // pieces in stream order -- perfect balance inside the SM with one __syncthreads per sweep, and bit-reproducible.
 //
-// Loads: software-pipelined ld.global.nc rounds in registers (D rounds of U chunks per lane in flight), or -- when the
-// shared memory left beside the vector allows it -- a per-warp ring filled with cp.async.bulk (TMA engine, mbarrier
-// completion): bytes in flight then cost no registers.
+// Loads: software-pipelined ld.global.nc rounds in registers (D rounds of U chunks per lane in flight); ResShape holds
+// the one (threads, U, D) of each handle type.
 //
 // The same kernel body serves three callers: the single-GPU solve (grid = one CTA per SM), one rank of a row-sharded
 // multi-GPU solve (candidate vectors and rank totals cross NVLink as self-validating LL cells) and, with G = 1 and
@@ -40,6 +39,16 @@ constexpr int kResThreads = 768;                  // widest resident instance (2
 constexpr int kResWarps = kResThreads / 32;
 constexpr int kResMaxM = 27648;                   // largest m whose fp64 trial vector (+ scratch) fits 227 KB
 constexpr int kPieceVals = 8;                     // a piece: 4 members x (|M| v, C v)
+
+// Load pipeline of the resident kernels per handle type (storage T, sharded or not): NT threads, D rounds of U chunks
+// per lane in flight.  On one H100 (sm_90a) the 512-thread fp32 pipeline gets 128 registers and spills less than a
+// 768-thread one, which is capped at 80; it was the fastest with both layouts (DESIGN.md section 6).  Shards keep
+// 768 threads (not measured on several H100s).  fp64 entries: one light 2 x 2 pipeline.
+template <int NT_, int U_, int D_> struct ResPipe { static constexpr int NT = NT_, U = U_, D = D_; };
+template <typename T, bool SHARDED> struct ResShapeOf { using type = ResPipe<512, 2, 2>; };
+template <> struct ResShapeOf<float, false> { using type = ResPipe<512, 2, 4>; };
+template <> struct ResShapeOf<float, true> { using type = ResPipe<768, 2, 3>; };
+template <typename T, bool SHARDED> using ResShape = typename ResShapeOf<T, SHARDED>::type;
 
 enum ResVec : int { R_U0 = 0, R_U1, R_G0, R_G1, R_MV0, R_MV1, R_CV0, R_CV1, R_SLOTS };
 enum ResStage : int { RS_RAW = 0, RS_DIV = 1, RS_STEP = 2 };
@@ -64,13 +73,10 @@ struct ResArgs {
   CommBlock* peer_comm[kMaxPeers];
   unsigned long long seq0;
   long long spin_limit;    // clock64 ticks a wait may last before it raises the time-out flag
-  int ll_gpu_scope;        // sharded staging: first look at an LL cell with a gpu-scope load (1) or a system-scope one (0)
-  int ring_stages;         // > 0: cp.async.bulk ring with this many stages per warp (RING instances)
   unsigned int pieces_cap, state_cap;  // on-chip piece table (entries) / row state (rows) per CTA, 0: keep them in HBM
   uint4* redll;            // [2][G][8] per-CTA partial sums as self-validating LL cells (zeroed before the launch)
   double* prof_cta;        // nullable: [G][8] per-CTA phase times in ns (sweeps, epilogues, exchanges, staging), items, chunks
   int prof_laps;           // thread 0 of every CTA reads %globaltimer four times per evaluation (phase split in clp_solution)
-  int stage_bulk;          // unsharded solver: the candidate vector enters shared memory by cp.async.bulk (res_stage_bulk)
   const int* wcol;         // packed layout: [G][warps][4] column of each member's last entry before the warp's stream (-1: none)
 };
 
@@ -109,31 +115,22 @@ __device__ __forceinline__ void mbar_wait(void* bar, unsigned int parity, int* e
 // ---------------------------------------------------------------------------------------------------------------
 constexpr unsigned int kStageBlocks = 8;  // sub-blocks (one mbarrier each) of a bulk-copied trial vector
 struct ResSmem {
-  unsigned int off_red, off_fin, off_wb, off_misc, off_bar, off_sbar, off_ring, total;
-  unsigned int stage_bytes;
+  unsigned int off_red, off_fin, off_wb, off_misc, off_sbar, total;
   // optional on-chip tables behind the plan's minimum (capacities chosen by the host, a few KB: the more shared
   // memory a CTA takes, the less L1 is left for the streaming loads): the CTA's piece table, and per row the solver
   // state (8 doubles) and a descriptor (global row, first / last warp of its pieces).  A CTA whose items / rows
   // exceed the capacities uses the HBM copies instead.
   unsigned int off_pieces, pieces_cap, off_state, state_cap, off_desc, total_ext;
 };
-// bytes of one chunk: 4 values + 4 column indices, or 4 packed words
-__host__ __device__ inline int res_chunk_bytes(int esize, bool packed) { return packed ? 16 : 4 * esize + 8; }
-__host__ __device__ inline unsigned int res_round_bytes(int U, int chunk) { return (unsigned int)(32 * U * chunk); }
-__host__ __device__ inline ResSmem res_smem_plan(int m, int NW, int ring_stages, int U, int chunk, unsigned int pieces_cap = 0,
-                                                 unsigned int state_cap = 0) {
+__host__ __device__ inline ResSmem res_smem_plan(int m, int NW, unsigned int pieces_cap = 0, unsigned int state_cap = 0) {
   ResSmem s;
   unsigned int o = (unsigned int)(((m + 1 + 1) & ~1) * 8);        // vs[0..m], vs[m] = 0
   s.off_red = o; o += (unsigned int)(NW * kRedVals * 8);
   s.off_fin = o; o += (unsigned int)((2 + kMaxPeers) * kRedVals * 8);
   s.off_wb = o; o += (unsigned int)((NW + 1) * 4);
   o = (o + 7u) & ~7u;
-  s.off_misc = o; o += 128 + (unsigned int)NW * 8;  // per-warp: phase bits of the ring's mbarriers (persist across sweeps) | start of its stream (item, end)
-  s.off_bar = o; o += (unsigned int)(ring_stages > 0 ? NW * ring_stages * 8 : 0);
+  s.off_misc = o; o += (unsigned int)NW * 8;  // per warp: start of its stream (item, end)
   s.off_sbar = o; o += kStageBlocks * 8u;  // mbarriers of the bulk-copy staging (res_stage_bulk)
-  o = (o + 127u) & ~127u;
-  s.stage_bytes = res_round_bytes(U, chunk);
-  s.off_ring = o; o += (unsigned int)(ring_stages > 0 ? NW * ring_stages : 0) * s.stage_bytes;
   s.total = o;
   o = (o + 15u) & ~15u;
   s.pieces_cap = pieces_cap; s.state_cap = state_cap;
@@ -219,8 +216,8 @@ __device__ __forceinline__ void ll_ld4(const uint4* p, unsigned int& lo, unsigne
 
 template <int NT, bool SHARDED>
 __device__ double res_stage(int mode, int m, const double* src, const uint4* cells, unsigned int tag, double z,
-                            double* vs, double* red_s, double* fin, int* errp, long long spin_limit, int ll_gpu_scope = 0,
-                            int rot = 0, bool raw = false) {
+                            double* vs, double* red_s, double* fin, int* errp, long long spin_limit, int rot = 0,
+                            bool raw = false) {
   // raw: the vector is staged as it is and nothing is summed (returns 0) -- the caller applies 1/|w| to the row results
   // Every CTA of the grid reads the SAME m values at the same moment.  With all CTAs walking the vector in the same
   // order, four 8-byte loads in flight per thread, this step took a fifth of the solver at m = 20 000 while the sweep
@@ -254,10 +251,8 @@ __device__ double res_stage(int mode, int m, const double* src, const uint4* cel
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           lo[2 * b + e] = hi[2 * b + e] = 0u; t1[2 * b + e] = t2[2 * b + e] = tag;
-          if (q[b] >= 0 && 2 * q[b] + e < m) {
-            if (ll_gpu_scope) ll_ld4<true>(cells + 2 * q[b] + e, lo[2 * b + e], t1[2 * b + e], hi[2 * b + e], t2[2 * b + e]);
-            else ll_ld4<false>(cells + 2 * q[b] + e, lo[2 * b + e], t1[2 * b + e], hi[2 * b + e], t2[2 * b + e]);
-          }
+          if (q[b] >= 0 && 2 * q[b] + e < m)
+            ll_ld4<true>(cells + 2 * q[b] + e, lo[2 * b + e], t1[2 * b + e], hi[2 * b + e], t2[2 * b + e]);
         }
       }
 #pragma unroll
@@ -452,8 +447,8 @@ __device__ __forceinline__ unsigned int res_item_of(const unsigned int* itemptr,
 // COH: the compact copy was written earlier IN THIS LAUNCH (batched problems): no ld.global.nc, L2-coherent loads instead
 // PACK: 4-byte packed entries (plain fp32 matrices): the columns come from the deltas, a warp whose stream starts inside
 // an item takes its members' columns there from a.wcol; the carry restarts at -1 with every new item
-template <typename T, int NT, int U, int D, bool RING, bool COH = false, bool PACK = false>
-__device__ void res_sweep(const ResArgs& a, const int bid, const double* vs, unsigned char* smem, const ResSmem& plan, int* errp,
+template <typename T, int NT, int U, int D, bool COH = false, bool PACK = false>
+__device__ void res_sweep(const ResArgs& a, const int bid, const double* vs, unsigned char* smem, const ResSmem& plan,
                           double* ptab, unsigned int isub) {
   constexpr int NW = NT / 32;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -471,7 +466,7 @@ __device__ void res_sweep(const ResArgs& a, const int bid, const double* vs, uns
 
   // ---- producer cursor (warp-uniform): the piece being loaded.  Where a warp's stream starts never changes during a
   // solve: found once (binary search over the item pointers = a chain of dependent L2 loads) and kept in shared memory
-  uint2* wstart = reinterpret_cast<uint2*>(smem + plan.off_misc + 128) + warp;
+  uint2* wstart = reinterpret_cast<uint2*>(smem + plan.off_misc) + warp;
   unsigned int cit, ce;
   {
     const uint2 w = *wstart;
@@ -520,114 +515,47 @@ __device__ void res_sweep(const ResArgs& a, const int bid, const double* vs, uns
   };
   const bool plain = sp.plain != 0;
 
-  if constexpr (!RING) {
-    // D rounds of U chunks per lane in registers; the refill of a round is issued right after it has been applied,
-    // so D - 1 rounds are always in flight behind the one being consumed
-    std::conditional_t<PACK, Packed4, Entry4<T>> E[D][U];
-    unsigned int mitem[D];
-    bool mlast[D], mvalid[D];
-    auto produce = [&](int s) {
-      mvalid[s] = !pdone;
-      if (pdone) return;
-      unsigned int jb, n;
-      advance(jb, n, mitem[s], mlast[s]);
+  // D rounds of U chunks per lane in registers; the refill of a round is issued right after it has been applied,
+  // so D - 1 rounds are always in flight behind the one being consumed
+  std::conditional_t<PACK, Packed4, Entry4<T>> E[D][U];
+  unsigned int mitem[D];
+  bool mlast[D], mvalid[D];
+  auto produce = [&](int s) {
+    mvalid[s] = !pdone;
+    if (pdone) return;
+    unsigned int jb, n;
+    advance(jb, n, mitem[s], mlast[s]);
 #pragma unroll
-      for (int u = 0; u < U; ++u) {
-        const unsigned int c = lane + 32u * u;
-        if constexpr (PACK) {
-          if (c < n) { if constexpr (COH) E[s][u].load_cg(pw, 4ull * (jb + c)); else E[s][u].load(pw, 4ull * (jb + c)); }
-          else E[s][u].neutral();
-        } else {
-          if (c < n) { if constexpr (COH) E[s][u].load_cg(val, idx, 4ull * (jb + c)); else E[s][u].load(val, idx, 4ull * (jb + c)); }
-          else E[s][u].neutral_at(padk);
-        }
+    for (int u = 0; u < U; ++u) {
+      const unsigned int c = lane + 32u * u;
+      if constexpr (PACK) {
+        if (c < n) { if constexpr (COH) E[s][u].load_cg(pw, 4ull * (jb + c)); else E[s][u].load(pw, 4ull * (jb + c)); }
+        else E[s][u].neutral();
+      } else {
+        if (c < n) { if constexpr (COH) E[s][u].load_cg(val, idx, 4ull * (jb + c)); else E[s][u].load(val, idx, 4ull * (jb + c)); }
+        else E[s][u].neutral_at(padk);
       }
-    };
-#pragma unroll
-    for (int s = 0; s < D; ++s) produce(s);
-    for (;;) {
-      bool done = false;
-#pragma unroll
-      for (int s = 0; s < D; ++s) {
-        if (!mvalid[s]) { done = true; break; }
-        if constexpr (PACK) res_apply_packed<U>(E[s], vs, sp.ebias, carry, aM, aC);
-        else {
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            if (plain) res_apply_chunk<T, true>(E[s][u], vs, aM[u & 1], aC[u & 1]);
-            else res_apply_chunk<T, false>(E[s][u], vs, aM[u & 1], aC[u & 1]);
-          }
-        }
-        if (mlast[s]) { flush(mitem[s]); carry = -1; }
-        produce(s);
-      }
-      if (done) break;
     }
-  } else {
-    // per-warp ring of D stages in shared memory, filled by cp.async.bulk (one copy for the values, one for the
-    // column indices of a round; packed: one copy of the words), completion on one mbarrier per stage
-    unsigned char* ring = smem + plan.off_ring + (size_t)warp * D * plan.stage_bytes;
-    unsigned long long* bars = reinterpret_cast<unsigned long long*>(smem + plan.off_bar) + warp * D;
-    unsigned int mitem[D], mn[D];
-    bool mlast[D], mvalid[D];
-    unsigned int* parity_slot = reinterpret_cast<unsigned int*>(smem + plan.off_misc) + warp;
-    unsigned int parity = *parity_slot;  // bit s: phase the consumer waits for on stage s (the barriers live across sweeps)
-    auto produce = [&](int s) {
-      mvalid[s] = !pdone;
-      if (pdone) return;
-      unsigned int jb;
-      advance(jb, mn[s], mitem[s], mlast[s]);
-      if (lane == 0) {
-        unsigned char* st = ring + (size_t)s * plan.stage_bytes;
-        if constexpr (PACK) {
-          mbar_expect_tx(&bars[s], mn[s] * 16u);
-          bulk_g2s(st, pw + 4ull * jb, mn[s] * 16u, &bars[s]);
-        } else {
-          const unsigned int bv = mn[s] * 4u * (unsigned int)sizeof(T), bi = mn[s] * 8u;
-          mbar_expect_tx(&bars[s], bv + bi);
-          bulk_g2s(st, val + 4ull * jb, bv, &bars[s]);
-          bulk_g2s(st + 32u * U * 4u * sizeof(T), idx + 4ull * jb, bi, &bars[s]);
+  };
+#pragma unroll
+  for (int s = 0; s < D; ++s) produce(s);
+  for (;;) {
+    bool done = false;
+#pragma unroll
+    for (int s = 0; s < D; ++s) {
+      if (!mvalid[s]) { done = true; break; }
+      if constexpr (PACK) res_apply_packed<U>(E[s], vs, sp.ebias, carry, aM, aC);
+      else {
+#pragma unroll
+        for (int u = 0; u < U; ++u) {
+          if (plain) res_apply_chunk<T, true>(E[s][u], vs, aM[u & 1], aC[u & 1]);
+          else res_apply_chunk<T, false>(E[s][u], vs, aM[u & 1], aC[u & 1]);
         }
       }
-    };
-#pragma unroll
-    for (int s = 0; s < D; ++s) produce(s);
-    for (;;) {
-      bool done = false;
-#pragma unroll
-      for (int s = 0; s < D; ++s) {
-        if (!mvalid[s]) { done = true; break; }
-        mbar_wait(&bars[s], (parity >> s) & 1u, errp);
-        parity ^= 1u << s;
-        const unsigned char* st = ring + (size_t)s * plan.stage_bytes;
-        if constexpr (PACK) {
-          Packed4 e[U];
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            const unsigned int c = lane + 32u * u;
-            if (c < mn[s]) e[u].w = *reinterpret_cast<const uint4*>(st + (size_t)c * 16);
-            else e[u].neutral();
-          }
-          res_apply_packed<U>(e, vs, sp.ebias, carry, aM, aC);
-        } else {
-#pragma unroll
-          for (int u = 0; u < U; ++u) {
-            const unsigned int c = lane + 32u * u;
-            Entry4<T> e;
-            if (c < mn[s]) e.load_shared(st + (size_t)c * 4 * sizeof(T), st + 32u * U * 4u * sizeof(T) + (size_t)c * 8);
-            else e.neutral_at(padk);
-            if (plain) res_apply_chunk<T, true>(e, vs, aM[u & 1], aC[u & 1]);
-            else res_apply_chunk<T, false>(e, vs, aM[u & 1], aC[u & 1]);
-          }
-        }
-        if (mlast[s]) { flush(mitem[s]); carry = -1; }
-        __syncwarp();  // every lane has read the stage before the next bulk copy may overwrite it
-        produce(s);
-      }
-      if (done) break;
+      if (mlast[s]) { flush(mitem[s]); carry = -1; }
+      produce(s);
     }
-    __syncwarp();
-    if (lane == 0) *parity_slot = parity;
+    if (done) break;
   }
 }
 
@@ -791,11 +719,11 @@ __device__ bool res_exchange(const ResArgs& a, const int bid, const double (&loc
 // ---------------------------------------------------------------------------------------------------------------
 // the solver body (shared by solver_resident_kernel and the batched kernel)
 // ---------------------------------------------------------------------------------------------------------------
-template <typename T, int NT, int U, int D, bool RING, bool SHARDED, bool SOLO, bool COH = false, bool PACK = false>
+template <typename T, int NT, int U, int D, bool SHARDED, bool SOLO, bool COH = false, bool PACK = false>
 __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   constexpr int NW = NT / 32;
   const int bid = SOLO ? 0 : (int)blockIdx.x;  // CTA index within the problem (batched: one CTA per problem)
-  const ResSmem plan = res_smem_plan(a.m, NW, RING ? D : 0, U, res_chunk_bytes((int)sizeof(T), PACK), a.pieces_cap, a.state_cap);
+  const ResSmem plan = res_smem_plan(a.m, NW, a.pieces_cap, a.state_cap);
   double* vs = reinterpret_cast<double*>(smem);
   double* red_s = reinterpret_cast<double*>(smem + plan.off_red);
   double* fin = reinterpret_cast<double*>(smem + plan.off_fin);
@@ -812,18 +740,13 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
     const unsigned int c_lo = a.sp.itemptr[it0], c_hi = a.sp.itemptr[it1];
     wb[threadIdx.x] = res_warp_bound(c_lo, c_hi, threadIdx.x, NW);
   }
-  if (threadIdx.x < NW) reinterpret_cast<uint2*>(smem + plan.off_misc + 128)[threadIdx.x] = make_uint2(0u, 0u);
-  if constexpr (RING) {
-    if (threadIdx.x < NW * D) mbar_init(reinterpret_cast<unsigned long long*>(smem + plan.off_bar) + threadIdx.x, 1);
-    if (threadIdx.x < NW) reinterpret_cast<unsigned int*>(smem + plan.off_misc)[threadIdx.x] = 0u;
-    fence_mbar_init();
-  }
+  if (threadIdx.x < NW) reinterpret_cast<uint2*>(smem + plan.off_misc)[threadIdx.x] = make_uint2(0u, 0u);
   // bulk-copy staging of the candidate vector (one unsharded problem on the whole GPU only)
   unsigned long long* const sbars = reinterpret_cast<unsigned long long*>(smem + plan.off_sbar);
   unsigned int sphase = 0u;
-  const bool stage_bulk = !SHARDED && !SOLO && a.stage_bulk != 0;
+  constexpr bool stage_bulk = !SHARDED && !SOLO;
   // candidate staged as it is, 1/|w| applied to the row results: whenever a CTA owns fewer rows than the vector has entries
-  const bool stage_raw = !SOLO && a.stage_bulk != 0;
+  constexpr bool stage_raw = !SOLO;
   if constexpr (!SHARDED && !SOLO) {
     if (threadIdx.x < kStageBlocks) mbar_init(&sbars[threadIdx.x], 1);
     fence_mbar_init();
@@ -901,7 +824,7 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   if (!res_exchange<NT, SHARDED, SOLO>(a, bid, loc, vals, red_par, round, seq, red_s, fin)) { status = 5; goto finish; } \
   RES_LAP(ns_ex);
 #define RES_SWEEP()                                                                                 \
-  res_sweep<T, NT, U, D, RING, COH, PACK>(a, bid, vs, smem, plan, errp, ptab, isub);                                 \
+  res_sweep<T, NT, U, D, COH, PACK>(a, bid, vs, smem, plan, ptab, isub);                                             \
   ++n_matvec;                                                                                       \
   __syncthreads();                                                                                  \
   RES_LAP(ns_mv);
@@ -909,7 +832,7 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   // ---- phase 0: u = M u0 + u0 (or u0), squared norm (clipper.cpp:193-198) ---------------------
   {
     if (P.rescale_u0) {
-      res_stage<NT, SHARDED>(RS_RAW, m, a.u0, nullptr, 0u, 1.0, vs, red_s, fin, errp, a.spin_limit, 0, bid * 416);
+      res_stage<NT, SHARDED>(RS_RAW, m, a.u0, nullptr, 0u, 1.0, vs, red_s, fin, errp, a.spin_limit, bid * 416);
       RES_LAP(ns_st);
       RES_SWEEP();
     }
@@ -935,7 +858,7 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         ? res_stage_bulk<NT>(RS_DIV, m, a.cand + (size_t)(cpar * 2) * mp, z, vs, sbars, sphase, red_s, fin, errp, bid)
         : res_stage<NT, SHARDED>(RS_DIV, m, a.cand + (size_t)(cpar * 2) * mp,
                                  SHARDED ? a.ll + (size_t)(cpar * 2) * mp : nullptr, ctag, z, vs, red_s, fin,
-                                 errp, a.spin_limit, a.ll_gpu_scope, bid * 416);
+                                 errp, a.spin_limit, bid * 416);
     RES_LAP(ns_st);
     RES_SWEEP();
     cur = 1;
@@ -990,11 +913,11 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         if (stage_raw) {
           if (stage_bulk) res_stage_bulk<NT>(RS_STEP, m, a.cand + coff, z, vs, sbars, sphase, red_s, fin, errp, bid, true);
           else res_stage<NT, SHARDED>(RS_STEP, m, a.cand + coff, SHARDED ? a.ll + coff : nullptr, ctag, z, vs, red_s, fin, errp,
-                                      a.spin_limit, a.ll_gpu_scope, bid * 416, true);
+                                      a.spin_limit, bid * 416, true);
           sumv = lzs ? div_by_invariant(sw, nrm_l, rinv_l) : sw;
         } else {
           sumv = res_stage<NT, SHARDED>(RS_STEP, m, a.cand + coff, SHARDED ? a.ll + coff : nullptr, ctag, z,
-                                        vs, red_s, fin, errp, a.spin_limit, a.ll_gpu_scope, bid * 416);
+                                        vs, red_s, fin, errp, a.spin_limit, bid * 416);
         }
         RES_LAP(ns_st);
         RES_SWEEP();
@@ -1092,20 +1015,22 @@ finish:
 #undef RES_SWEEP
 }
 
-template <typename T, int NT, int U, int D, bool RING, bool SHARDED, bool PACK = false>
-__global__ void __launch_bounds__(NT, 1) solver_resident_kernel(ResArgs a) {
+template <typename T, bool SHARDED, bool PACK = false>
+__global__ void __launch_bounds__(ResShape<T, SHARDED>::NT, 1) solver_resident_kernel(ResArgs a) {
   extern __shared__ __align__(128) unsigned char clp_res_smem[];
-  res_solve_body<T, NT, U, D, RING, SHARDED, false, false, PACK>(a, clp_res_smem);
+  using S = ResShape<T, SHARDED>;
+  res_solve_body<T, S::NT, S::U, S::D, SHARDED, false, false, PACK>(a, clp_res_smem);
 }
 
-// stand-alone mat-vec on the resident layout: stage v, sweep, per-row epilogue -- one launch, no device-wide barrier
-template <typename T, int NT, int U, int D, bool RING, bool PACK = false>
-__global__ void __launch_bounds__(NT, 1) matvec_resident_kernel(ResArgs a, const double* v, double dpen, double* y,
-                                                                double* Mv_out, double* Cv_out) {
+// stand-alone mat-vec on the resident layout: stage v, sweep, per-row epilogue -- one launch, no device-wide barrier.
+// S: the ResShape of the handle's solver (the piece table and the warps' start columns are laid out for it)
+template <typename T, typename S, bool PACK = false>
+__global__ void __launch_bounds__(S::NT, 1) matvec_resident_kernel(ResArgs a, const double* v, double dpen, double* y,
+                                                                   double* Mv_out, double* Cv_out) {
   extern __shared__ __align__(128) unsigned char clp_res_smem[];
   unsigned char* smem = clp_res_smem;
-  constexpr int NW = NT / 32;
-  const ResSmem plan = res_smem_plan(a.m, NW, RING ? D : 0, U, res_chunk_bytes((int)sizeof(T), PACK), a.pieces_cap, a.state_cap);
+  constexpr int NT = S::NT, NW = NT / 32;
+  const ResSmem plan = res_smem_plan(a.m, NW, a.pieces_cap, a.state_cap);
   double* vs = reinterpret_cast<double*>(smem);
   double* red_s = reinterpret_cast<double*>(smem + plan.off_red);
   double* fin = reinterpret_cast<double*>(smem + plan.off_fin);
@@ -1113,18 +1038,13 @@ __global__ void __launch_bounds__(NT, 1) matvec_resident_kernel(ResArgs a, const
   const int bid = (int)blockIdx.x;
   const unsigned int it0 = a.sp.cta_first[bid], it1 = a.sp.cta_first[bid + 1];
   if (threadIdx.x <= NW) wb[threadIdx.x] = res_warp_bound(a.sp.itemptr[it0], a.sp.itemptr[it1], threadIdx.x, NW);
-  if (threadIdx.x < NW) reinterpret_cast<uint2*>(smem + plan.off_misc + 128)[threadIdx.x] = make_uint2(0u, 0u);
-  if constexpr (RING) {
-    if (threadIdx.x < NW * D) mbar_init(reinterpret_cast<unsigned long long*>(smem + plan.off_bar) + threadIdx.x, 1);
-    if (threadIdx.x < NW) reinterpret_cast<unsigned int*>(smem + plan.off_misc)[threadIdx.x] = 0u;
-    fence_mbar_init();
-  }
+  if (threadIdx.x < NW) reinterpret_cast<uint2*>(smem + plan.off_misc)[threadIdx.x] = make_uint2(0u, 0u);
   __syncthreads();
-  const double sumv = res_stage<NT, false>(RS_RAW, a.m, v, nullptr, 0u, 1.0, vs, red_s, fin, &a.sb->error, a.spin_limit, 0, bid * 416);
+  const double sumv = res_stage<NT, false>(RS_RAW, a.m, v, nullptr, 0u, 1.0, vs, red_s, fin, &a.sb->error, a.spin_limit, bid * 416);
   const bool ptab_sh = (it1 - it0) + (unsigned int)NW <= plan.pieces_cap;
   double* const ptab = ptab_sh ? reinterpret_cast<double*>(smem + plan.off_pieces) : a.pieces + (size_t)bid * NW * kPieceVals;
   const unsigned int isub = ptab_sh ? it0 : 0u;
-  res_sweep<T, NT, U, D, RING, false, PACK>(a, bid, vs, smem, plan, &a.sb->error, ptab, isub);
+  res_sweep<T, NT, S::U, S::D, false, PACK>(a, bid, vs, smem, plan, ptab, isub);
   __syncthreads();
   const int nrow = (int)(it1 - it0) * 4;
   unsigned int wmask = 0u;

@@ -49,9 +49,6 @@ struct SparseView {
   int rows_pad;
   int plain;                     // every kept entry has M > 0 and C = 1
   const unsigned int* cta_first; // [G + 1] first item of every CTA (balanced by bytes), see sparse_partition_kernel
-  const unsigned int* cta_chunk; // [G + 1] first chunk of every CTA's range
-  unsigned int head_chunks;      // chunks at the head of its range a CTA asks L2 to fetch while it waits (0: off)
-  int head_where;                // 1: before the wait that ends the combine step, 2: also before the one that ends the sweep
   int packed;                    // whole-row layout with 4-byte entries (val holds the words, no off16; see pack_word)
   unsigned int ebias;            // packed: (fp32 exponent of code 0) << 23
 };
@@ -159,10 +156,10 @@ __global__ void sparse_count_kernel(const T* M, long long ld, int m, int rows, i
 
 // pass 2: one block (1024 threads) per column segment sorts the rows by slice length, longest first (counting sort
 // over the nb = W/4 + 2 possible lengths in chunks; ties in row order: a stable sort, so the layout is reproducible).
-//   rowid[seg][pos] = row at sorted position pos, rank[seg][row] = its position
+//   rowid[seg][pos] = row at sorted position pos
 // Dynamic shared memory: (nb + 1) counters.
 // Packed builds (pc.on()) sort by kept entries + fillers: the stored length.
-__global__ void sell_sort_kernel(const unsigned int* cnt4, int rows_pad, int nb, unsigned int* rowid, unsigned int* rank,
+__global__ void sell_sort_kernel(const unsigned int* cnt4, int rows_pad, int nb, unsigned int* rowid,
                                  unsigned long long* total_entries /* nullable: += kept entries */, PackCount pc) {
   extern __shared__ unsigned int hist[];
   __shared__ unsigned int wsum[32];
@@ -222,11 +219,7 @@ __global__ void sell_sort_kernel(const unsigned int* cnt4, int rows_pad, int nb,
       __syncthreads();                  // spinning warps was several times slower)
     }
     start = __shfl_sync(0xffffffffu, start, leader);
-    if (have) {
-      const unsigned int pos = start + before;
-      rowid[(size_t)blockIdx.x * rows_pad + pos] = (unsigned int)r;
-      rank[(size_t)blockIdx.x * rows_pad + r] = pos;
-    }
+    if (have) rowid[(size_t)blockIdx.x * rows_pad + start + before] = (unsigned int)r;
   }
 }
 
@@ -292,64 +285,9 @@ __global__ void sparse_scan_fix_kernel(unsigned int* cnt4, int n, int nseg, cons
   for (int i = threadIdx.x; i < n; i += blockDim.x) a[i] += (unsigned int)base;
 }
 
-// pass 4: one warp per (padded) local row writes its kept entries, in column order, into its member lane of
-// its item in every segment, then the padding up to the item's length.
-template <typename T>
-__global__ void sparse_fill_kernel(const T* M, long long ld, int m, int rows, int rows_pad, int W, int nseg,
-                                   const unsigned int* itemptr, const unsigned int* rank, T* val, unsigned short* off16,
-                                   int probe_no_conflict) {
-  const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-  if (warp >= rows_pad) return;
-  const int NI = rows_pad >> 2;
-  for (int s = 0; s < nseg; ++s) {
-    const unsigned int pos = rank[(size_t)s * rows_pad + warp];
-    const unsigned int* ip = itemptr + (size_t)s * (NI + 1) + (pos >> 2);
-    const unsigned long long base = 4ull * ip[0] + 4ull * (pos & 3u);  // entry index of (chunk 0, member pos & 3)
-    const unsigned int cap = ip[1] - ip[0];                              // entries this member may hold (4 x chunks / 4)
-    // entry w of the slice lives at base + 16 * (w / 4) + (w % 4)
-    unsigned int n = 0;
-    if (warp < rows) {
-      const int c0 = s * W, c1 = min(m, c0 + W);
-      for (int j0 = c0; j0 < c1; j0 += 128) {
-        const int j = j0 + lane * 4;
-        T x[4];
-        unsigned int keep = 0;
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          x[e] = (j + e < c1) ? M[(size_t)warp * ld + j + e] : encode<T>(0.0, false);
-          keep |= (!is_neutral<T>(x[e]) ? 1u : 0u) << e;
-        }
-        const unsigned int cnt = __popc(keep);
-        unsigned int pre = cnt;  // inclusive scan over lanes
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const unsigned int y = __shfl_up_sync(0xffffffffu, pre, o);
-          if (lane >= o) pre += y;
-        }
-        const unsigned int total = __shfl_sync(0xffffffffu, pre, 31);
-        unsigned int w = n + (pre - cnt);
-#pragma unroll
-        for (int e = 0; e < 4; ++e)
-          if (keep & (1u << e)) {
-            const unsigned long long at = base + 16ull * (w >> 2) + (w & 3u);
-            val[at] = x[e]; off16[at] = (unsigned short)(8 * (j + e - c0)); ++w;
-            // timing probe only (wrong results): every half-warp of the sweep reads 16 distinct banks
-            if (probe_no_conflict) off16[at] = (unsigned short)(8 * (((at >> 2) - ip[0]) & 15u));
-          }
-        n += total;
-      }
-    }
-    for (unsigned int w = n + lane; w < cap; w += 32) {
-      const unsigned long long at = base + 16ull * (w >> 2) + (w & 3u);
-      val[at] = encode<T>(0.0, false); off16[at] = (unsigned short)kZeroSlot;
-    }
-  }
-}
-
-// pass 4, item-wise: one warp per item reads its four member rows together and compacts them through four
-// shared-memory rings; chunk k of all four members is then 64 contiguous bytes of val (32 of off16), so a flush
-// of 8 chunks per member is one fully coalesced 512-byte store (the row-wise kernel above issues 4- and 2-byte
-// stores that each touch a different sector).
+// pass 4: one warp per item reads its four member rows together and compacts them through four shared-memory
+// rings; chunk k of all four members is then 64 contiguous bytes of val (32 of off16), so a flush of 8 chunks per
+// member is one fully coalesced 512-byte store.
 constexpr int kFillWarps = 4;
 constexpr int kRing = 256;  // entries per member ring: < 36 left after a flush + <= 128 new ones per step
 // one warp: the item whose chunks are [b, e) of the stream and whose members are rows r[0..3]; columns [c0, c1)
@@ -495,9 +433,6 @@ template <> struct Entry4<float> {
   __device__ __forceinline__ float get(int e) const { return e == 0 ? x.x : e == 1 ? x.y : e == 2 ? x.z : x.w; }
   __device__ __forceinline__ void neutral() { x = make_float4(-0.f, -0.f, -0.f, -0.f); k = make_uint2(kZeroSlot | (kZeroSlot << 16), kZeroSlot | (kZeroSlot << 16)); }
   __device__ __forceinline__ void neutral_at(unsigned int kk) { x = make_float4(-0.f, -0.f, -0.f, -0.f); k = make_uint2(kk, kk); }
-  __device__ __forceinline__ void load_shared(const void* pv, const void* pi) {
-    x = *reinterpret_cast<const float4*>(pv); k = *reinterpret_cast<const uint2*>(pi);
-  }
 };
 template <> struct Entry4<double> {
   double2 a, b; uint2 k;
@@ -514,9 +449,6 @@ template <> struct Entry4<double> {
   __device__ __forceinline__ double get(int e) const { return e == 0 ? a.x : e == 1 ? a.y : e == 2 ? b.x : b.y; }
   __device__ __forceinline__ void neutral() { a = make_double2(-0.0, -0.0); b = a; k = make_uint2(kZeroSlot | (kZeroSlot << 16), kZeroSlot | (kZeroSlot << 16)); }
   __device__ __forceinline__ void neutral_at(unsigned int kk) { a = make_double2(-0.0, -0.0); b = a; k = make_uint2(kk, kk); }
-  __device__ __forceinline__ void load_shared(const void* pv, const void* pi) {
-    a = reinterpret_cast<const double2*>(pv)[0]; b = reinterpret_cast<const double2*>(pv)[1]; k = *reinterpret_cast<const uint2*>(pi);
-  }
 };
 __device__ __forceinline__ unsigned int off_of(const uint2& k, int e) {
   return e == 0 ? (k.x & 0xffffu) : e == 1 ? (k.x >> 16) : e == 2 ? (k.y & 0xffffu) : (k.y >> 16);
@@ -568,7 +500,7 @@ __device__ __forceinline__ unsigned long long sparse_item_cost(const unsigned in
 }
 
 __global__ void sparse_partition_kernel(const unsigned int* itemptr, int rows_pad, int nseg, int G, unsigned int* cta_first,
-                                        unsigned int* cta_chunk, unsigned int item_cost) {
+                                        unsigned int item_cost) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > G) return;
   const int NI = rows_pad >> 2;
@@ -582,30 +514,6 @@ __global__ void sparse_partition_kernel(const unsigned int* itemptr, int rows_pa
   }
   if (b == G) lo = N;
   cta_first[b] = lo;
-  cta_chunk[b] = (unsigned int)(sparse_item_cost(itemptr, NI, nseg, lo, item_cost) - (unsigned long long)item_cost * lo);
-}
-
-// asks L2 to fetch [p, p + bytes) -- p 16-byte aligned, bytes a non-zero multiple of 16
-__device__ __forceinline__ void l2_prefetch(const void* p, unsigned int bytes) {
-  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" :: "l"(p), "r"(bytes) : "memory");
-}
-
-// Called by every CTA right before it waits on a device-wide barrier of the solver: HBM is idle during the
-// synchronisation and combine steps of an evaluation (a sixth of an evaluation at config 2), so the head of the range
-// this CTA will stream in the NEXT sweep -- the matrix does not depend on the line-search decision -- is pulled
-// into the 50 MB L2 meanwhile; the sweep then starts from L2 while HBM works on the rest.
-template <typename T>
-__device__ __forceinline__ void sparse_prefetch_head(const SparseView& sp) {
-  if (sp.head_chunks == 0u) return;
-  constexpr unsigned int kPiece = 256;  // chunks per request: 4 KB of fp32 values + 2 KB of offsets
-  const unsigned int c0 = sp.cta_chunk[blockIdx.x];
-  const unsigned int c1 = min(sp.cta_chunk[blockIdx.x + 1], c0 + sp.head_chunks);
-  const unsigned int c = c0 + kPiece * threadIdx.x;
-  if (c < c1) {
-    const unsigned int n = min(kPiece, c1 - c);  // multiple of 4
-    l2_prefetch(reinterpret_cast<const T*>(sp.val) + 4ull * c, n * 4u * (unsigned int)sizeof(T));
-    l2_prefetch(sp.off16 + 4ull * c, n * 8u);
-  }
 }
 
 // whole sparse pass of one CTA: same partial layout as matvec_phase (partM/partC [NSEG][rows_pad]).

@@ -574,77 +574,8 @@ def test_screened_scoring_fp32_store(clp, orc, d, mindist, scale, shift):
 
 
 # ------------------------------------------------------------------------------------------
-# resident-vector solver: every load pipeline of its sweep (register rounds and cp.async.bulk rings), the size limit
+# resident-vector solver: the size limit (its two layouts: tests/test_gpu_packed.py)
 # ------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("m", [3000, 9000])
-def test_resident_load_pipelines_agree(clp, orc, m):
-    """CLP_RES_CFG selects how the resident sweep streams the compact copy: register pipelines (0, 1, 2) or per-warp
-    shared-memory rings filled by cp.async.bulk with mbarrier completion (3 .. 6).  Same arithmetic, same grouping of
-    the sums per row -> identical decisions; every one must match the oracle."""
-    import os
-    from clipper_b200 import datagen
-    prob = datagen.config_problem("c2", m); cfg = prob["cfg"]
-    o = orc.Oracle(); o.score_euclidean(prob["D1"], prob["D2"], prob["A"], sigma=cfg["sigma"], epsilon=cfg["epsilon"])
-    so = o.solve(prob["u0"])
-    v = np.random.default_rng(m).random(m)
-    ref = None
-    old = os.environ.get("CLP_RES_CFG")
-    try:
-        for cfgid in range(7):
-            os.environ["CLP_RES_CFG"] = str(cfgid)   # read when the handle is created
-            c = make_euclid(clp, sigma=cfg["sigma"], epsilon=cfg["epsilon"])
-            c.score_pairwise_consistency(prob["D1"], prob["D2"], prob["A"])
-            assert c.dense_mode() == 6
-            y, Mv, Cv = c.matvec(v, 0.6)
-            c.solve(prob["u0"]); s = c.get_solution()
-            assert sorted(s.nodes) == sorted(so.nodes.tolist())
-            assert abs(s.score - so.score) <= 1e-5 * abs(so.score)
-            if ref is None:
-                ref = (Mv, Cv, s)
-            else:
-                assert np.abs(Mv - ref[0]).max() <= 1e-12 * max(1.0, np.abs(ref[0]).max())
-                assert np.array_equal(Cv, ref[1]) or np.abs(Cv - ref[1]).max() <= 1e-12 * max(1.0, np.abs(ref[1]).max())
-                assert s.nodes == ref[2].nodes and s.n_evals == ref[2].n_evals and s.ifinal == ref[2].ifinal
-                assert abs(s.score - ref[2].score) <= 2e-11 * abs(ref[2].score)
-    finally:
-        if old is None:
-            os.environ.pop("CLP_RES_CFG", None)
-        else:
-            os.environ["CLP_RES_CFG"] = old
-
-
-@pytest.mark.parametrize("m", [3001])
-def test_resident_staging_paths_agree(clp, orc, m):
-    """CLP_STAGE_BULK=1 (default): the candidate enters shared memory as it is through cp.async.bulk and 1/|w| is applied
-    to the row results; 0: register loads, every entry normalised by every CTA.  Same inlier set as the oracle either
-    way, objective equal to rounding.  Odd m: the last entry takes the
-    scalar path beside the 16-byte-granular bulk copies."""
-    import os
-    from clipper_b200 import datagen
-    prob = datagen.config_problem("c2", m); cfg = prob["cfg"]
-    o = orc.Oracle(); o.score_euclidean(prob["D1"], prob["D2"], prob["A"], sigma=cfg["sigma"], epsilon=cfg["epsilon"])
-    so = o.solve(prob["u0"])
-    got = []
-    old = os.environ.get("CLP_STAGE_BULK")
-    try:
-        for flag in ("1", "0"):
-            os.environ["CLP_STAGE_BULK"] = flag   # read when the handle is created
-            c = make_euclid(clp, sigma=cfg["sigma"], epsilon=cfg["epsilon"])
-            c.score_pairwise_consistency(prob["D1"], prob["D2"], prob["A"])
-            assert c.dense_mode() == 6
-            c.solve(prob["u0"]); s = c.get_solution()
-            assert sorted(s.nodes) == sorted(so.nodes.tolist())
-            assert abs(s.score - so.score) <= 1e-5 * abs(so.score)
-            got.append(s)
-    finally:
-        if old is None:
-            os.environ.pop("CLP_STAGE_BULK", None)
-        else:
-            os.environ["CLP_STAGE_BULK"] = old
-    assert got[0].nodes == got[1].nodes
-    assert abs(got[0].score - got[1].score) <= 1e-9 * abs(got[1].score)
-
-
 def test_resident_at_its_size_limit(clp, orc):
     """m = 27 648: the fp64 trial vector takes 221 KB of the 227 KB of shared memory, the on-chip epilogue tables do
     not fit any more (HBM fallback); one column more and the segmented solver takes over."""
