@@ -297,7 +297,7 @@ class CLIPPER:
 
     def set_dense_mode(self, mode):
         """4 (default) auto; 6 compact rows + resident trial vector (m <= 27648); 3 compact rows, column segments;
-        2 upper triangle read once, two-sided update; 1 stripes/full; 0 segments"""
+        2 upper triangle read once, two-sided update; 0 segments; any other value raises ClipperError"""
         _capi.check(self._h, self._lib.clp_set_dense_mode(self._h, int(mode)))
 
     def set_grid_cap(self, n_ctas):
@@ -305,7 +305,7 @@ class CLIPPER:
         _capi.check(self._h, self._lib.clp_set_grid_cap(self._h, int(n_ctas)))
 
     def dense_mode(self):
-        """effective sweep mode of the current problem (sharded handles fall back from 2 to 1)"""
+        """effective sweep mode of the current problem (sharded handles fall back from 2 to 0)"""
         a, b = C.c_int(), C.c_int()
         _capi.check(self._h, self._lib.clp_get_dense_mode(self._h, C.byref(a), C.byref(b)))
         return int(b.value)

@@ -88,21 +88,15 @@ struct clp_handle_s {
   std::vector<int32_t> A_host;  // column-major m x 2
   DevBuf A_dev;                 // int32 [2m]
   DevBuf E1, E2, D1dev, D2dev, F12;  // F12: fp32 positions of both endpoints (screening pass of the scoring kernel)
-  int score_filter = env_int("CLP_SCORE_FILTER", 1);
-  // resident-vector solver (clp_resident.cuh): the default whenever the whole trial vector fits shared memory
-  int res_enabled = env_int("CLP_RESIDENT", 1);
-  int res_smem_extra = env_int("CLP_RES_SMEM_EXTRA", 1);  // 0: launch with the plan's minimum (piece table / row state in HBM)
   int prof_ctas = env_int("CLP_PROF_CTAS", 0);      // print the per-CTA phase times of every resident solve (stderr)
   int prof_host = env_int("CLP_PROF_HOST", 0);      // print wall-clock marks of the scoring / solve calls (stderr)
   int prof_laps = env_int("CLP_PROF_LAPS", 1);      // in-kernel phase timers (the split reported in clp_solution.prof_*)
-  int res_G_env = env_int("CLP_RES_G", 0);          // > 0: CTAs of the resident kernels (A/B runs)
-  int item_cost = env_int("CLP_ITEM_COST", (int)kItemCost);  // fixed cost of an item in the partition of the sweep (A/B runs)
   DevBuf prof_buf;
+  // resident-vector solver (clp_resident.cuh): the default whenever the whole trial vector fits shared memory
   int res_G = 0;                                    // CTAs of the resident kernels for the current matrix
   int res_NI = 0;
   bool compact_resident = false;                    // layout of the current compact copy: full rows + column indices
   int smem_optin = 0;                               // cudaDevAttrMaxSharedMemoryPerBlockOptin
-  int fuse_count = env_int("CLP_FUSE_COUNT", 1);  // scoring kernel counts the kept entries (skips sparse_count_kernel)
   bool score_pending = false;                       // a scoring launch's error flag has not been read back yet
   bool counts_fused = false;                        // sp_ptr4 already holds the counts of the current matrix
   long long counts_m = 0; int counts_rows_pad = 0, counts_nseg = 0, counts_W = 0;  // ... which was this one
@@ -126,7 +120,7 @@ struct clp_handle_s {
   Plan plan{};
   long long mpad = 0;
   // stripe decomposition (clp_dense2.cuh)
-  int dense_mode = 4;     // requested: 0 segments, 1 stripes/full, 2 stripes/upper-triangle two-sided,
+  int dense_mode = 4;     // requested: 0 segments, 2 stripes/upper-triangle two-sided (one GPU),
                           //            3 compact rows (segmented), 6 compact rows + resident vector,
                           //            4 auto (6 if the vector fits shared memory, else 3, when the graph is sparse enough; else 2 / 0)
   int dense_mode_eff = 2; // effective, decided when the matrix is finalised
@@ -209,17 +203,16 @@ Plan make_plan(long long m, int rows_pad, int G) {
   return p;
 }
 
-// stripe decomposition: item enumeration, per-CTA runs, buffers (clp_dense2.cuh)
+// stripe decomposition of the upper triangle: item enumeration, per-CTA runs, buffers (clp_dense2.cuh)
 int build_plan2(clp_handle h) {
   const int G = h->plan.G;
   Plan2& p = h->plan2;
   p.G = G;
-  p.sym = h->dense_mode_eff == 2 ? 1 : 0;
   p.NST = (int)((h->m + kStripe - 1) / kStripe);
   p.NRT = h->rows_pad / kRowTile;
   std::vector<long long> prefix((size_t)p.NST + 1, 0);
-  for (int J = 0; J < p.NST; ++J) {
-    const long long nt = p.sym ? std::min<long long>(p.NRT, (long long)(J + 1) * (kStripe / kRowTile)) : p.NRT;
+  for (int J = 0; J < p.NST; ++J) {  // stripe J holds the row tiles up to its diagonal block
+    const long long nt = std::min<long long>(p.NRT, (long long)(J + 1) * (kStripe / kRowTile));
     prefix[(size_t)J + 1] = prefix[(size_t)J] + nt;
   }
   p.T = prefix[(size_t)p.NST];
@@ -241,13 +234,12 @@ int build_plan2(clp_handle h) {
     kmax = std::max(kmax, k);
   }
   p.KMAX = kmax;
-  // symmetric mode: per stripe, the ordered list of column-partial slots (one per CTA run crossing the stripe)
+  // per stripe, the ordered list of column-partial slots (one per CTA run crossing the stripe)
   std::vector<int> slot_begin((size_t)p.NST + 1, 0), slot_list;
   for (int J = 0; J < p.NST; ++J) {
     slot_begin[(size_t)J] = (int)slot_list.size();
-    if (p.sym)
-      for (int b = lo[(size_t)J]; b <= hi[(size_t)J]; ++b)
-        if (has[(size_t)b]) slot_list.push_back(b * kmax + (J - first[(size_t)b]));
+    for (int b = lo[(size_t)J]; b <= hi[(size_t)J]; ++b)
+      if (has[(size_t)b]) slot_list.push_back(b * kmax + (J - first[(size_t)b]));
   }
   slot_begin[(size_t)p.NST] = (int)slot_list.size();
   // device copies of the small integer tables
@@ -274,7 +266,7 @@ int build_plan2(clp_handle h) {
   p.slot_list = p.slot_begin + p.NST + 1;
   // partial-product buffers
   const size_t n_row = (size_t)p.NST * h->rows_pad;
-  const size_t n_col = p.sym ? (size_t)G * p.KMAX * kStripe : 0;
+  const size_t n_col = (size_t)G * p.KMAX * kStripe;
   CLP_CUDA(h, h->d2buf.ensure((2 * n_row + 2 * n_col + (size_t)G) * sizeof(double) + 64));
   double* d = h->d2buf.as<double>();
   h->d2.rowM = d; h->d2.rowC = d + n_row;
@@ -307,7 +299,7 @@ int res_warps(clp_handle h) {
 // all 227 KB leaves no L1 for the streaming sweep.
 void res_pick_caps(clp_handle h, unsigned int* pieces_cap, unsigned int* state_cap) {
   *pieces_cap = 0; *state_cap = 0;
-  if (!h->res_smem_extra || h->res_G < 1) return;
+  if (h->res_G < 1) return;
   const int NW = res_warps(h);
   const unsigned int items = (unsigned int)((h->res_NI + h->res_G - 1) / h->res_G);
   // the partition is balanced by bytes, so CTAs holding short rows hold more items than the mean: 2x the mean + slack
@@ -328,7 +320,7 @@ unsigned int res_launch_smem(clp_handle h) {
 
 // can the resident solver take a problem of this size on this handle?
 bool resident_possible(clp_handle h, long long m) {
-  if (!h->res_enabled || m > kResMaxM || m > 65535) return false;
+  if (m > kResMaxM || m > 65535) return false;
   if (!(h->dense_mode == 4 || h->dense_mode == 6)) return false;
   return (long long)res_smem_plan((int)m, kResThreads / 32).total <= (long long)h->smem_optin;
 }
@@ -500,7 +492,6 @@ int build_sparse(clp_handle h, bool force, bool resident) {
     const long long by_bytes = (long long)((double)h->sp_nnz * h->entry_bytes() / (32.0 * 1024.0));
     G = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(h->grid_cap > 0 ? std::min(h->grid_cap, h->sm_count) : h->sm_count, NI / 2),
                                                         std::max<long long>(1, by_bytes)));
-    if (h->res_G_env > 0) G = std::max(1, std::min(h->res_G_env, std::min(h->sm_count, std::max(1, NI / 2))));
     h->res_G = G;
     CLP_CUDA(h, res_set_attrs<T>(h));
     const int NW = res_warps(h);
@@ -510,8 +501,7 @@ int build_sparse(clp_handle h, bool force, bool resident) {
     CLP_CUDA(h, h->res_redll.ensure((size_t)2 * G * kRedVals * sizeof(uint4)));
   }
   CLP_CUDA(h, h->sp_part.ensure(((size_t)G + 1) * sizeof(unsigned int)));
-  sparse_partition_kernel<<<(G + 1 + 255) / 256, 256, 0, h->stream>>>(h->sp.itemptr, h->rows_pad, nseg, G, h->sp_part.as<unsigned int>(),
-                                                                      (unsigned int)std::max(0, h->item_cost));
+  sparse_partition_kernel<<<(G + 1 + 255) / 256, 256, 0, h->stream>>>(h->sp.itemptr, h->rows_pad, nseg, G, h->sp_part.as<unsigned int>());
   CLP_CUDA(h, cudaGetLastError());
   h->sp.cta_first = h->sp_part.as<unsigned int>();
   if (h->sp.packed) {  // where every warp of the resident kernels starts: once per build, not per sweep
@@ -552,10 +542,10 @@ int finalize_matrix_impl(clp_handle h) {
     else if (rc == kKeepDense) eff = (h->world > 1) ? 0 : 2;
     else return rc;
   }
-  if (eff == 2 && h->world > 1) eff = 1;
+  if (eff == 2 && h->world > 1) eff = 0;  // a shard holds row blocks, not the whole upper triangle
   if (eff != 3 && eff != 6) { if (int rc = set_plan_for(h, eff)) return rc; }
   h->dense_mode_eff = eff;
-  if (eff == 1 || eff == 2) { if (int rc = build_plan2(h)) return rc; }
+  if (eff == 2) { if (int rc = build_plan2(h)) return rc; }
   return CLP_OK;
 }
 
@@ -610,20 +600,22 @@ int read_sync(clp_handle h, SyncBlock* sb) {
   return CLP_OK;
 }
 
+// fp32 storage and (PointNormal, or Euclidean with d = 2 or 3): the scoring kernel screens every pair in fp32 first
+// and also counts the kept entries (first pass of the compact build); every other case runs the plain kernel.  The
+// screened kernel's shared-memory block is sized for fp32 storage.
+bool screened_scoring(clp_handle h, int kind, int d) {
+  return h->storage == CLP_STORE_F32 && (kind == 1 || d == 2 || d == 3);
+}
+
 template <typename T, bool MIRROR>
 int launch_score_m(clp_handle h, int kind, int d, const ScoreArgs& a) {
   dim3 grid((unsigned)(h->ld / 128), (unsigned)(h->rows_pad / kRowTile));
-  if constexpr (sizeof(T) == 4) {  // the screened kernel's shared-memory block is sized for fp32 storage
-   if (h->score_filter) {
-    if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
+  if constexpr (sizeof(T) == 4) {
+    if (!screened_scoring(h, kind, d)) score_tile_kernel<T, 0, 0, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
+    else if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
     else if (d == 3) score_tile_kernel<T, 0, 3, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
-    else if (d == 2) score_tile_kernel<T, 0, 2, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
-    else score_tile_kernel<T, 0, 0, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
-    CLP_CUDA(h, cudaGetLastError());
-    return CLP_OK;
-   }
-  }
-  {
+    else score_tile_kernel<T, 0, 2, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
+  } else {
     if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
     else if (d == 3) score_tile_kernel<T, 0, 3, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
     else if (d == 2) score_tile_kernel<T, 0, 2, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
@@ -662,8 +654,8 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   const int cnt_nseg = res_layout ? 1 : h->plan.NSEG, cnt_W = res_layout ? (int)h->ld : h->plan.W;
   a.cnt = nullptr; a.W = cnt_W; a.win = nullptr; a.wwords = 0; a.expo = nullptr;
   h->counts_fused = false;
-  if (h->score_filter && h->fuse_count && h->storage == CLP_STORE_F32 && (kind == 1 || d == 2 || d == 3) &&
-      (h->dense_mode == 3 || h->dense_mode == 4 || h->dense_mode == 6)) {
+  const bool compact_next = (h->dense_mode == 3 || h->dense_mode == 4 || h->dense_mode == 6);
+  if (compact_next && screened_scoring(h, kind, d)) {
     // the screened scoring kernel also counts the kept entries per (segment, row): first pass of the compact build
     const size_t nptr = (size_t)cnt_nseg * (h->rows_pad + 1);
     CLP_CUDA(h, h->sp_ptr4.ensure(nptr * sizeof(unsigned int)));
@@ -679,7 +671,6 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   a.d = d; a.p0 = p0; a.p1 = p1; a.p2 = p2; a.p3 = p3; a.affinityeps = h->prm.affinityeps;
   int rc = (h->storage == CLP_STORE_F64) ? launch_score<double>(h, kind, d, a) : launch_score<float>(h, kind, d, a);
   if (rc) return rc;
-  const bool compact_next = (h->dense_mode == 3 || h->dense_mode == 4 || h->dense_mode == 6);
   if (!compact_next) {  // dense sweeps: nothing else synchronises with the scoring launch
     SyncBlock host;
     if ((rc = read_sync(h, &host))) return rc;
@@ -769,8 +760,7 @@ int launch_matvec(clp_handle h, const StageArgs& st, const double* v, double d, 
     CLP_CUDA(h, cudaGetLastError());
     matvec_combine_kernel<<<cb, 256, 0, h->stream>>>(mat_view(h), p, partM, partC, h->small.as<double>(), v, d, y, Mv, Cv);
   } else {
-    if (h->dense_mode_eff == 2) matvec2_partials_kernel<T, true><<<h->plan2.G, kThreads, 0, h->stream>>>(mat_view(h), h->plan2, st, h->d2);
-    else matvec2_partials_kernel<T, false><<<h->plan2.G, kThreads, 0, h->stream>>>(mat_view(h), h->plan2, st, h->d2);
+    matvec2_partials_kernel<T><<<h->plan2.G, kThreads, 0, h->stream>>>(mat_view(h), h->plan2, st, h->d2);
     CLP_CUDA(h, cudaGetLastError());
     matvec2_combine_kernel<<<cb, 256, 0, h->stream>>>(mat_view(h), h->plan2, h->d2, v, d, y, Mv, Cv);
   }
@@ -791,8 +781,7 @@ template <typename T>
 cudaError_t launch_solver(clp_handle h, SolverArgs& a) {
   void* args[] = {&a};
   const void* fn = h->dense_mode_eff == 3 ? (const void*)solver_kernel<T, 3>
-                 : h->dense_mode_eff == 2 ? (const void*)solver_kernel<T, 2>
-                 : h->dense_mode_eff == 1 ? (const void*)solver_kernel<T, 1> : (const void*)solver_kernel<T, 0>;
+                 : h->dense_mode_eff == 2 ? (const void*)solver_kernel<T, 2> : (const void*)solver_kernel<T, 0>;
   return cudaLaunchCooperativeKernel(fn, dim3(h->plan.G), dim3(kThreads), args, 0, h->stream);
 }
 
@@ -983,19 +972,17 @@ int clp_create(int device, int storage, clp_handle* out) {
   if ((e = h->sync.ensure(sizeof(SyncBlock))) != cudaSuccess) return bail("cudaMalloc", e);
   int occ = 0, occ3 = 0;
   {
-    int o0 = 0, o1 = 0, o2 = 0;
+    int o0 = 0, o2 = 0;
     if (storage == CLP_STORE_F64) {
       e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o0, solver_kernel<double, 0>, kThreads, 0);
-      if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o1, solver_kernel<double, 1>, kThreads, 0);
       if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o2, solver_kernel<double, 2>, kThreads, 0);
       if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ3, solver_kernel<double, 3>, kThreads, 0);
     } else {
       e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o0, solver_kernel<float, 0>, kThreads, 0);
-      if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o1, solver_kernel<float, 1>, kThreads, 0);
       if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o2, solver_kernel<float, 2>, kThreads, 0);
       if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ3, solver_kernel<float, 3>, kThreads, 0);
     }
-    occ = std::min(o0, std::min(o1, o2));
+    occ = std::min(o0, o2);
   }
   if (e != cudaSuccess || occ < 1 || occ3 < 1) return bail("occupancy query (is the sm_90a image loadable?)", e);
   h->ctas_per_sm = std::min(occ, 2);
@@ -1419,7 +1406,7 @@ int clp_get_dense_mode(clp_handle h, int* requested, int* effective) {
 }
 
 int clp_set_dense_mode(clp_handle h, int mode) {
-  if (!h || mode < 0 || mode > 6 || mode == 5) return fail(h, CLP_ERR_INVALID, "sweep mode must be 0..4 or 6");
+  if (!h || mode < 0 || mode > 6 || mode == 1 || mode == 5) return fail(h, CLP_ERR_INVALID, "sweep mode must be 0, 2, 3, 4 or 6");
   h->dense_mode = mode;
   if (h->has_matrix) {
     CLP_CUDA(h, cudaSetDevice(h->device));

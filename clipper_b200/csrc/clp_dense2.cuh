@@ -8,8 +8,8 @@
 //   * the lane's 8 entries of v stay in REGISTERS for the whole run (no shared-memory staging of v);
 //   * row sums: per 4-row chunk each warp reduces its 8 partial sums with a halving butterfly
 //     (18 SHFL), the 8 warps of the CTA are added through 4 KB of shared memory once per 32-row tile;
-//   * SYMMETRIC mode (single GPU): only tiles of the UPPER triangle are read.  Every element
-//     s = M_ij (i<j) is applied twice in-tile:  y_i += |s| v_j  (row sum, as before) and
+//   * only tiles of the UPPER triangle are read (single GPU: the store holds the whole symmetric matrix).
+//     Every element s = M_ij (i<j) is applied twice in-tile:  y_i += |s| v_j  (row sum) and
 //     y_j += |s| v_i  (column sum, 16 register accumulators per lane that live across the whole run).
 //     HBM traffic per objective evaluation drops from 4 m^2 to ~2 m^2 bytes (fp32 storage).
 //     Inside the diagonal 2048 x 2048 block the strict-upper mask c > r is applied per element and
@@ -28,7 +28,6 @@ constexpr int kMaxStripes = 128; // m <= 262144
 struct Plan2 {
   int G;        // CTAs
   int NST;      // stripes
-  int sym;      // 1: upper triangle only, two-sided update
   int KMAX;     // max number of stripes one CTA's run touches (column-partial slots per CTA)
   int NRT;      // local 32-row tiles
   long long T;  // total items
@@ -37,14 +36,14 @@ struct Plan2 {
   const int* stripe_cta_lo;      // [NST] first / last CTA whose run intersects stripe J
   const int* stripe_cta_hi;
   const int* cta_has_items;      // [G] 0 for CTAs without items (problems with fewer items than CTAs)
-  const int* slot_begin;         // [NST+1] symmetric mode: range in slot_list of the column-partial slots of stripe J
+  const int* slot_begin;         // [NST+1] range in slot_list of the column-partial slots of stripe J
   const int* slot_list;          // slot = cta * KMAX + (J - first stripe of cta), in CTA order
 };
 
 struct Dense2Buffers {
   double* rowM;   // [NST][rows_pad]  row-type partial products  (M and C)
   double* rowC;
-  double* colM;   // [G*KMAX][kStripe] column-type partial products (symmetric mode)
+  double* colM;   // [G*KMAX][kStripe] column-type partial products
   double* colC;
   double* sumpart;  // [G] per-CTA partial sums of the staged vector
 };
@@ -93,7 +92,7 @@ template <> struct Elem4<double> {
   __device__ __forceinline__ double get(int e) const { return e == 0 ? a.x : e == 1 ? a.y : e == 2 ? b.x : b.y; }
 };
 
-// one stored element applied to the row sums (and, symmetric mode, to the column sums).  The C bit is
+// one stored element applied to the row sums (and, SYM, to the column sums).  The C bit is
 // turned into the double 1.0 / 0.0 with two integer instructions ({~(bits>>31) & 0x3ff00000, 0}) and the
 // constraint sums are plain FMAs -- ptxas turns predicated fp64 adds into DADD + 2 FSEL, which costs more.
 __device__ __forceinline__ double cbit_as_double(int hibits) {
@@ -125,7 +124,7 @@ __device__ __forceinline__ float neutral_if(bool kill, float x) { return kill ? 
 __device__ __forceinline__ double neutral_if(bool kill, double x) { return kill ? -0.0 : x; }
 
 // 4 rows x 4 columns of one lane (one 128-column step): apply to the row and column accumulators
-template <typename T, bool SYM, bool DIAG>
+template <typename T, bool DIAG>
 __device__ __forceinline__ void dense2_apply(const Elem4<T> (&a)[4], const double (&vc)[4], const double (&vr)[4],
                                              int gi, int cfirst, double (&acc)[8], double (&colM)[4], double (&colC)[4]) {
 #pragma unroll
@@ -134,13 +133,13 @@ __device__ __forceinline__ void dense2_apply(const Elem4<T> (&a)[4], const doubl
     for (int e = 0; e < 4; ++e) {
       auto x = a[r].get(e);
       if (DIAG) x = neutral_if((cfirst + e) <= (gi + r), x);  // keep the strict upper part only
-      apply_elem<SYM>(x, vc[e], vr[r], acc[r], acc[4 + r], colM[e], colC[e]);
+      apply_elem<true>(x, vc[e], vr[r], acc[r], acc[4 + r], colM[e], colC[e]);
     }
 }
 
 // One 32-row tile for one warp: 8 chunks of 4 rows x 256 columns, software-pipelined at the granularity of
 // one 128-column step (the loads of the next step are in flight while the current one is consumed).
-template <typename T, bool SYM, bool DIAG>
+template <typename T, bool DIAG>
 __device__ __forceinline__ void dense2_tile(const T* prow, long long ld, bool ok1, int qend, const double (&vc)[2][4],
                                             const double* vr_tile, int gi0, int c0, double (&colM)[2][4],
                                             double (&colC)[2][4], double* rowpart_warp) {
@@ -159,20 +158,18 @@ __device__ __forceinline__ void dense2_tile(const T* prow, long long ld, bool ok
       if (ok1) B[r].load(p + (size_t)r * ld + 128);
       else B[r].neutral();
     }
-    double vr[4] = {0.0, 0.0, 0.0, 0.0};
-    if (SYM) {
+    double vr[4];
 #pragma unroll
-      for (int r = 0; r < 4; ++r) vr[r] = vr_tile[4 * q + r];
-    }
+    for (int r = 0; r < 4; ++r) vr[r] = vr_tile[4 * q + r];
     double acc[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) acc[i] = 0.0;
-    dense2_apply<T, SYM, DIAG>(A, vc[0], vr, gi, c0, acc, colM[0], colC[0]);
+    dense2_apply<T, DIAG>(A, vc[0], vr, gi, c0, acc, colM[0], colC[0]);
     if (q + 1 < qend) {
 #pragma unroll
       for (int r = 0; r < 4; ++r) A[r].load(p + (size_t)(4 + r) * ld);
     }
-    dense2_apply<T, SYM, DIAG>(B, vc[1], vr, gi, c0 + 128, acc, colM[1], colC[1]);
+    dense2_apply<T, DIAG>(B, vc[1], vr, gi, c0 + 128, acc, colM[1], colC[1]);
     const double tot = warp_reduce8(acc);
     if ((lane & 3) == 0) {
       const int qv = lane >> 2;  // 0..3: M of row qv, 4..7: C of row qv-4
@@ -186,7 +183,7 @@ __device__ __forceinline__ void dense2_tile(const T* prow, long long ld, bool ok
 
 // One run of row tiles [rt_a, rt_b) inside stripe J.
 // smem: rowpart[2][8 warps][32 rows][2] + vr[2][32] doubles (double-buffered: one CTA sync per tile).
-template <typename T, bool SYM>
+template <typename T>
 __device__ void dense2_run(const MatView& mv, const StageArgs& st, double nrm, int J, int rt_a, int rt_b,
                            const Dense2Buffers& buf, size_t col_slot, double* smem) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -216,7 +213,7 @@ __device__ void dense2_run(const MatView& mv, const StageArgs& st, double nrm, i
 
   // entries of the staged vector for the 32 rows of a tile (the column sums need v_row)
   auto stage_rows = [&](int rt, int bufi) {
-    if (SYM && threadIdx.x < kRowTile) {
+    if (threadIdx.x < kRowTile) {
       const int g = mv.row0 + rt * kRowTile + threadIdx.x;
       vr_s[bufi * kRowTile + threadIdx.x] = (g < mv.m) ? staged_value(st, g, nrm) : 0.0;
     }
@@ -229,7 +226,7 @@ __device__ void dense2_run(const MatView& mv, const StageArgs& st, double nrm, i
     if (rt + 1 < rt_b) stage_rows(rt + 1, pb ^ 1);  // for the next tile; published by this tile's sync
     const int lr0 = rt * kRowTile;          // local row of the tile
     const int gi0 = mv.row0 + lr0;          // global row
-    const bool diag = SYM && (gi0 >= J * kStripe);  // tile lies inside the diagonal block of the stripe
+    const bool diag = gi0 >= J * kStripe;   // tile lies inside the diagonal block of the stripe
     // number of 4-row chunks that can hold a strict-upper element (c > r) for this warp's columns
     int qend = has_cols ? kRowTile / 4 : 0;
     if (diag && has_cols) {
@@ -238,8 +235,8 @@ __device__ void dense2_run(const MatView& mv, const StageArgs& st, double nrm, i
     }
     const T* prow = Mbase + (size_t)lr0 * ld + c0;
     double* rp = rowpart + (size_t)(pb * kWarps + warp) * kRowTile * 2;
-    if (diag) dense2_tile<T, SYM, true>(prow, ld, ok1, qend, vc, vr_s + pb * kRowTile, gi0, c0, colM, colC, rp);
-    else dense2_tile<T, SYM, false>(prow, ld, ok1, qend, vc, vr_s + pb * kRowTile, gi0, c0, colM, colC, rp);
+    if (diag) dense2_tile<T, true>(prow, ld, ok1, qend, vc, vr_s + pb * kRowTile, gi0, c0, colM, colC, rp);
+    else dense2_tile<T, false>(prow, ld, ok1, qend, vc, vr_s + pb * kRowTile, gi0, c0, colM, colC, rp);
     __syncthreads();
     if (threadIdx.x < 2 * kRowTile) {  // add the 8 warps in order, publish the row-type partials of this tile
       const int row = threadIdx.x >> 1, which = threadIdx.x & 1;
@@ -251,19 +248,18 @@ __device__ void dense2_run(const MatView& mv, const StageArgs& st, double nrm, i
     }
   }
   __syncthreads();  // the next run (or phase) reuses the buffers
-  if (SYM) {  // column-type partials of the whole run
+  // column-type partials of the whole run
 #pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      const size_t off = col_slot * kStripe + warp * kWarpCols + s * 128 + lane * 4;
-      *reinterpret_cast<double4*>(buf.colM + off) = make_double4(colM[s][0], colM[s][1], colM[s][2], colM[s][3]);
-      *reinterpret_cast<double4*>(buf.colC + off) = make_double4(colC[s][0], colC[s][1], colC[s][2], colC[s][3]);
-    }
+  for (int s = 0; s < 2; ++s) {
+    const size_t off = col_slot * kStripe + warp * kWarpCols + s * 128 + lane * 4;
+    *reinterpret_cast<double4*>(buf.colM + off) = make_double4(colM[s][0], colM[s][1], colM[s][2], colM[s][3]);
+    *reinterpret_cast<double4*>(buf.colC + off) = make_double4(colC[s][0], colC[s][1], colC[s][2], colC[s][3]);
   }
 }
 
 // whole dense pass of one CTA: (1) its slice of the staged vector -> st.dst and the partial sum,
 // (2) its contiguous share of the (stripe, row tile) items
-template <typename T, bool SYM>
+template <typename T>
 __device__ __forceinline__ void dense2_phase(const MatView& mv, const Plan2& p, const StageArgs& st, const Dense2Buffers& buf,
                              double* smem) {
   const double nrm = sqrt(st.z);
@@ -296,40 +292,38 @@ __device__ __forceinline__ void dense2_phase(const MatView& mv, const Plan2& p, 
   while (t < t1) {
     const long long sbeg = p.tile_prefix[J], send = p.tile_prefix[J + 1];
     const long long tend = t1 < send ? t1 : send;
-    dense2_run<T, SYM>(mv, st, nrm, J, (int)(t - sbeg), (int)(tend - sbeg), buf,
+    dense2_run<T>(mv, st, nrm, J, (int)(t - sbeg), (int)(tend - sbeg), buf,
                        (size_t)blockIdx.x * p.KMAX + k, smem);
     t = tend; ++J; ++k;
   }
 }
 
-// Mhat v, Chat v of local row lr: row-type partials of every stripe that holds the row, then (symmetric)
-// the column-type partials of every CTA run that crossed the row's own stripe -- always in the same order
+// Mhat v, Chat v of local row lr: row-type partials of every stripe that holds the row, then the column-type
+// partials of every CTA run that crossed the row's own stripe -- always in the same order
 __device__ __forceinline__ void dense2_gather(const MatView& mv, const Plan2& p, const Dense2Buffers& buf, int lr,
                                               double& Mv, double& Cv) {
   const int i = mv.row0 + lr;
   const int Ji = i / kStripe;
   double a = 0.0, c = 0.0;
-  for (int J = p.sym ? Ji : 0; J < p.NST; ++J) {
+  for (int J = Ji; J < p.NST; ++J) {
     a += buf.rowM[(size_t)J * mv.rows_pad + lr];
     c += buf.rowC[(size_t)J * mv.rows_pad + lr];
   }
-  if (p.sym) {
-    const int s0 = p.slot_begin[Ji], s1 = p.slot_begin[Ji + 1];
-    const size_t col = (size_t)(i - Ji * kStripe);
-    int t = s0;
-    for (; t + 4 <= s1; t += 4) {  // independent loads in batches of 4, added in list order
-      const size_t o0 = (size_t)p.slot_list[t] * kStripe + col, o1 = (size_t)p.slot_list[t + 1] * kStripe + col;
-      const size_t o2 = (size_t)p.slot_list[t + 2] * kStripe + col, o3 = (size_t)p.slot_list[t + 3] * kStripe + col;
-      const double m0 = buf.colM[o0], m1 = buf.colM[o1], m2 = buf.colM[o2], m3 = buf.colM[o3];
-      const double c0 = buf.colC[o0], c1 = buf.colC[o1], c2 = buf.colC[o2], c3 = buf.colC[o3];
-      a += m0; a += m1; a += m2; a += m3;
-      c += c0; c += c1; c += c2; c += c3;
-    }
-    for (; t < s1; ++t) {
-      const size_t o = (size_t)p.slot_list[t] * kStripe + col;
-      a += buf.colM[o];
-      c += buf.colC[o];
-    }
+  const int s0 = p.slot_begin[Ji], s1 = p.slot_begin[Ji + 1];
+  const size_t col = (size_t)(i - Ji * kStripe);
+  int t = s0;
+  for (; t + 4 <= s1; t += 4) {  // independent loads in batches of 4, added in list order
+    const size_t o0 = (size_t)p.slot_list[t] * kStripe + col, o1 = (size_t)p.slot_list[t + 1] * kStripe + col;
+    const size_t o2 = (size_t)p.slot_list[t + 2] * kStripe + col, o3 = (size_t)p.slot_list[t + 3] * kStripe + col;
+    const double m0 = buf.colM[o0], m1 = buf.colM[o1], m2 = buf.colM[o2], m3 = buf.colM[o3];
+    const double c0 = buf.colC[o0], c1 = buf.colC[o1], c2 = buf.colC[o2], c3 = buf.colC[o3];
+    a += m0; a += m1; a += m2; a += m3;
+    c += c0; c += c1; c += c2; c += c3;
+  }
+  for (; t < s1; ++t) {
+    const size_t o = (size_t)p.slot_list[t] * kStripe + col;
+    a += buf.colM[o];
+    c += buf.colC[o];
   }
   Mv = a; Cv = c;
 }

@@ -888,15 +888,15 @@ __global__ void __launch_bounds__(kThreads, 3)
 matvec_sparse_partials_kernel(MatView mv, Plan p, StageArgs st, SparseView sp, double* partM, double* partC) {
   __shared__ __align__(16) double vs[kSegMax + 2];
   __shared__ double red_smem[kWarps];
-  sparse_phase<T, false>(mv, p, st, sp, partM, partC, vs, red_smem);
+  sparse_phase<T>(mv, p, st, sp, partM, partC, vs, red_smem);
 }
 
 // the same two steps for the stripe decomposition (clp_dense2.cuh)
-template <typename T, bool SYM>
+template <typename T>
 __global__ void __launch_bounds__(kThreads, 2)
 matvec2_partials_kernel(MatView mv, Plan2 p, StageArgs st, Dense2Buffers buf) {
   __shared__ __align__(16) double smem[2 * 8 * 32 * 2 + 2 * 32];
-  dense2_phase<T, SYM>(mv, p, st, buf, smem);
+  dense2_phase<T>(mv, p, st, buf, smem);
 }
 
 __global__ void matvec2_combine_kernel(MatView mv, Plan2 p, Dense2Buffers buf, const double* v, double d, double* y,
@@ -960,7 +960,7 @@ struct SolverArgs {
   double* partC;
   double* segsum;    // [NSEG]
   double* red;       // [2][G][kRedVals]  per-CTA partial sums, double-buffered
-  Plan2 plan2;       // stripe decomposition (MODE 1, 2)
+  Plan2 plan2;       // stripe decomposition (MODE 2)
   Dense2Buffers d2;
   SparseView sp;     // compact rows (MODE 3)
   double* u_final;   // [m] copy of the final iterate
@@ -1085,8 +1085,8 @@ __device__ bool exchange_sums(const SolverArgs& a, const double (&loc)[kRedVals]
   return *reinterpret_cast<volatile int*>(&sb->error) == 0;
 }
 
-// MODE 0: column-segment decomposition (matvec_phase); 1: stripes, full matrix; 2: stripes, upper triangle
-// read once and applied two-sidedly (single GPU); 3: compact rows (clp_sparse.cuh) in the MODE-0 decomposition
+// MODE 0: column-segment decomposition (matvec_phase); 2: stripes, upper triangle read once and applied
+// two-sidedly (single GPU); 3: compact rows (clp_sparse.cuh) in the MODE-0 decomposition
 template <typename T, int MODE>
 __global__ void __launch_bounds__(kThreads, MODE == 3 ? 3 : 2) solver_kernel(SolverArgs a) {
   __shared__ __align__(16) double vs[kSegMax + 2];
@@ -1127,13 +1127,13 @@ __global__ void __launch_bounds__(kThreads, MODE == 3 ? 3 : 2) solver_kernel(Sol
   _Pragma("unroll") for (int q_ = 0; q_ < kRedVals; ++q_) loc[q_] = 0.0;
   // rows are dealt to the CTAs in chunks of 32 consecutive rows, round-robin (chunk c -> CTA c % G):
   // coalesced inside a warp, and every CTA gets rows from all parts of the matrix (the gather cost of a
-  // row grows with its stripe index in the symmetric mode)
+  // row grows with its stripe index in MODE 2)
 #define CLP_FOR_ROWS(lr)                                                                    \
   for (int lr = (blockIdx.x + p.G * (threadIdx.x >> 5)) * 32 + (threadIdx.x & 31); lr < mv.rows; lr += p.G * kWarps * 32)
 #define CLP_DENSE_PASS()                                                                    \
   if constexpr (MODE == 0) matvec_phase<T>(mv, p, st, a.partM, a.partC, vs, red_smem);      \
-  else if constexpr (MODE == 3) sparse_phase<T, false>(mv, p, st, a.sp, a.partM, a.partC, vs, red_smem); \
-  else dense2_phase<T, MODE == 2>(mv, a.plan2, st, a.d2, vs);
+  else if constexpr (MODE == 3) sparse_phase<T>(mv, p, st, a.sp, a.partM, a.partC, vs, red_smem); \
+  else dense2_phase<T>(mv, a.plan2, st, a.d2, vs);
 #define CLP_GATHER()                                                                        \
   if constexpr (MODE == 0 || MODE == 3) gather_partials(a.partM, a.partC, p.NSEG, mv.rows_pad, lr, Mv, Cv); \
   else dense2_gather(mv, a.plan2, a.d2, lr, Mv, Cv);

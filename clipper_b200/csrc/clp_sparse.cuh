@@ -38,8 +38,8 @@ namespace clp {
 constexpr unsigned int kZeroSlot = kSegMax * 8;  // byte offset of the zero element behind the staged segment
 constexpr int kSellUnroll = 3;                   // chunks per lane and round; two rounds are in flight
 constexpr unsigned int kItemCost = 128;          // fixed cost of an item (pointer fetch, pipeline restart, reduction, store) in chunks;
-                                                 // too small a charge leaves the CTAs holding many short items running long
-                                                 // (CLP_ITEM_COST overrides it); irrelevant for the whole-row layout
+                                                 // too small a charge leaves the CTAs holding many short items running long;
+                                                 // irrelevant for the whole-row layout
 
 struct SparseView {
   const void* val;               // T [4 * chunks]
@@ -491,26 +491,24 @@ __device__ __forceinline__ void sell_apply_round(const Entry4<T> (&E)[kSellUnrol
 // (chunks + kItemCost per item), found by bisection on itemptr; inside a CTA the warps draw items from a
 // shared-memory counter.  (Dealing 32-row tiles round-robin, as the dense sweep does, left the slowest CTA
 // with 1.23x the mean bytes at config 2.)
-__device__ __forceinline__ unsigned long long sparse_item_cost(const unsigned int* itemptr, int NI, int nseg, unsigned int g,
-                                                              unsigned int item_cost = kItemCost) {
+__device__ __forceinline__ unsigned long long sparse_item_cost(const unsigned int* itemptr, int NI, int nseg, unsigned int g) {
   const unsigned int seg = g / (unsigned int)NI, it = g - seg * (unsigned int)NI;
   const unsigned int at = (seg >= (unsigned int)nseg) ? itemptr[(size_t)(nseg - 1) * (NI + 1) + NI]
                                                       : itemptr[(size_t)seg * (NI + 1) + it];
-  return (unsigned long long)at + (unsigned long long)item_cost * g;
+  return (unsigned long long)at + (unsigned long long)kItemCost * g;
 }
 
-__global__ void sparse_partition_kernel(const unsigned int* itemptr, int rows_pad, int nseg, int G, unsigned int* cta_first,
-                                        unsigned int item_cost) {
+__global__ void sparse_partition_kernel(const unsigned int* itemptr, int rows_pad, int nseg, int G, unsigned int* cta_first) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b > G) return;
   const int NI = rows_pad >> 2;
   const unsigned int N = (unsigned int)nseg * (unsigned int)NI;
-  const unsigned long long total = sparse_item_cost(itemptr, NI, nseg, N, item_cost);
+  const unsigned long long total = sparse_item_cost(itemptr, NI, nseg, N);
   const unsigned long long target = total * (unsigned long long)b / (unsigned long long)G;  // total < 2^34, b <= G <= 3 CTAs x SMs
   unsigned int lo = 0, hi = N;  // smallest g with cost(g) >= target
   while (lo < hi) {
     const unsigned int mid = lo + ((hi - lo) >> 1);
-    if (sparse_item_cost(itemptr, NI, nseg, mid, item_cost) >= target) hi = mid; else lo = mid + 1;
+    if (sparse_item_cost(itemptr, NI, nseg, mid) >= target) hi = mid; else lo = mid + 1;
   }
   if (b == G) lo = N;
   cta_first[b] = lo;
@@ -521,7 +519,7 @@ __global__ void sparse_partition_kernel(const unsigned int* itemptr, int rows_pa
 // (Tried and dropped: a plain-only instance capped at 64 registers for 4 CTAs/SM -- what the sweep gained, the
 // two synchronisation steps of the evaluation lost again with the larger grid; a bulk L2 prefetch of the next
 // item (cp.async.bulk.prefetch.L2) -- slower.)
-template <typename T, bool PLAIN_ONLY>
+template <typename T>
 __device__ void sparse_phase(const MatView& mv, const Plan& p, const StageArgs& st, const SparseView& sp,
                              double* partM, double* partC, double* vs, double* red_smem) {
   __shared__ int next_item;
@@ -572,7 +570,7 @@ __device__ void sparse_phase(const MatView& mv, const Plan& p, const StageArgs& 
           if (itn >= it1) en = jn - lane;  // no next item: nothing to load
         }
         sell_load_round<T>(sp, Y, jn, en);
-        if (PLAIN_ONLY || sp.plain) sell_apply_round<T, true>(X, vs, aM, aC);
+        if (sp.plain) sell_apply_round<T, true>(X, vs, aM, aC);
         else sell_apply_round<T, false>(X, vs, aM, aC);
         if (last) {
           double accM = aM[0] + aM[1], accC = aC[0] + aC[1];

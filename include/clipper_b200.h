@@ -189,13 +189,14 @@ int clp_set_grid_cap(clp_handle h, int n_ctas);
  *   6: compact copy + RESIDENT trial vector (m <= 27648): the non-neutral entries are packed as (fp32 value, 16-bit
  *     column index) into a sliced-ELL layout over whole rows (rows sorted by length, four at a time, interleaved in
  *     4-entry chunks); every CTA keeps the whole trial vector in shared memory and owns complete rows, so an
- *     objective evaluation needs ONE device-wide synchronisation (clp_resident.cuh); 6 bytes per kept entry;
+ *     objective evaluation needs ONE device-wide synchronisation (clp_resident.cuh); 4 bytes per kept entry (column
+ *     delta + scaled value) for plain fp32 matrices on one GPU whose values span at most 15 binades, else 6 bytes;
  *   3: compact copy cut into column segments of <= 4096 (any m <= 262144): (fp32 value, 16-bit column offset),
  *     same sliced-ELL layout per segment, two device-wide synchronisations per evaluation (SURVEY 8f #3);
  *   2: column stripes, ONLY the upper triangle is read and every element is applied two-sidedly in-tile
- *     -> ~2 m^2 bytes per objective evaluation (fp32 storage), single GPU;
- *   1: column stripes, full matrix (4 m^2 bytes);
- *   0: first-generation column-segment decomposition, full matrix (4 m^2 bytes). */
+ *     -> ~2 m^2 bytes per objective evaluation (fp32 storage), single GPU; a sharded handle runs 0 instead;
+ *   0: column-segment decomposition, full matrix (4 m^2 bytes).
+ * Any other mode (1, 5, ...) is rejected with CLP_ERR_INVALID. */
 int clp_set_dense_mode(clp_handle h, int mode);
 int clp_get_dense_mode(clp_handle h, int* requested, int* effective);
 /* entries kept by the compact copy (all local rows) and the algorithmic bytes one sparse pass reads */

@@ -435,12 +435,12 @@ def test_full_size_c2_properties(clp):
 
 
 # ------------------------------------------------------------------------------------------
-# the three ways of sweeping the dense matrix must agree (and each must match the oracle)
+# every sweep mode must agree with mode 0 (and each must match the oracle)
 # ------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("storage", [0, 1])
 @pytest.mark.parametrize("m", [7, 100, 2047, 2049, 4500, 6200])
-def test_dense_modes_agree(clp, orc, m, storage):
-    """mode 2 reads only the upper triangle (two-sided in-tile update); modes 1 / 0 read the full matrix;
+def test_sweep_modes_agree(clp, orc, m, storage):
+    """mode 2 reads only the upper triangle (two-sided in-tile update); mode 0 reads the full matrix;
     mode 3 sweeps the segmented compact copy, mode 6 the full-row compact copy with the resident trial vector
     (another kernel: one synchronisation per evaluation); 4 picks automatically (= 6 at these sizes).  Sizes straddle
     the 2048-column stripe boundary, the diagonal-block logic and the 128-column segment steps."""
@@ -452,7 +452,7 @@ def test_dense_modes_agree(clp, orc, m, storage):
     rng = np.random.default_rng(m)
     v = rng.random(m)
     res = []
-    modes = (0, 1, 2, 3, 6, 4)
+    modes = (0, 2, 3, 6, 4)
     effective = []
     for mode in modes:
         c = make_euclid(clp, sigma=cfg["sigma"], epsilon=cfg["epsilon"], storage=storage)
@@ -462,7 +462,7 @@ def test_dense_modes_agree(clp, orc, m, storage):
         y, Mv, Cv = c.matvec(v, 0.6)
         c.solve(prob["u0"]); s = c.get_solution()
         res.append((y, Mv, Cv, s))
-    assert effective[:5] == [0, 1, 2, 3, 6] and effective[5] in (2, 6)
+    assert effective[:4] == [0, 2, 3, 6] and effective[4] in (2, 6)
     for k in range(1, len(modes)):
         assert np.abs(res[k][1] - res[0][1]).max() <= 1e-12 * max(1.0, np.abs(res[0][1]).max())
         assert np.abs(res[k][2] - res[0][2]).max() <= 1e-12 * max(1.0, np.abs(res[0][2]).max())
@@ -474,12 +474,19 @@ def test_dense_modes_agree(clp, orc, m, storage):
         # step) and its final objective to well below the solver's own stopping tolerance tol_F = 1e-9
         # (1e-12 held for every case on the round-1 synthetic cloud; on the bunny cloud the m = 4500 case reaches 4e-12
         # between two segmented sweeps: the differences are rounding noise amplified along ~70 evaluations)
-        same_kernel = effective[k] in (0, 1, 2, 3)
+        same_kernel = effective[k] in (0, 2, 3)
         assert abs(sk.score - s0.score) <= (1e-11 if same_kernel else 2e-11) * abs(s0.score)
         assert np.abs(sk.u - s0.u).max() <= (1e-11 if same_kernel else 1e-10)
     for _, _, _, s in res:
         assert sorted(s.nodes) == sorted(so.nodes.tolist())
         assert abs(s.score - so.score) <= (1e-9 if storage == 1 else 1e-5) * abs(so.score)
+
+
+def test_full_matrix_stripe_sweep_is_rejected(clp):
+    """there is no mode 1 (the stripe sweep reads the upper triangle only, as mode 2): asking for it is an error"""
+    c = make_euclid(clp)
+    with pytest.raises(clp.ClipperError):
+        c.set_dense_mode(1)
 
 
 @pytest.mark.parametrize("storage", [0, 1])

@@ -11,7 +11,9 @@ pytestmark = pytest.mark.gpu
 def _single(clp, prob, cfg, storage):
     ip = clp.invariants.EuclideanDistanceParams(); ip.sigma, ip.epsilon = cfg["sigma"], cfg["epsilon"]
     c = clp.CLIPPER(clp.invariants.EuclideanDistance(ip), clp.Params(), storage=storage)
-    c.set_dense_mode(1)  # the sweep the shards use (full matrix, stripes): same summation order -> 1e-12 comparable
+    # the segmented full-matrix sweep (what a sharded handle runs for a dense matrix); the shards make their own
+    # automatic choice, so their sums are grouped differently -> the 1e-10 bounds of the comparisons
+    c.set_dense_mode(0)
     c.score_pairwise_consistency(prob["D1"], prob["D2"], prob["A"])
     c.solve(prob["u0"])
     return c
@@ -30,7 +32,7 @@ def _group(clp, prob, cfg, devices, storage, same_device):
 
 @pytest.mark.parametrize("storage", [0, 1])
 @pytest.mark.parametrize("world,m", [(2, 1000), (2, 2500), (2, 777)])  # 3 shards x 122 regs do not fit one SM
-def test_sharded_same_device_matches_single(built, world, m, storage):
+def test_sharded_same_device_matches_segmented_single(built, world, m, storage):
     import clipper_b200 as clp
     from clipper_b200 import datagen
     prob = datagen.config_problem("c2", m); cfg = prob["cfg"]
