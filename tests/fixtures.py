@@ -57,6 +57,31 @@ def m20():
 DSD_NODES_20 = [3, 5, 12, 14, 15]
 
 
+def bytes_per_pass(kept, packed, esize=4):
+    """what one pass over the whole-row compact copy reads: entries (kept + one filler per empty 16-column window when
+    packed), rows sorted by length, four per item padded to the longest, plus 20 bytes of descriptors per item.
+    kept: the m x m boolean pattern of the stored off-diagonal entries, dense or scipy.sparse; esize: bytes of a stored
+    value (a 6-byte entry of fp32 storage is the value and a 16-bit column index)"""
+    import scipy.sparse as sp
+    m = kept.shape[0]
+    nwin = (m + 15) // 16
+    if sp.issparse(kept):
+        K = sp.csr_matrix(kept, dtype=bool); K.eliminate_zeros(); K.sort_indices()
+        lens = np.diff(K.indptr).astype(np.int64)
+        rows = np.repeat(np.arange(m, dtype=np.int64), lens)
+        occ = np.bincount(np.unique(rows * nwin + K.indices // 16) // nwin, minlength=m)
+    else:
+        lens = kept.sum(1).astype(np.int64)
+        occ = np.pad(kept, ((0, 0), (0, 16 * nwin - m))).reshape(m, nwin, 16).any(2).sum(1)
+    if packed:
+        lens = lens + (nwin - occ)
+    rows_pad = -(-m // 32) * 32
+    cls = np.zeros(rows_pad, np.int64)
+    cls[:m] = (lens + 3) // 4
+    stored = 16 * int(np.sort(cls)[::-1][0::4].sum())
+    return (4 if packed else esize + 2) * stored + rows_pad // 4 * 20
+
+
 def planecloud():
     """Plane normals of two LiDAR scans as 6xn point-normal data with zeroed points."""
     D1 = np.array([

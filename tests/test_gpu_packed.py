@@ -5,6 +5,8 @@ import os
 import numpy as np
 import pytest
 
+from fixtures import bytes_per_pass as _bytes_per_pass
+
 pytestmark = pytest.mark.gpu
 
 
@@ -43,22 +45,6 @@ def _euclid(clp, cfg):
     ip = clp.invariants.EuclideanDistanceParams()
     ip.sigma, ip.epsilon = cfg["sigma"], cfg["epsilon"]
     return clp.CLIPPER(clp.invariants.EuclideanDistance(ip), clp.Params())
-
-
-def _bytes_per_pass(kept, packed):
-    """what one pass over the whole-row compact copy reads: entries (kept + one filler per empty 16-column window when
-    packed), rows sorted by length, four per item padded to the longest, plus 20 bytes of descriptors per item"""
-    m = kept.shape[0]
-    lens = kept.sum(1).astype(np.int64)
-    if packed:
-        nwin = (m + 15) // 16
-        occ = np.pad(kept, ((0, 0), (0, 16 * nwin - m))).reshape(m, nwin, 16).any(2).sum(1)
-        lens = lens + (nwin - occ)
-    rows_pad = -(-m // 32) * 32
-    cls = np.zeros(rows_pad, np.int64)
-    cls[:m] = (lens + 3) // 4
-    stored = 16 * int(np.sort(cls)[::-1][0::4].sum())
-    return (4 if packed else 6) * stored + rows_pad // 4 * 20
 
 
 def _run(clp, prob, pack, v):
