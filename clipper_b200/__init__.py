@@ -14,9 +14,9 @@ CUDA kernels (clipper_b200/csrc); there is no CPU fallback for the built-in inva
 """
 from . import _capi
 from ._capi import ClipperError, STORE_F32, STORE_F64
-from .api import (CLIPPER, Params, Solution, Rounding, MCParams, SDPParams, invariants, utils, dsd,
+from .api import (CLIPPER, Params, Solution, Rounding, MCMethod, MCParams, SDPParams, invariants, utils, dsd,
                   __version__)
 from .batch import BatchCLIPPER
 
-__all__ = ["CLIPPER", "Params", "Solution", "Rounding", "MCParams", "SDPParams", "invariants", "utils",
+__all__ = ["CLIPPER", "Params", "Solution", "Rounding", "MCMethod", "MCParams", "SDPParams", "invariants", "utils",
            "dsd", "BatchCLIPPER", "ClipperError", "STORE_F32", "STORE_F64", "__version__"]

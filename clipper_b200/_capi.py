@@ -27,7 +27,9 @@ SYMBOLS = [
     "clp_set_ctas_per_sm", "clp_set_grid_cap", "clp_set_dense_mode", "clp_get_dense_mode", "clp_sparse_info",
     "clp_batch_create", "clp_batch_destroy", "clp_batch_last_error", "clp_batch_set_params",
     "clp_batch_solve_euclidean", "clp_batch_solve_pointnormal", "clp_batch_info",
+    "clp_max_clique", "clp_core_numbers",
 ]
+MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 
 
 class ClpParams(C.Structure):
@@ -49,6 +51,16 @@ class ClpSolution(C.Structure):
         ("n_evals", C.c_int64), ("n_matvec", C.c_int64), ("n_inner", C.c_int64),
         ("kernel_ms", C.c_double),
         ("prof_matvec_ms", C.c_double), ("prof_combine_ms", C.c_double), ("prof_exchange_ms", C.c_double),
+    ]
+
+
+class ClpMcInfo(C.Structure):
+    """clp_mc_info: statistics of one clp_max_clique call."""
+    _fields_ = [
+        ("n_nodes", C.c_int32), ("max_core", C.c_int32), ("lower_bound", C.c_int32), ("upper_bound", C.c_int32),
+        ("proven", C.c_int32), ("timed_out", C.c_int32), ("n_edges", C.c_int64), ("n_branches", C.c_int64),
+        ("t", C.c_double), ("kernel_ms", C.c_double),
+        ("adjacency_ms", C.c_double), ("peel_ms", C.c_double), ("heuristic_ms", C.c_double), ("search_ms", C.c_double),
     ]
 
 
@@ -125,6 +137,8 @@ def load():
     L.clp_batch_solve_pointnormal.argtypes = [vp, i32, pp, lp, pp, lp, pp, lp, pp, dbl, dbl, dbl, dbl,
                                               C.POINTER(ClpSolution), pp, pp]
     L.clp_batch_info.argtypes = [vp, ip, lp, lp]
+    L.clp_max_clique.argtypes = [vp, C.c_int, dbl, ip, C.POINTER(ClpMcInfo)]
+    L.clp_core_numbers.argtypes = [vp, ip]
     _lib = L
     return L
 

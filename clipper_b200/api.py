@@ -12,8 +12,11 @@ Differences that are deliberate and additive:
   * ``set_sparse_matrix_data`` exists (the reference forgot to bind it, SURVEY D8c).
   * ``dsd.solve`` is exported (the reference fills ``dsd`` with the utils by mistake, SURVEY D8b;
     both the mistaken names and the intended ``solve`` are present).
-  * ``solve_as_maximum_clique`` / ``solve_as_msrc_sdr`` behave like a reference build without
-    PMC / SCS (maxclique.cpp:141-144, sdp.cpp:298-302): they print a warning and select nothing.
+  * ``solve_as_maximum_clique(MCParams())`` runs on the GPU (clp_max_clique: KCORE, HEU, EXACT) instead of
+    PMC; its Solution carries the call's statistics in ``mc_info``.  Without params this mirror still behaves
+    like a build without PMC (warning, nothing selected), as it always did.  ``core_numbers()`` is additive.
+  * ``solve_as_msrc_sdr`` behaves like a reference build without SCS (sdp.cpp:298-302): it prints a
+    warning and selects nothing.
 """
 import ctypes as C
 import types
@@ -204,8 +207,15 @@ class Params:
         return "<CLIPPER Parameters>"
 
 
+class MCMethod:
+    """reference maxclique.h:16 (same order)"""
+    EXACT = 0
+    HEU = 1
+    KCORE = 2
+
+
 class MCParams:
-    """reference maxclique.h:18-24 (kept for source compatibility; PMC is not part of the hot path)"""
+    """reference maxclique.h:18-24 (same fields and defaults; threads is not used by the GPU solver)"""
 
     def __init__(self):
         self.method = 0
@@ -251,6 +261,7 @@ class Solution:
         self.n_inner = 0
         self.kernel_ms = 0.0
         self.prof_ms = (0.0, 0.0, 0.0)  # in-kernel split: dense passes, combine loops, exchange
+        self.mc_info = None  # solve_as_maximum_clique: the clp_mc_info fields as a dict
 
     def __repr__(self):
         return "<CLIPPER Solution>"
@@ -404,9 +415,42 @@ class CLIPPER:
         self._soln = out
 
     def solve_as_maximum_clique(self, params=None):
-        """reference clipper.cpp:82-97 with a build lacking PMC (maxclique.cpp:141-144)"""
-        print("Warning: clipper_b200 does not bundle PMC; maximum-clique solver unavailable.")
-        self._finish_unavailable()
+        """reference clipper.cpp:82-97: maximum clique of the constraint graph on the GPU (clp_max_clique).
+        params: MCParams (method EXACT / HEU / KCORE, time_limit in seconds, verbose); threads is not used.
+        The solution holds the nodes ascending, u = 0, score = -1, and the call's statistics in mc_info.
+        Called without params, this mirror keeps its earlier behaviour (a build without PMC: a warning, nothing
+        selected, score = -1), so code written against it sees no change; pass MCParams() to run the solver."""
+        if params is None:
+            print("Warning: solve_as_maximum_clique() without MCParams selects nothing; "
+                  "pass clipper_b200.MCParams() to run the GPU maximum-clique solver.")
+            self._finish_unavailable()
+            return
+        m = self._m()
+        nodes = np.zeros(max(m, 1), dtype=np.int32)
+        info = _capi.ClpMcInfo()
+        _capi.check(self._h, self._lib.clp_max_clique(self._h, int(params.method), float(params.time_limit),
+                                                      _ip(nodes), C.byref(info)))
+        if params.verbose:
+            print("maxclique: n %d edges %d max core %d lb %d ub %d omega %d proven %d%s | adjacency %.3f ms, "
+                  "peel %.3f ms, heuristic %.3f ms, search %.3f ms (%d branches)"
+                  % (m, info.n_edges, info.max_core, info.lower_bound, info.upper_bound, info.n_nodes, info.proven,
+                     " (time limit)" if info.timed_out else "", info.adjacency_ms, info.peel_ms, info.heuristic_ms,
+                     info.search_ms, info.n_branches))
+        s = Solution()
+        s.t = info.t
+        s.nodes = nodes[: info.n_nodes].tolist()
+        s.u0 = self._soln.u0  # untouched, as in the reference
+        s.u = np.zeros(m)
+        s.score = -1
+        s.kernel_ms = info.kernel_ms
+        s.mc_info = {name: getattr(info, name) for name, _ in _capi.ClpMcInfo._fields_}
+        self._soln = s
+
+    def core_numbers(self):
+        """core number of every vertex of the constraint graph (additive; clp_core_numbers)"""
+        out = np.zeros(max(self._m(), 1), dtype=np.int32)
+        _capi.check(self._h, self._lib.clp_core_numbers(self._h, _ip(out)))
+        return out[: self._m()].copy()
 
     def solve_as_msrc_sdr(self, params=None):
         """reference clipper.cpp:101-113 with a build lacking SCS (sdp.cpp:298-302)"""

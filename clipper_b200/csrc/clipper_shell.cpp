@@ -12,6 +12,7 @@
 #include "clipper/utils.h"
 #include "clipper_b200.h"
 
+#include <algorithm>
 #include <cmath>
 #include <iostream>
 #include <random>
@@ -158,19 +159,41 @@ void CLIPPER::solve(const Eigen::VectorXd& u0)
   n_evals_ = s.n_evals;
 }
 
-// reference clipper.cpp:82-97
+namespace {
+
+// clp_max_clique on a handle that holds the graph; one stats line when verbose
+std::vector<int> max_clique_on(clp_handle h, const maxclique::Params& params)
+{
+  int64_t m = 0;
+  check(h, clp_num_associations(h, &m), "clp_num_associations");
+  std::vector<int32_t> nodes((size_t)std::max<int64_t>(m, 1));
+  clp_mc_info info;
+  check(h, clp_max_clique(h, (int)params.method, (double)params.time_limit, nodes.data(), &info), "clp_max_clique");
+  if (params.verbose)
+    std::cout << "maxclique: n " << m << " edges " << info.n_edges << " max core " << info.max_core << " lb "
+              << info.lower_bound << " ub " << info.upper_bound << " omega " << info.n_nodes << " proven " << info.proven
+              << (info.timed_out ? " (time limit)" : "") << " | adjacency " << info.adjacency_ms << " ms, peel "
+              << info.peel_ms << " ms, heuristic " << info.heuristic_ms << " ms, search " << info.search_ms << " ms ("
+              << info.n_branches << " branches)" << std::endl;
+  return std::vector<int>(nodes.begin(), nodes.begin() + info.n_nodes);
+}
+
+}  // namespace
+
+// reference clipper.cpp:82-97, on the graph already in HBM (no dense round trip); params.threads is not used
 void CLIPPER::solveAsMaximumClique(const maxclique::Params& params)
 {
-  Eigen::MatrixXd C = getConstraintMatrix();
-  for (long i = 0; i < (long)C.rows(); ++i) C(i, i) -= 1.0;
+  clp_handle h = static_cast<clp_handle>(handle());
+  int64_t m = 0;
+  check(h, clp_num_associations(h, &m), "clp_num_associations");
   utils::Timer tim;
   tim.start();
-  std::vector<int> nodes = maxclique::solve(C, params);
+  std::vector<int> nodes = max_clique_on(h, params);
   tim.stop();
   soln_.t = tim.getElapsedSeconds();
   soln_.ifinal = 0;
   std::swap(soln_.nodes, nodes);
-  soln_.u = Eigen::VectorXd::Zero(C.cols());
+  soln_.u = Eigen::VectorXd::Zero(m);
   soln_.score = -1;
 }
 
@@ -348,10 +371,21 @@ Solution solve(const Eigen::MatrixXd&, const Eigen::MatrixXd&, const Params&)
 }  // namespace sdp
 
 namespace maxclique {
-std::vector<int> solve(const Eigen::MatrixXd&, const Params&)
+// reference maxclique.cpp:46-147 on device 0: any nonzero of the strict upper triangle of A is an edge
+std::vector<int> solve(const Eigen::MatrixXd& A, const Params& params)
 {
-  std::cout << "Warning: clipper was not built with PMC; maximum clique solver unavailable." << std::endl;
-  return {};
+  const int64_t n = (int64_t)A.rows();
+  if (A.cols() != A.rows()) throw std::runtime_error("clipper_b200: maxclique::solve expects a square matrix");
+  if (n == 0) return {};
+  clp_handle h = nullptr;
+  if (clp_create(0, CLP_STORE_F32, &h) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_create: ") + clp_last_error(nullptr));
+  std::shared_ptr<void> guard(h, [](void* p) { clp_destroy(static_cast<clp_handle>(p)); });
+  Eigen::MatrixXd M = Eigen::MatrixXd::Zero(n, n), C = Eigen::MatrixXd::Zero(n, n);
+  for (int64_t j = 0; j < n; ++j)
+    for (int64_t i = 0; i < j; ++i) C(i, j) = A(i, j) != 0 ? 1.0 : 0.0;
+  check(h, clp_set_dense(h, M.data(), C.data(), n), "clp_set_dense");
+  return max_clique_on(h, params);
 }
 }  // namespace maxclique
 

@@ -4,6 +4,7 @@
 // There is NO CPU implementation of the hot path in this library: every scoring / mat-vec /
 // solve call launches the sm_90a kernels of clp_kernels.cuh or fails with an error code.
 #include "clp_kernels.cuh"
+#include "clp_clique.cuh"
 #include "clp_host_utils.h"
 #include "../../include/clipper_b200.h"
 
@@ -132,6 +133,9 @@ struct clp_handle_s {
   Plan2 plan2{};
   Dense2Buffers d2{};
   DevBuf d2buf, plan2buf;
+  // maximum clique (clp_clique.cuh): the bitset adjacency is built on the first call and dropped with the matrix
+  DevBuf mc_adj, mc_work, mc_scratch;
+  bool mc_adj_valid = false;
 
   size_t esize() const { return storage == CLP_STORE_F64 ? 8 : 4; }
   int entry_bytes() const { return sp.packed ? 4 : (int)esize() + 2; }  // compact copy: bytes per stored entry
@@ -556,6 +560,9 @@ int ensure_matrix(clp_handle h, long long m) {
   if (m <= 0) return fail(h, CLP_ERR_INVALID, "number of associations must be positive");
   if (m > (long long)kMaxSeg * kSegMax) return fail(h, CLP_ERR_INVALID, "m exceeds the supported maximum (262144)");
   CLP_CUDA(h, cudaSetDevice(h->device));
+  h->mc_adj_valid = false;  // the max-clique adjacency describes the previous matrix
+  h->mc_adj.release();
+  h->mc_scratch.release();
   h->m = m;
   shard_rows(m, h->rank, h->world, &h->row0, &h->rows);
   h->rows_pad = (int)round_up(std::max(h->rows, 1), kRowTile);
@@ -924,6 +931,260 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
   return CLP_OK;
 }
 
+// ------------------------------------------------------------------------------------------
+// maximum clique (clp_clique.cuh)
+// ------------------------------------------------------------------------------------------
+struct McLayout {  // int32 regions of mc_work, then 8-byte ones
+  int *deg0, *deg, *core, *rnd, *frontier, *later, *seeds, *roots, *nodes;
+  unsigned *alive, *ctr;
+  int *out, *flags;
+  long long* tprefix;
+  unsigned long long *best, *next, *branches, *deadline;
+};
+
+size_t mc_layout(long long m, int W, char* base, McLayout* L) {
+  size_t off = 0;
+  auto take = [&](size_t bytes) { char* p = base + off; off += (bytes + 15) / 16 * 16; return p; };
+  const size_t mi = (size_t)m * sizeof(int);
+  L->deg0 = (int*)take(mi); L->deg = (int*)take(mi); L->core = (int*)take(mi); L->rnd = (int*)take(mi);
+  L->frontier = (int*)take(mi); L->later = (int*)take(mi); L->seeds = (int*)take(mi); L->roots = (int*)take(mi);
+  L->nodes = (int*)take(mi + sizeof(int));
+  L->alive = (unsigned*)take((size_t)W * sizeof(unsigned)); L->ctr = (unsigned*)take(4 * sizeof(unsigned));
+  L->out = (int*)take(4 * sizeof(int)); L->flags = (int*)take(4 * sizeof(int));
+  L->tprefix = (long long*)take(((size_t)m + 1) * sizeof(long long));
+  L->best = (unsigned long long*)take(8); L->next = (unsigned long long*)take(8);
+  L->branches = (unsigned long long*)take(8); L->deadline = (unsigned long long*)take(8);
+  return off;
+}
+
+struct McPeeled {
+  std::vector<int32_t> core, rnd;
+  int max_core = 0;
+  long long n_edges = 0;
+  float adj_ms = 0.f, peel_ms = 0.f;
+};
+
+struct McEvents {  // timing of one call; destroyed with the call
+  cudaEvent_t e[8] = {};
+  ~McEvents() { for (cudaEvent_t x : e) if (x) cudaEventDestroy(x); }
+};
+
+float mc_elapsed(cudaEvent_t a, cudaEvent_t b) {
+  float ms = 0.f;
+  return cudaEventElapsedTime(&ms, a, b) == cudaSuccess ? ms : 0.f;
+}
+
+// bitset adjacency (built once per matrix) + k-core peel; core numbers and removal iterations come back to the host
+int mc_prepare(clp_handle h, McLayout* L, McPeeled* out, McEvents& ev) {
+  if (!h->has_matrix) return fail(h, CLP_ERR_INVALID, "maximum clique before any affinity matrix was scored or set");
+  if (h->world > 1) return fail(h, CLP_ERR_UNSUPPORTED, "maximum clique on a sharded handle (a rank holds only its own rows)");
+  CLP_CUDA(h, cudaSetDevice(h->device));
+  const long long m = h->m;
+  const int W = (int)((m + 31) / 32);
+  McLayout probe;
+  const size_t work = mc_layout(m, W, nullptr, &probe);
+  CLP_CUDA(h, h->mc_work.ensure(work));
+  mc_layout(m, W, h->mc_work.as<char>(), L);
+  for (cudaEvent_t& x : ev.e) CLP_CUDA(h, cudaEventCreate(&x));
+  CLP_CUDA(h, cudaEventRecord(ev.e[0], h->stream));
+  const bool rebuild = !h->mc_adj_valid;
+  if (rebuild) {
+    CLP_CUDA(h, h->mc_adj.ensure((size_t)m * W * sizeof(unsigned)));
+    if (h->storage == CLP_STORE_F64)
+      mc_adjacency_kernel<double><<<(unsigned)m, kMcThreads, 0, h->stream>>>(h->Mbuf.as<double>(), h->ld, (int)m, W, h->mc_adj.as<unsigned>(), L->deg0);
+    else
+      mc_adjacency_kernel<float><<<(unsigned)m, kMcThreads, 0, h->stream>>>(h->Mbuf.as<float>(), h->ld, (int)m, W, h->mc_adj.as<unsigned>(), L->deg0);
+    CLP_CUDA(h, cudaGetLastError());
+  }
+  CLP_CUDA(h, cudaEventRecord(ev.e[1], h->stream));
+  // peel: one cooperative launch, every CTA co-resident
+  int occ = 0;
+  CLP_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, mc_peel_kernel, kMcPeelThreads, 0));
+  if (occ < 1) return fail(h, CLP_ERR_CUDA, "k-core peel kernel cannot be resident");
+  const int G = h->sm_count * std::min(occ, 2);
+  CLP_CUDA(h, cudaMemcpyAsync(L->deg, L->deg0, (size_t)m * sizeof(int), cudaMemcpyDeviceToDevice, h->stream));
+  CLP_CUDA(h, cudaMemsetAsync(L->ctr, 0, 4 * sizeof(unsigned), h->stream));
+  if (int rc = reset_sync(h)) return rc;
+  McPeelArgs pa;
+  pa.adj = h->mc_adj.as<unsigned>(); pa.m = (int)m; pa.W = W;
+  pa.deg = L->deg; pa.alive = L->alive; pa.core = L->core; pa.rnd = L->rnd; pa.frontier = L->frontier;
+  pa.ctr = L->ctr; pa.out = L->out;
+  pa.bar.sb = h->sync.as<SyncBlock>(); pa.bar.nleaf = std::min(32, G); pa.bar.G = G;
+  void* args[] = {&pa};
+  CLP_CUDA(h, cudaLaunchCooperativeKernel((const void*)mc_peel_kernel, dim3(G), dim3(kMcPeelThreads), args, 0, h->stream));
+  CLP_CUDA(h, cudaEventRecord(ev.e[2], h->stream));
+  out->core.resize((size_t)m); out->rnd.resize((size_t)m);
+  std::vector<int32_t> deg0((size_t)m);
+  int hout[4] = {0, 0, 0, 0};
+  CLP_CUDA(h, cudaMemcpyAsync(out->core.data(), L->core, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaMemcpyAsync(out->rnd.data(), L->rnd, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaMemcpyAsync(deg0.data(), L->deg0, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaMemcpyAsync(hout, L->out, sizeof(hout), cudaMemcpyDeviceToHost, h->stream));
+  SyncBlock sb;
+  if (int rc = read_sync(h, &sb)) return rc;  // synchronises the stream
+  if (sb.error) return fail(h, CLP_ERR_TIMEOUT, "k-core peel: device-wide barrier timed out");
+  h->mc_adj_valid = true;
+  out->max_core = hout[0];
+  long long deg_sum = 0;
+  for (int32_t x : deg0) deg_sum += x;
+  out->n_edges = deg_sum / 2;
+  out->adj_ms = rebuild ? mc_elapsed(ev.e[0], ev.e[1]) : 0.f;
+  out->peel_ms = mc_elapsed(ev.e[1], ev.e[2]);
+  return CLP_OK;
+}
+
+int mc_solve(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, clp_mc_info* info) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return fail(h, CLP_ERR_INVALID, "unknown maximum-clique method");
+  McLayout L;
+  McPeeled pk;
+  McEvents ev;
+  if (int rc = mc_prepare(h, &L, &pk, ev)) return rc;
+  const long long m = h->m;
+  const int W = (int)((m + 31) / 32);
+  const unsigned* adj = h->mc_adj.as<unsigned>();
+  std::vector<int32_t> nodes;
+  int lb = 0, proven = 0, timed_out = 0;
+  long long branches = 0;
+  float heu_ms = 0.f, search_ms = 0.f;
+  if (method == CLP_MC_KCORE) {  // maxclique.cpp:89-100
+    for (long long v = 0; v < m; ++v) if (pk.core[(size_t)v] >= pk.max_core) nodes.push_back((int32_t)v);
+  } else {
+    // degeneracy order: (removal iteration, index) ascending; seeds and roots run in reverse (descending core)
+    std::vector<int32_t> order((size_t)m);
+    for (long long v = 0; v < m; ++v) order[(size_t)v] = (int32_t)v;
+    std::stable_sort(order.begin(), order.end(), [&](int32_t x, int32_t y) { return pk.rnd[(size_t)x] < pk.rnd[(size_t)y]; });
+    std::vector<int32_t> rev(order.rbegin(), order.rend());
+    CLP_CUDA(h, cudaMemcpyAsync(L.seeds, rev.data(), (size_t)m * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CLP_CUDA(h, cudaMemsetAsync(L.best, 0, sizeof(unsigned long long), h->stream));
+    const size_t row_bytes = (size_t)W * sizeof(unsigned);
+    if (row_bytes > (size_t)h->smem_optin) return fail(h, CLP_ERR_UNSUPPORTED, "maximum clique: m too large for the heuristic's shared-memory bitset");
+    const int wpc = (int)std::max<size_t>(1, std::min<size_t>(kMcThreads / 32, (size_t)(h->smem_optin - 1024) / row_bytes));
+    const size_t smem = (size_t)wpc * row_bytes;
+    CLP_CUDA(h, cudaFuncSetAttribute(mc_heu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, row_bytes)));
+    const unsigned grid = (unsigned)std::min<long long>((m + wpc - 1) / wpc, (long long)h->sm_count * 16);
+    CLP_CUDA(h, cudaEventRecord(ev.e[3], h->stream));
+    mc_heu_kernel<<<grid, wpc * 32, smem, h->stream>>>(adj, (int)m, W, L.core, L.seeds, L.best, -1, L.nodes);
+    CLP_CUDA(h, cudaGetLastError());
+    unsigned long long best = 0;
+    CLP_CUDA(h, cudaMemcpyAsync(&best, L.best, sizeof(best), cudaMemcpyDeviceToHost, h->stream));
+    CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+    const int seed = (int)(0xffffffffu - (unsigned)(best & 0xffffffffull));
+    mc_heu_kernel<<<1, 32, row_bytes, h->stream>>>(adj, (int)m, W, L.core, L.seeds, L.best, seed, L.nodes);
+    CLP_CUDA(h, cudaGetLastError());
+    CLP_CUDA(h, cudaEventRecord(ev.e[4], h->stream));
+    lb = (int)(best >> 32);
+    nodes.resize((size_t)lb);
+    int replay_size = 0;
+    CLP_CUDA(h, cudaMemcpyAsync(nodes.data(), L.nodes, (size_t)lb * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CLP_CUDA(h, cudaMemcpyAsync(&replay_size, L.nodes + m, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+    heu_ms = mc_elapsed(ev.e[3], ev.e[4]);
+    if (replay_size != lb) return fail(h, CLP_ERR_CUDA, "maximum clique: heuristic replay disagrees with its winner");
+    const int ub = pk.max_core + 1;
+    proven = (lb == ub) ? 1 : 0;
+    if (method == CLP_MC_EXACT && lb < ub && time_limit_s > 0) {
+      if (pk.max_core > kMcMaxCore)
+        return fail(h, CLP_ERR_UNSUPPORTED, "maximum clique EXACT: max core " + std::to_string(pk.max_core) +
+                                                " exceeds the search's limit of " + std::to_string(kMcMaxCore) + " (use HEU or KCORE)");
+      // roots: core + 1 > lb, reverse degeneracy order; a root with many candidates becomes one task per candidate
+      const int nwl = kMcThreads / 32;
+      mc_later_count_kernel<<<(unsigned)std::min<long long>((m + nwl - 1) / nwl, (long long)h->sm_count * 16), kMcThreads, 0, h->stream>>>(
+          adj, (int)m, W, L.rnd, L.later);
+      CLP_CUDA(h, cudaGetLastError());
+      std::vector<int32_t> later((size_t)m);
+      CLP_CUDA(h, cudaMemcpyAsync(later.data(), L.later, (size_t)m * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+      CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+      std::vector<int32_t> roots;
+      std::vector<long long> tprefix(1, 0);
+      for (int32_t v : rev) {
+        if (pk.core[(size_t)v] + 1 <= lb || later[(size_t)v] + 1 <= lb) continue;
+        roots.push_back(v);
+        tprefix.push_back(tprefix.back() + (later[(size_t)v] > kMcSplit ? later[(size_t)v] : 1));
+      }
+      const long long ntasks = tprefix.back();
+      unsigned long long best_s = mc_key((unsigned)lb, 0u);
+      unsigned hflags[4] = {0u, 0u, 0u, 0u};
+      if (ntasks > 0) {
+        int K = 1;
+        for (int32_t v : roots) K = std::max(K, (int)later[(size_t)v]);
+        const int KW = (K + 31) / 32;
+        const unsigned arena_cap = (unsigned)std::min<long long>((long long)K * (K + 1) / 2 + 64, 1ll << 18);
+        const size_t stride = mc_scratch_bytes(K, KW, arena_cap);
+        size_t free_b = 0, total_b = 0;
+        CLP_CUDA(h, cudaMemGetInfo(&free_b, &total_b));
+        const long long want = (long long)h->sm_count * 2 * kMcSearchWarps;
+        long long nworkers = std::min<long long>(want, (long long)(free_b / 2 / stride));
+        nworkers = nworkers / kMcSearchWarps * kMcSearchWarps;
+        if (nworkers < kMcSearchWarps)
+          return fail(h, CLP_ERR_ALLOC, "maximum clique EXACT: not enough device memory for the search scratch");
+        CLP_CUDA(h, h->mc_scratch.ensure((size_t)nworkers * stride));
+        CLP_CUDA(h, cudaMemcpyAsync(L.roots, roots.data(), roots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+        CLP_CUDA(h, cudaMemcpyAsync(L.tprefix, tprefix.data(), tprefix.size() * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
+        CLP_CUDA(h, cudaMemcpyAsync(L.best, &best_s, sizeof(best_s), cudaMemcpyHostToDevice, h->stream));
+        CLP_CUDA(h, cudaMemsetAsync(L.next, 0, sizeof(unsigned long long), h->stream));
+        CLP_CUDA(h, cudaMemsetAsync(L.branches, 0, sizeof(unsigned long long), h->stream));
+        CLP_CUDA(h, cudaMemsetAsync(L.flags, 0, 4 * sizeof(int), h->stream));
+        const double left = time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+        const double left_ns = std::max(0.0, left) * 1e9;
+        const unsigned long long limit_ns = left_ns >= 1.8e19 ? ~0ull : (unsigned long long)left_ns;
+        McSearchArgs sa;
+        sa.adj = adj; sa.m = (int)m; sa.W = W; sa.rnd = L.rnd; sa.roots = L.roots; sa.tprefix = L.tprefix;
+        sa.nroots = (int)roots.size(); sa.ntasks = ntasks; sa.K = K; sa.KW = KW; sa.arena_cap = arena_cap;
+        sa.scratch = h->mc_scratch.as<unsigned char>(); sa.stride = stride;
+        sa.best = L.best; sa.next_task = L.next; sa.n_branches = L.branches; sa.flags = L.flags; sa.deadline = L.deadline;
+        sa.replay_task = -1; sa.replay_size = 0; sa.nodes_out = L.nodes;
+        const size_t ssmem = (size_t)kMcSearchWarps * 2 * KW * sizeof(unsigned);
+        CLP_CUDA(h, cudaFuncSetAttribute(mc_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+        CLP_CUDA(h, cudaEventRecord(ev.e[5], h->stream));
+        mc_deadline_kernel<<<1, 1, 0, h->stream>>>(L.deadline, limit_ns);
+        mc_search_kernel<<<(unsigned)(nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, h->stream>>>(sa);
+        CLP_CUDA(h, cudaGetLastError());
+        unsigned long long hb[2] = {0ull, 0ull};
+        CLP_CUDA(h, cudaMemcpyAsync(&hb[0], L.best, 8, cudaMemcpyDeviceToHost, h->stream));
+        CLP_CUDA(h, cudaMemcpyAsync(&hb[1], L.branches, 8, cudaMemcpyDeviceToHost, h->stream));
+        CLP_CUDA(h, cudaMemcpyAsync(hflags, L.flags, sizeof(hflags), cudaMemcpyDeviceToHost, h->stream));
+        CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+        best_s = hb[0]; branches = (long long)hb[1];
+        const int s = (int)(best_s >> 32);
+        if (s > lb) {  // a task beat the heuristic: replay it for the nodes
+          sa.replay_task = (long long)(0xffffffffu - (unsigned)(best_s & 0xffffffffull));
+          sa.replay_size = s;
+          mc_search_kernel<<<1, 32, 2 * KW * sizeof(unsigned), h->stream>>>(sa);
+          CLP_CUDA(h, cudaGetLastError());
+          int got = 0;
+          CLP_CUDA(h, cudaMemcpyAsync(&got, L.nodes + m, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+          CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+          if (got < s || got > m) return fail(h, CLP_ERR_CUDA, "maximum clique: search replay did not reproduce its clique");
+          nodes.resize((size_t)got);
+          CLP_CUDA(h, cudaMemcpyAsync(nodes.data(), L.nodes, (size_t)got * sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        }
+        CLP_CUDA(h, cudaEventRecord(ev.e[6], h->stream));
+        CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+        search_ms = mc_elapsed(ev.e[5], ev.e[6]);
+      }
+      timed_out = hflags[0] ? 1 : 0;
+      proven = (hflags[0] == 0u && hflags[1] == 0u) ? 1 : 0;
+    }
+    std::sort(nodes.begin(), nodes.end());
+  }
+  if (nodes_out && !nodes.empty()) std::memcpy(nodes_out, nodes.data(), nodes.size() * sizeof(int32_t));
+  if (info) {
+    info->n_nodes = (int32_t)nodes.size();
+    info->max_core = pk.max_core;
+    info->lower_bound = lb;
+    info->upper_bound = pk.max_core + 1;
+    info->proven = proven;
+    info->timed_out = timed_out;
+    info->n_edges = pk.n_edges;
+    info->n_branches = branches;
+    info->adjacency_ms = pk.adj_ms; info->peel_ms = pk.peel_ms; info->heuristic_ms = heu_ms; info->search_ms = search_ms;
+    info->kernel_ms = pk.adj_ms + pk.peel_ms + heu_ms + search_ms;
+    info->t = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  }
+  return CLP_OK;
+}
+
 }  // namespace
 
 // ==========================================================================================
@@ -1001,7 +1262,8 @@ int clp_destroy(clp_handle h) {
     if (h->peer_opened[r]) { cudaIpcCloseMemHandle(h->peer_open_ptr[r][0]); cudaIpcCloseMemHandle(h->peer_open_ptr[r][1]); }
   h->comm.release();
   for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
-                    &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf})
+                    &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
+                    &h->mc_adj, &h->mc_work, &h->mc_scratch})
     b->release();
   if (h->pinned) cudaFreeHost(h->pinned);
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1224,6 +1486,24 @@ int clp_solve_dev(clp_handle h, const double* u0_dev, clp_solution* out, double*
   CLP_CUDA(h, cudaSetDevice(h->device));
   CLP_CUDA(h, cudaMemcpyAsync(h->u0dev.p, u0_dev, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
   return guarded(h, [&] { return solve_core(h, out, nullptr, u_out_dev, nodes_out, t0); });
+}
+
+// ---- maximum clique -------------------------------------------------------------------------
+int clp_max_clique(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, clp_mc_info* info) {
+  if (!h) return CLP_ERR_INVALID;
+  return guarded(h, [&] { return mc_solve(h, method, time_limit_s, nodes_out, info); });
+}
+
+int clp_core_numbers(clp_handle h, int32_t* core_out) {
+  if (!h || !core_out) return CLP_ERR_INVALID;
+  return guarded(h, [&] {
+    McLayout L;
+    McPeeled pk;
+    McEvents ev;
+    if (int rc = mc_prepare(h, &L, &pk, ev)) return rc;
+    std::memcpy(core_out, pk.core.data(), pk.core.size() * sizeof(int32_t));
+    return CLP_OK;
+  });
 }
 
 // ---- mat-vec ------------------------------------------------------------------------------

@@ -202,6 +202,42 @@ int clp_get_dense_mode(clp_handle h, int* requested, int* effective);
 /* entries kept by the compact copy (all local rows) and the algorithmic bytes one sparse pass reads */
 int clp_sparse_info(clp_handle h, int64_t* nnz_kept, int64_t* bytes_per_pass);
 
+/* ---- maximum clique of the constraint graph (solveAsMaximumClique, clipper.cpp:82-97, maxclique.cpp:89-140) --------
+ * The graph is C without its diagonal: {i,j} is an edge iff C_ij = 1 (the sign bit of the stored element is clear),
+ * whatever M_ij is.  Methods keep the order of clipper::maxclique::Method:
+ *   CLP_MC_EXACT: a maximum clique.  lb = size of the HEU clique, ub = max core + 1; lb == ub returns the HEU clique,
+ *     else a branch-and-bound on the device searches for a larger one until it is proven or time_limit_s expires
+ *     (then the best clique found is returned with proven = 0, timed_out = 1).  time_limit_s <= 0 returns the HEU
+ *     clique without searching.  The search sizes its scratch from the max core: a max core above 8191 is
+ *     CLP_ERR_UNSUPPORTED (KCORE and HEU have no such limit).  Once proven, the clique returned does not depend on
+ *     the schedule (largest clique of the first search task, in the fixed task order, that holds one).
+ *   CLP_MC_HEU: greedy clique from every seed v (K = {v}, P = N(v); repeatedly add the u in P of highest core number,
+ *     ties to the lowest index, P &= N(u)); the largest K, ties to the smallest seed.
+ *   CLP_MC_KCORE: every vertex whose core number equals the max core (an edgeless graph returns every vertex).
+ * nodes_out (m int32) receives the nodes in ascending order (info->n_nodes of them); info may be NULL.  m = 1 gives
+ * {0}.  A sharded handle returns CLP_ERR_UNSUPPORTED.  The bitset adjacency (m^2/8 bytes) is built on the first call
+ * and dropped when a new matrix is scored or set. */
+#define CLP_MC_EXACT 0
+#define CLP_MC_HEU 1
+#define CLP_MC_KCORE 2
+typedef struct clp_mc_info {
+  int32_t n_nodes;      /* size of the returned node set                                         */
+  int32_t max_core;     /* largest core number                                                    */
+  int32_t lower_bound;  /* size of the HEU clique (0 for KCORE)                                   */
+  int32_t upper_bound;  /* max_core + 1                                                           */
+  int32_t proven;       /* 1: the nodes are known to be a maximum clique (lb == ub, or the search completed) */
+  int32_t timed_out;    /* 1: the search stopped at time_limit_s                                  */
+  int64_t n_edges;      /* edges of the graph                                                     */
+  int64_t n_branches;   /* branch-and-bound nodes expanded                                        */
+  double t;             /* wall-clock seconds of the call                                         */
+  double kernel_ms;     /* device time of all kernels of the call (CUDA events)                   */
+  /* phase split (CUDA events): adjacency build (0 when reused), peel, heuristic, search */
+  double adjacency_ms, peel_ms, heuristic_ms, search_ms;
+} clp_mc_info;
+int clp_max_clique(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, clp_mc_info* info);
+/* core number of every vertex of the same graph (m int32) */
+int clp_core_numbers(clp_handle h, int32_t* core_out);
+
 /* ---- batches of small problems: hundreds of registrations in ONE launch (SURVEY 8f rank 4) ------------------------
  * The reference's benchmark solves its m <= 2048 problems one after the other (benchmarks/main.cpp:254-270: a fresh
  * clipper::CLIPPER, scorePairwiseConsistency, solve per trial).  A batch handle takes the whole list: ONE CTA per
