@@ -28,6 +28,7 @@ SYMBOLS = [
     "clp_batch_create", "clp_batch_destroy", "clp_batch_last_error", "clp_batch_set_params",
     "clp_batch_solve_euclidean", "clp_batch_solve_pointnormal", "clp_batch_info",
     "clp_max_clique", "clp_core_numbers",
+    "clp_batch_max_clique_euclidean", "clp_batch_max_clique_pointnormal", "clp_batch_max_clique_graphs",
 ]
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 
@@ -139,6 +140,12 @@ def load():
     L.clp_batch_info.argtypes = [vp, ip, lp, lp]
     L.clp_max_clique.argtypes = [vp, C.c_int, dbl, ip, C.POINTER(ClpMcInfo)]
     L.clp_core_numbers.argtypes = [vp, ip]
+    mip = C.POINTER(ClpMcInfo)
+    L.clp_batch_max_clique_euclidean.argtypes = [vp, i32, i32, pp, lp, pp, lp, pp, lp, dbl, dbl, dbl, C.c_int, dbl,
+                                                 mip, pp, pp]
+    L.clp_batch_max_clique_pointnormal.argtypes = [vp, i32, pp, lp, pp, lp, pp, lp, dbl, dbl, dbl, dbl, C.c_int, dbl,
+                                                   mip, pp, pp]
+    L.clp_batch_max_clique_graphs.argtypes = [vp, i32, lp, pp, pp, C.c_int, dbl, mip, pp, pp]
     _lib = L
     return L
 

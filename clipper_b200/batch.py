@@ -4,13 +4,15 @@ The reference's own operating point is m <= 2048 associations per registration a
 one after the other, each with a fresh clipper::CLIPPER (reference benchmarks/main.cpp:206-208, 254-270).  ``BatchCLIPPER``
 takes the whole list: one CTA per problem scores the pairs, builds the compact copy and runs the solver, no device-wide
 synchronisation anywhere; results per problem are those of ``CLIPPER.score_pairwise_consistency`` + ``solve``.
+``BatchCLIPPER.max_clique_many`` and ``maxclique_many`` solve each problem of such a list as a maximum clique
+(clp_batch_max_clique_*): per problem the answer of ``CLIPPER.solve_as_maximum_clique`` on an fp32 handle.
 """
 import ctypes as C
 
 import numpy as np
 
 from . import _capi
-from .api import EuclideanDistance, PointNormalDistance, Params, Solution, _check_f64
+from .api import EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64
 
 
 class BatchCLIPPER:
@@ -46,6 +48,58 @@ class BatchCLIPPER:
         a, b, c = C.c_int32(), C.c_int64(), C.c_int64()
         self._check(self._lib.clp_batch_info(self._b, C.byref(a), C.byref(b), C.byref(c)))
         return int(a.value), int(b.value), int(c.value)
+
+    def max_clique_many(self, problems, params=None):
+        """problems: the dicts of solve_many (u0 is not needed); params: MCParams (method, time_limit for the whole
+        call, verbose; threads is not used).  Scores every problem with the batch's invariant and affinityeps and
+        returns one api.Solution per problem, as CLIPPER.solve_as_maximum_clique sets it (nodes ascending, u = 0,
+        score = -1, mc_info) plus ``core``, the core numbers."""
+        problems = list(problems)
+        n = len(problems)
+        if n == 0:
+            return []
+        params = params if params is not None else MCParams()
+        self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
+        keep = []
+        vp = C.c_void_p
+        D1p, D2p, Ap = (vp * n)(), (vp * n)(), (vp * n)()
+        n1, n2, m = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
+        ms = []
+        d = None
+        for k, p in enumerate(problems):
+            D1 = np.asfortranarray(_check_f64(p["D1"], "D1")); D2 = np.asfortranarray(_check_f64(p["D2"], "D2"))
+            if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
+                raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+            if d is None:
+                d = D1.shape[0]
+            elif d != D1.shape[0]:
+                raise ValueError("all problems of a batch must have the same data dimension")
+            A = p.get("A")
+            if A is None or np.size(A) == 0:
+                mk = D1.shape[1] * D2.shape[1]; Ak = None
+            else:
+                if not isinstance(A, np.ndarray) or A.dtype != np.int32 or A.ndim != 2 or A.shape[1] != 2:
+                    raise TypeError("A must be an (m, 2) numpy int32 array")
+                Ak = np.asfortranarray(A); mk = Ak.shape[0]
+            keep += [D1, D2, Ak]
+            ms.append(mk)
+            D1p[k], D2p[k] = D1.ctypes.data, D2.ctypes.data
+            Ap[k] = Ak.ctypes.data if Ak is not None else None
+            n1[k], n2[k], m[k] = D1.shape[1], D2.shape[1], (mk if Ak is not None else 0)
+        inv = self._invariant
+        out, args = _mc_outputs(ms, params)
+        if isinstance(inv, EuclideanDistance):
+            q = inv.params()
+            rc = self._lib.clp_batch_max_clique_euclidean(self._b, n, int(d), D1p, n1, D2p, n2, Ap, m, float(q.sigma),
+                                                          float(q.epsilon), float(q.mindist), *args)
+        else:
+            if d != 6:
+                raise ValueError("PointNormalDistance expects 6 x n data")
+            q = inv.params()
+            rc = self._lib.clp_batch_max_clique_pointnormal(self._b, n, D1p, n1, D2p, n2, Ap, m, float(q.sigp),
+                                                            float(q.epsp), float(q.sign), float(q.epsn), *args)
+        self._check(rc)
+        return out()
 
     def solve_many(self, problems):
         """problems: sequence of dicts with D1 (d, n1) float64, D2 (d, n2) float64, A (m, 2) int32 or None (all-to-all)
@@ -111,3 +165,102 @@ class BatchCLIPPER:
             o.prof_ms = (s.prof_matvec_ms, s.prof_combine_ms, s.prof_exchange_ms)
             out.append(o)
         return out
+
+
+def _mc_outputs(ms, params):
+    """output arrays of one batched maximum-clique call for problems of ms[p] vertices: the trailing C-ABI arguments
+    (method, time limit, infos, nodes, cores) and a function that turns them into Solutions after the call"""
+    n = len(ms)
+    vp = C.c_void_p
+    infos = (_capi.ClpMcInfo * n)()
+    nodes = [np.zeros(max(mk, 1), np.int32) for mk in ms]
+    cores = [np.zeros(max(mk, 1), np.int32) for mk in ms]
+    nodep, corep = (vp * n)(), (vp * n)()
+    for k in range(n):
+        nodep[k], corep[k] = nodes[k].ctypes.data, cores[k].ctypes.data
+
+    def finish():
+        out = []
+        for k in range(n):
+            info = infos[k]
+            s = Solution()
+            s.t = info.t
+            s.nodes = nodes[k][: info.n_nodes].tolist()
+            s.u = np.zeros(ms[k])
+            s.score = -1
+            s.kernel_ms = info.kernel_ms
+            s.mc_info = {name: getattr(info, name) for name, _ in _capi.ClpMcInfo._fields_}
+            s.core = cores[k][: ms[k]].copy()
+            out.append(s)
+        if params.verbose and n:
+            i0 = infos[0]
+            print("maxclique batch: %d problems, proven %d, timed out %d | adjacency %.3f ms, peel %.3f ms, "
+                  "heuristic %.3f ms, search %.3f ms, wall %.3f ms"
+                  % (n, sum(infos[k].proven for k in range(n)), sum(infos[k].timed_out for k in range(n)),
+                     i0.adjacency_ms, i0.peel_ms, i0.heuristic_ms, i0.search_ms, 1e3 * i0.t * n))
+        return out
+
+    args = (int(params.method), float(params.time_limit), infos, nodep, corep)
+    return finish, args
+
+
+def graph_to_csc(G):
+    """The graph of a square dense array or scipy sparse matrix as the strictly-upper CSC pattern the C-ABI takes:
+    (m, colptr int64 (m + 1), rowidx int32), rows ascending within a column.  Any nonzero entry above the diagonal is
+    an edge (the rule of maxclique::solve); the diagonal and the lower triangle are ignored."""
+    import scipy.sparse as sp
+    if sp.issparse(G):
+        if len(G.shape) != 2 or G.shape[0] != G.shape[1]:
+            raise ValueError("a graph must be a square matrix, got shape %s" % (G.shape,))
+        S = sp.csc_matrix(G, copy=True)
+        S.sum_duplicates()
+        U = sp.triu(S, k=1, format="csc")
+        U.eliminate_zeros()
+        U.sort_indices()
+        m = G.shape[0]
+        colptr, rowidx = U.indptr.astype(np.int64), U.indices.astype(np.int32)
+    else:
+        A = np.asarray(G)
+        if A.ndim != 2 or A.shape[0] != A.shape[1]:
+            raise ValueError("a graph must be a square matrix, got shape %s" % (A.shape,))
+        m = A.shape[0]
+        cols, rows = np.nonzero(np.triu(A != 0, 1).T)  # column-major order of the upper triangle
+        colptr = np.zeros(m + 1, np.int64)
+        np.cumsum(np.bincount(cols, minlength=m), out=colptr[1:])
+        rowidx = rows.astype(np.int32)
+    if m == 0:
+        raise ValueError("a graph needs at least one vertex")
+    return m, np.ascontiguousarray(colptr), np.ascontiguousarray(rowidx)
+
+
+def maxclique_many(graphs, params=None, device=0):
+    """Maximum clique of every graph of a list in one batched call (clp_batch_max_clique_graphs), the batched
+    counterpart of maxclique::solve(A, params): graphs are square numpy arrays or scipy sparse matrices, any nonzero
+    entry above the diagonal is an edge, m <= 4096 vertices each.  params: MCParams (default: EXACT, 3600 s for the
+    whole call).  Returns one api.Solution per graph (nodes ascending, u = 0, score = -1, mc_info, core)."""
+    graphs = list(graphs)
+    n = len(graphs)
+    if n == 0:
+        return []
+    params = params if params is not None else MCParams()
+    csc = [graph_to_csc(G) for G in graphs]
+    lib = _capi.load()
+    b = C.c_void_p()
+    rc = lib.clp_batch_create(int(device), C.byref(b))
+    if rc != _capi.OK:
+        msg = lib.clp_batch_last_error(None)
+        raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+    try:
+        vp = C.c_void_p
+        m = (C.c_int64 * n)(*[c[0] for c in csc])
+        cpp, rip = (vp * n)(), (vp * n)()
+        for k, (_, cp, ri) in enumerate(csc):
+            cpp[k], rip[k] = cp.ctypes.data, (ri.ctypes.data if ri.size else None)
+        out, args = _mc_outputs([c[0] for c in csc], params)
+        rc = lib.clp_batch_max_clique_graphs(b, n, m, cpp, rip, *args)
+        if rc != _capi.OK:
+            msg = lib.clp_batch_last_error(b)
+            raise _capi.ClipperError(rc, msg.decode() if msg else "")
+        return out()
+    finally:
+        lib.clp_batch_destroy(b)

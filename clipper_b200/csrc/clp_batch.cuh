@@ -114,6 +114,143 @@ __device__ __forceinline__ unsigned int batch_block_exscan(unsigned int x, unsig
   return sc[w] + (inc - x);
 }
 
+// steps 1-2 of a batched problem, shared by batch_solve_kernel and the batched maximum clique (clp_batch_clique.cuh):
+// gather the endpoints of every association, score every pair into the fp32 matrix M (leading dimension ld, the
+// layout of the dense store) and count the kept entries of every row into cnt (shared, rows_pad entries).  An
+// association index out of range sets *error = 2.  Ends with a block barrier.
+template <int KIND, int DD>
+__device__ __forceinline__ void batch_score_pairs(const BatchProblem& P, const double* D1, const double* D2, const int* Aall,
+                                                  double p0, double p1, double p2, double p3, double affinityeps,
+                                                  int* error, double* E1, double* E2, float4* F1, float4* F2, int* Ag,
+                                                  float* M, unsigned int* cnt, unsigned short* queues, float* tiles,
+                                                  float* redf, float& s_R) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int m = P.m;
+  const int ld = (m + 127) / 128 * 128;
+  const int rows_pad = (m + 3) / 4 * 4;
+  // ---- 1. endpoints of every association (gather_endpoints_kernel), fp32 positions, R = max |coordinate|
+  float big = 0.f;
+  int bad = 0;
+  for (int i = tid; i < m; i += kBatchThreads) {
+    int a0, a1;
+    if (P.a_off >= 0) { a0 = Aall[P.a_off + i]; a1 = Aall[P.a_off + m + i]; }
+    else { a0 = i / P.n2; a1 = i % P.n2; }
+    Ag[i] = a0; Ag[m + i] = a1;
+    if (a0 < 0 || a0 >= P.n1 || a1 < 0 || a1 >= P.n2) { bad = 1; a0 = 0; a1 = 0; }
+    float f1[3] = {0.f, 0.f, 0.f}, f2[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int q = 0; q < DD; ++q) {
+      const double x1 = D1[(size_t)a0 * DD + q], x2 = D2[(size_t)a1 * DD + q];
+      E1[(size_t)i * DD + q] = x1; E2[(size_t)i * DD + q] = x2;
+      if (q < 3) {
+        f1[q] = (float)x1; f2[q] = (float)x2;
+        const float m1 = fabsf(f1[q]), m2 = fabsf(f2[q]);
+        big = fmaxf(big, (m1 == m1) ? m1 : __int_as_float(0x7f800000));
+        big = fmaxf(big, (m2 == m2) ? m2 : __int_as_float(0x7f800000));
+      }
+    }
+    F1[i] = make_float4(f1[0], f1[1], f1[2], 0.f);
+    F2[i] = make_float4(f2[0], f2[1], f2[2], 0.f);
+  }
+  if (bad) atomicExch(error, 2);
+  {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) big = fmaxf(big, __shfl_xor_sync(0xffffffffu, big, o));
+    if (lane == 0) redf[warp] = big;
+    __syncthreads();
+    if (tid == 0) { float t = 0.f; for (int w = 0; w < kBatchWarps; ++w) t = fmaxf(t, redf[w]); s_R = t; }
+    __syncthreads();
+  }
+
+  // ---- 2. scoring: warp per row, 128 columns per step; screening + survivor queue as in score_tile_kernel.
+  //      A row's warp evaluates its diagonal block of 128 columns and the blocks to the right of it; an entry kept in
+  //      a block right of the diagonal block is also stored transposed (the pair functions are symmetric bit for bit:
+  //      squared differences and commutative products), so every pair outside the diagonal blocks is evaluated once
+  //      (ref clipper.cpp:31-56 fills the upper triangle and mirrors it).
+  unsigned short* queue = queues + warp * 128;
+  float* tile = tiles + warp * 128;
+  for (int i = tid; i < rows_pad; i += kBatchThreads) cnt[i] = 0u;
+  {
+    const float4 neutral4 = make_float4(-0.0f, -0.0f, -0.0f, -0.0f);
+    for (int i = 128 + warp; i < m; i += kBatchWarps) {  // the blocks left of the diagonal block: transposed stores only
+      const int jd = i & ~127;
+      for (int j = lane * 4; j < jd; j += 128) *reinterpret_cast<float4*>(M + (size_t)i * ld + j) = neutral4;
+    }
+  }
+  __syncthreads();
+  {
+    const float R = s_R;
+    const double eps = p1;  // epsilon (Euclidean) / epsp (PointNormal): the position-consistency bound
+    const float thr = screen_threshold(eps, R);
+    for (int i = warp; i < rows_pad; i += kBatchWarps) {
+      unsigned int kept = 0;
+      if (i < m) {
+        const int ai0 = Ag[i], ai1 = Ag[m + i];
+        const float4 f1i = F1[i], f2i = F2[i];
+        const int jdiag = i & ~127;
+        for (int j0 = jdiag; j0 < ld; j0 += 128) {
+          unsigned int qn = 0;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int j = j0 + lane * 4 + e;
+            tile[lane * 4 + e] = -0.0f;
+            bool cand = false;
+            if (j < m && j != i) {
+              const int aj0 = Ag[j], aj1 = Ag[m + j];
+              const float4 f1j = F1[j], f2j = F2[j];
+              const float x1 = f1i.x - f1j.x, y1 = f1i.y - f1j.y, z1 = f1i.z - f1j.z;
+              const float x2 = f2i.x - f2j.x, y2 = f2i.y - f2j.y, z2 = f2i.z - f2j.z;
+              const float l1 = sqrt_approx(fmaf(z1, z1, fmaf(y1, y1, x1 * x1)));
+              const float l2 = sqrt_approx(fmaf(z2, z2, fmaf(y2, y2, x2 * x2)));
+              cand = ai0 != aj0 && ai1 != aj1 && !(fabsf(l1 - l2) >= thr);  // distinctness: ref clipper.cpp:35-38
+            }
+            const unsigned int vote = __ballot_sync(0xffffffffu, cand);
+            if (cand) queue[qn + __popc(vote & ((1u << lane) - 1u))] = (unsigned short)((e << 5) | lane);
+            qn += __popc(vote);
+          }
+          __syncwarp();
+          for (unsigned int k = lane; k < qn; k += 32) {
+            const unsigned int code = queue[k];
+            const int e = code >> 5, l = code & 31;
+            const int j = j0 + l * 4 + e;
+            double e1i[DD], e2i[DD], e1j[DD], e2j[DD];
+#pragma unroll
+            for (int t = 0; t < DD; ++t) {
+              e1i[t] = E1[(size_t)i * DD + t]; e2i[t] = E2[(size_t)i * DD + t];
+              e1j[t] = E1[(size_t)j * DD + t]; e2j[t] = E2[(size_t)j * DD + t];
+            }
+            double scr;
+            if (KIND == 0) {
+              const double l1 = point_dist<DD>(e1i, e1j, 0), l2 = point_dist<DD>(e2i, e2j, 0);
+              scr = euclid_score(l1, l2, p0, p1, p2);
+            } else {
+              const double l1 = point_dist<3>(e1i, e1j, 0), l2 = point_dist<3>(e2i, e2j, 0);
+              const double dot1 = __dadd_rn(__dadd_rn(__dmul_rn(e1i[3 % DD], e1j[3 % DD]), __dmul_rn(e1i[4 % DD], e1j[4 % DD])), __dmul_rn(e1i[5 % DD], e1j[5 % DD]));
+              const double dot2 = __dadd_rn(__dadd_rn(__dmul_rn(e2i[3 % DD], e2j[3 % DD]), __dmul_rn(e2i[4 % DD], e2j[4 % DD])), __dmul_rn(e2i[5 % DD], e2j[5 % DD]));
+              scr = pointnormal_score(l1, l2, dot1, dot2, p0, p1, p2, p3);
+            }
+            if (keep_score(scr, affinityeps)) {  // ref clipper.cpp:53-64
+              const float enc = encode<float>(scr, true);
+              tile[l * 4 + e] = enc;
+              if (j0 != jdiag) { M[(size_t)j * ld + i] = enc; atomicAdd(&cnt[j], 1u); }
+            }
+          }
+          __syncwarp();
+          const float4 o4 = *reinterpret_cast<const float4*>(tile + lane * 4);
+          *reinterpret_cast<float4*>(M + (size_t)i * ld + j0 + lane * 4) = o4;
+          kept += (is_neutral<float>(o4.x) ? 0u : 1u) + (is_neutral<float>(o4.y) ? 0u : 1u) +
+                  (is_neutral<float>(o4.z) ? 0u : 1u) + (is_neutral<float>(o4.w) ? 0u : 1u);
+          __syncwarp();
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
+      }
+      if (lane == 0 && kept) atomicAdd(&cnt[i], kept);
+    }
+  }
+  __syncthreads();
+}
+
 template <int KIND, int DD>
 __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs ba) {
   extern __shared__ __align__(128) unsigned char clp_batch_smem[];
@@ -151,130 +288,11 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
     const double* D1 = ba.D1 + P.d1_off;
     const double* D2 = ba.D2 + P.d2_off;
 
-    // ---- 1. endpoints of every association (gather_endpoints_kernel), fp32 positions, R = max |coordinate|
-    float big = 0.f;
-    int bad = 0;
-    for (int i = tid; i < m; i += kBatchThreads) {
-      int a0, a1;
-      if (P.a_off >= 0) { a0 = ba.A[P.a_off + i]; a1 = ba.A[P.a_off + m + i]; }
-      else { a0 = i / P.n2; a1 = i % P.n2; }
-      Ag[i] = a0; Ag[m + i] = a1;
-      if (a0 < 0 || a0 >= P.n1 || a1 < 0 || a1 >= P.n2) { bad = 1; a0 = 0; a1 = 0; }
-      float f1[3] = {0.f, 0.f, 0.f}, f2[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-      for (int q = 0; q < DD; ++q) {
-        const double x1 = D1[(size_t)a0 * DD + q], x2 = D2[(size_t)a1 * DD + q];
-        E1[(size_t)i * DD + q] = x1; E2[(size_t)i * DD + q] = x2;
-        if (q < 3) {
-          f1[q] = (float)x1; f2[q] = (float)x2;
-          const float m1 = fabsf(f1[q]), m2 = fabsf(f2[q]);
-          big = fmaxf(big, (m1 == m1) ? m1 : __int_as_float(0x7f800000));
-          big = fmaxf(big, (m2 == m2) ? m2 : __int_as_float(0x7f800000));
-        }
-      }
-      F1[i] = make_float4(f1[0], f1[1], f1[2], 0.f);
-      F2[i] = make_float4(f2[0], f2[1], f2[2], 0.f);
-    }
-    if (bad) atomicExch(&ba.sb->error, 2);
-    {
-      float* redf = reinterpret_cast<float*>(smem + batch_smem_plan(ba.max_m).scan);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) big = fmaxf(big, __shfl_xor_sync(0xffffffffu, big, o));
-      if (lane == 0) redf[warp] = big;
-      __syncthreads();
-      if (tid == 0) { float t = 0.f; for (int w = 0; w < kBatchWarps; ++w) t = fmaxf(t, redf[w]); s_R = t; }
-      __syncthreads();
-    }
-
-    // ---- 2. scoring: warp per row, 128 columns per step; screening + survivor queue as in score_tile_kernel.
-    //      A row's warp evaluates its diagonal block of 128 columns and the blocks to the right of it; an entry kept in
-    //      a block right of the diagonal block is also stored transposed (the pair functions are symmetric bit for bit:
-    //      squared differences and commutative products), so every pair outside the diagonal blocks is evaluated once
-    //      (ref clipper.cpp:31-56 fills the upper triangle and mirrors it).
     const BatchSmem bs = batch_smem_plan(ba.max_m);
     unsigned int* cnt = reinterpret_cast<unsigned int*>(smem + bs.cnt);                          // [rows_pad]
-    unsigned short* queue = reinterpret_cast<unsigned short*>(smem + bs.queue) + warp * 128;
-    float* tile = reinterpret_cast<float*>(smem + bs.tile) + warp * 128;
-    for (int i = tid; i < rows_pad; i += kBatchThreads) cnt[i] = 0u;
-    {
-      const float4 neutral4 = make_float4(-0.0f, -0.0f, -0.0f, -0.0f);
-      for (int i = 128 + warp; i < m; i += kBatchWarps) {  // the blocks left of the diagonal block: transposed stores only
-        const int jd = i & ~127;
-        for (int j = lane * 4; j < jd; j += 128) *reinterpret_cast<float4*>(M + (size_t)i * ld + j) = neutral4;
-      }
-    }
-    __syncthreads();
-    {
-      const float R = s_R;
-      const double eps = ba.p1;  // epsilon (Euclidean) / epsp (PointNormal): the position-consistency bound
-      const float thr = screen_threshold(eps, R);
-      for (int i = warp; i < rows_pad; i += kBatchWarps) {
-        unsigned int kept = 0;
-        if (i < m) {
-          const int ai0 = Ag[i], ai1 = Ag[m + i];
-          const float4 f1i = F1[i], f2i = F2[i];
-          const int jdiag = i & ~127;
-          for (int j0 = jdiag; j0 < ld; j0 += 128) {
-            unsigned int qn = 0;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const int j = j0 + lane * 4 + e;
-              tile[lane * 4 + e] = -0.0f;
-              bool cand = false;
-              if (j < m && j != i) {
-                const int aj0 = Ag[j], aj1 = Ag[m + j];
-                const float4 f1j = F1[j], f2j = F2[j];
-                const float x1 = f1i.x - f1j.x, y1 = f1i.y - f1j.y, z1 = f1i.z - f1j.z;
-                const float x2 = f2i.x - f2j.x, y2 = f2i.y - f2j.y, z2 = f2i.z - f2j.z;
-                const float l1 = sqrt_approx(fmaf(z1, z1, fmaf(y1, y1, x1 * x1)));
-                const float l2 = sqrt_approx(fmaf(z2, z2, fmaf(y2, y2, x2 * x2)));
-                cand = ai0 != aj0 && ai1 != aj1 && !(fabsf(l1 - l2) >= thr);  // distinctness: ref clipper.cpp:35-38
-              }
-              const unsigned int vote = __ballot_sync(0xffffffffu, cand);
-              if (cand) queue[qn + __popc(vote & ((1u << lane) - 1u))] = (unsigned short)((e << 5) | lane);
-              qn += __popc(vote);
-            }
-            __syncwarp();
-            for (unsigned int k = lane; k < qn; k += 32) {
-              const unsigned int code = queue[k];
-              const int e = code >> 5, l = code & 31;
-              const int j = j0 + l * 4 + e;
-              double e1i[DD], e2i[DD], e1j[DD], e2j[DD];
-#pragma unroll
-              for (int t = 0; t < DD; ++t) {
-                e1i[t] = E1[(size_t)i * DD + t]; e2i[t] = E2[(size_t)i * DD + t];
-                e1j[t] = E1[(size_t)j * DD + t]; e2j[t] = E2[(size_t)j * DD + t];
-              }
-              double scr;
-              if (KIND == 0) {
-                const double l1 = point_dist<DD>(e1i, e1j, 0), l2 = point_dist<DD>(e2i, e2j, 0);
-                scr = euclid_score(l1, l2, ba.p0, ba.p1, ba.p2);
-              } else {
-                const double l1 = point_dist<3>(e1i, e1j, 0), l2 = point_dist<3>(e2i, e2j, 0);
-                const double dot1 = __dadd_rn(__dadd_rn(__dmul_rn(e1i[3 % DD], e1j[3 % DD]), __dmul_rn(e1i[4 % DD], e1j[4 % DD])), __dmul_rn(e1i[5 % DD], e1j[5 % DD]));
-                const double dot2 = __dadd_rn(__dadd_rn(__dmul_rn(e2i[3 % DD], e2j[3 % DD]), __dmul_rn(e2i[4 % DD], e2j[4 % DD])), __dmul_rn(e2i[5 % DD], e2j[5 % DD]));
-                scr = pointnormal_score(l1, l2, dot1, dot2, ba.p0, ba.p1, ba.p2, ba.p3);
-              }
-              if (keep_score(scr, ba.affinityeps)) {  // ref clipper.cpp:53-64
-                const float enc = encode<float>(scr, true);
-                tile[l * 4 + e] = enc;
-                if (j0 != jdiag) { M[(size_t)j * ld + i] = enc; atomicAdd(&cnt[j], 1u); }
-              }
-            }
-            __syncwarp();
-            const float4 o4 = *reinterpret_cast<const float4*>(tile + lane * 4);
-            *reinterpret_cast<float4*>(M + (size_t)i * ld + j0 + lane * 4) = o4;
-            kept += (is_neutral<float>(o4.x) ? 0u : 1u) + (is_neutral<float>(o4.y) ? 0u : 1u) +
-                    (is_neutral<float>(o4.z) ? 0u : 1u) + (is_neutral<float>(o4.w) ? 0u : 1u);
-            __syncwarp();
-          }
-#pragma unroll
-          for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
-        }
-        if (lane == 0 && kept) atomicAdd(&cnt[i], kept);
-      }
-    }
-    __syncthreads();
+    batch_score_pairs<KIND, DD>(P, D1, D2, ba.A, ba.p0, ba.p1, ba.p2, ba.p3, ba.affinityeps, &ba.sb->error, E1, E2, F1, F2,
+                                Ag, M, cnt, reinterpret_cast<unsigned short*>(smem + bs.queue),
+                                reinterpret_cast<float*>(smem + bs.tile), reinterpret_cast<float*>(smem + bs.scan), s_R);
 
     const unsigned long long t_scored = global_ns();
     // ---- 3. full-row sliced-ELL copy: sort rows by length (longest first), items of four, scan, fill

@@ -5,6 +5,7 @@
 // solve call launches the sm_90a kernels of clp_kernels.cuh or fails with an error code.
 #include "clp_kernels.cuh"
 #include "clp_clique.cuh"
+#include "clp_batch_clique.cuh"
 #include "clp_host_utils.h"
 #include "../../include/clipper_b200.h"
 
@@ -1708,6 +1709,8 @@ struct clp_batch_s {
   std::string err;
   int sm_count = 0, smem_optin = 0;
   DevBuf in_d1, in_d2, in_a, in_u0, out_u, probs, outs, nnz, sync, scratch, prof;
+  // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
+  DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
   int prof_on = env_int("CLP_PROF_BATCH", 0);
   void* pinned = nullptr; size_t pinned_cap = 0;
   int last_ctas = 0; long long last_scratch = 0, last_nnz = 0;
@@ -1892,6 +1895,326 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const double* cons
   for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
   return CLP_OK;
 }
+
+// ---- batched maximum clique (clp_batch_clique.cuh) ----------------------------------------------------------------
+// kind 0 / 1: scored problems (EuclideanDistance d = 2, 3 / PointNormalDistance); kind 2: graphs given as strictly-upper
+// CSC patterns.  Phase A, then for EXACT with a positive time limit phases B and C: two host synchronisations.
+struct McBatchInput {
+  const double* const* D1 = nullptr; const int64_t* n1 = nullptr;
+  const double* const* D2 = nullptr; const int64_t* n2 = nullptr;
+  const int32_t* const* A = nullptr; const int64_t* m = nullptr;
+  const int64_t* const* colptr = nullptr; const int32_t* const* rowidx = nullptr;
+  double p[4] = {0.0, 0.0, 0.0, 0.0};
+};
+
+const void* mcb_prepare_fn(int kind, int dd) {
+  if (kind == kMcbKindGraph) return (const void*)mc_batch_prepare_kernel<kMcbKindGraph, 1>;
+  if (kind == 1) return (const void*)mc_batch_prepare_kernel<1, 6>;
+  return dd == 3 ? (const void*)mc_batch_prepare_kernel<0, 3> : (const void*)mc_batch_prepare_kernel<0, 2>;
+}
+
+int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatchInput& in, int method, double time_limit_s,
+                     clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  if (!b) return CLP_ERR_INVALID;
+  const auto t_begin = std::chrono::steady_clock::now();
+  if (nprob <= 0 || !infos || !in.m) return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return bfail(b, CLP_ERR_INVALID, "unknown maximum-clique method");
+  const bool graph = kind == kMcbKindGraph;
+  if (graph ? (!in.colptr || !in.rowidx) : (!in.D1 || !in.n1 || !in.D2 || !in.n2))
+    return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (!graph && !((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
+    return bfail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
+  const bool search = method == CLP_MC_EXACT && time_limit_s > 0;
+  CLP_BCUDA(b, cudaSetDevice(b->device));
+  // ---- problem table, per-problem regions and the concatenated inputs, validated here
+  std::vector<McBatchProblem> probs((size_t)nprob);
+  long long nd1 = 0, nd2 = 0, na = 0, ne = 0, nadj = 0, nv = 0, nt = 0;
+  int max_m = 1;
+  for (int p = 0; p < nprob; ++p) {
+    McBatchProblem& q = probs[(size_t)p];
+    std::memset(&q, 0, sizeof(q));
+    long long mp = 0;
+    if (graph) {
+      mp = (long long)in.m[p];
+      if (mp <= 0 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 vertices");
+      const int64_t* cp = in.colptr[p];
+      const int32_t* ri = in.rowidx[p];
+      if (!cp || cp[0] != 0) return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr must start at 0");
+      for (long long c = 0; c < mp; ++c) {
+        if (cp[c + 1] < cp[c]) return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr decreases");
+        for (int64_t k = cp[c]; k < cp[c + 1]; ++k)
+          if (!ri || ri[k] < 0 || ri[k] >= c)
+            return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": entry (" + std::to_string(ri ? ri[k] : -1) + ", " +
+                                                  std::to_string(c) + ") is not strictly upper (row < column)");
+      }
+      q.e_off = ne; q.ne = cp[mp];
+      ne += cp[mp];
+    } else {
+      if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return bfail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
+      const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
+      mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
+      if (mp <= 0 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
+      if (!a2a)
+        for (long long i = 0; i < mp; ++i) {
+          const int32_t a0 = in.A[p][i], a1 = in.A[p][mp + i];
+          if (a0 < 0 || a0 >= in.n1[p] || a1 < 0 || a1 >= in.n2[p])
+            return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
+        }
+      q.sp.d1_off = nd1; q.sp.d2_off = nd2; q.sp.a_off = a2a ? -1 : na; q.sp.u_off = 0;
+      q.sp.n1 = (int)in.n1[p]; q.sp.n2 = (int)in.n2[p];
+      nd1 += (long long)dd * in.n1[p]; nd2 += (long long)dd * in.n2[p]; if (!a2a) na += 2 * mp;
+    }
+    q.sp.m = (int)mp;
+    const long long W = (mp + 31) / 32;
+    q.adj_off = nadj; nadj += mp * W;
+    q.v_off = nv; nv += (4 * mp + 1 + 3) & ~3LL;
+    q.t_off = nt; nt += mp + 1;
+    max_m = std::max(max_m, (int)mp);
+  }
+  // ---- inputs through the pinned staging buffer
+  const size_t bytes_in = (size_t)(nd1 + nd2) * 8 + (size_t)(na + 2 * ne) * 4 + (size_t)nprob * sizeof(McBatchProblem) + 64;
+  const size_t bytes_out = (size_t)nv * 4 + (size_t)nprob * (sizeof(McBatchOut) + 3 * 8 + 2 * 4) + 64;
+  const size_t need = std::max(bytes_in, bytes_out) + 4096;
+  if (need > b->pinned_cap) {
+    if (b->pinned) { cudaFreeHost(b->pinned); b->pinned = nullptr; b->pinned_cap = 0; }
+    CLP_BCUDA(b, cudaMallocHost(&b->pinned, need));
+    b->pinned_cap = need;
+  }
+  char* hp = reinterpret_cast<char*>(b->pinned);
+  double* h_d1 = reinterpret_cast<double*>(hp);
+  double* h_d2 = h_d1 + nd1;
+  int32_t* h_a = reinterpret_cast<int32_t*>(h_d2 + nd2);
+  int32_t* h_e = h_a + na;
+  McBatchProblem* h_pr = reinterpret_cast<McBatchProblem*>(reinterpret_cast<char*>(h_e) + (((size_t)(2 * ne) * 4 + 15) & ~(size_t)15));
+  for (int p = 0; p < nprob; ++p) {
+    const McBatchProblem& q = probs[(size_t)p];
+    if (graph) {
+      const int64_t* cp = in.colptr[p];
+      int32_t* e = h_e + 2 * q.e_off;
+      for (int c = 0; c < q.sp.m; ++c)
+        for (int64_t k = cp[c]; k < cp[c + 1]; ++k) { *e++ = in.rowidx[p][k]; *e++ = c; }
+    } else {
+      std::memcpy(h_d1 + q.sp.d1_off, in.D1[p], (size_t)dd * q.sp.n1 * 8);
+      std::memcpy(h_d2 + q.sp.d2_off, in.D2[p], (size_t)dd * q.sp.n2 * 8);
+      if (q.sp.a_off >= 0) std::memcpy(h_a + q.sp.a_off, in.A[p], (size_t)2 * q.sp.m * 4);
+    }
+  }
+  std::memcpy(h_pr, probs.data(), (size_t)nprob * sizeof(McBatchProblem));
+  CLP_BCUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
+  CLP_BCUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
+  CLP_BCUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
+  CLP_BCUDA(b, b->mc_edges.ensure((size_t)ne * 8 + 16));
+  CLP_BCUDA(b, b->mc_probs.ensure((size_t)nprob * sizeof(McBatchProblem)));
+  CLP_BCUDA(b, b->mc_adj.ensure((size_t)nadj * 4 + 16));
+  CLP_BCUDA(b, b->mc_vint.ensure((size_t)nv * 4 + 16));
+  CLP_BCUDA(b, b->mc_tpre.ensure((size_t)nt * 8 + 16));
+  CLP_BCUDA(b, b->mc_out.ensure((size_t)nprob * sizeof(McBatchOut)));
+  if (nd1) CLP_BCUDA(b, cudaMemcpyAsync(b->in_d1.p, h_d1, (size_t)nd1 * 8, cudaMemcpyHostToDevice, b->stream));
+  if (nd2) CLP_BCUDA(b, cudaMemcpyAsync(b->in_d2.p, h_d2, (size_t)nd2 * 8, cudaMemcpyHostToDevice, b->stream));
+  if (na) CLP_BCUDA(b, cudaMemcpyAsync(b->in_a.p, h_a, (size_t)na * 4, cudaMemcpyHostToDevice, b->stream));
+  if (ne) CLP_BCUDA(b, cudaMemcpyAsync(b->mc_edges.p, h_e, (size_t)ne * 8, cudaMemcpyHostToDevice, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(b->mc_probs.p, h_pr, (size_t)nprob * sizeof(McBatchProblem), cudaMemcpyHostToDevice, b->stream));
+  if (graph) CLP_BCUDA(b, cudaMemsetAsync(b->mc_adj.p, 0, (size_t)nadj * 4, b->stream));
+  CLP_BCUDA(b, cudaMemsetAsync(b->mc_out.p, 0, (size_t)nprob * sizeof(McBatchOut), b->stream));
+  CLP_BCUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+
+  // ---- phase A: one CTA per problem, as many CTAs as are co-resident and, for scored problems, fit their scratch
+  const McbSmem sm = mcb_smem_plan(max_m);
+  if ((long long)sm.total > (long long)b->smem_optin) return bfail(b, CLP_ERR_UNSUPPORTED, "batched maximum clique: shared memory plan exceeds the device limit");
+  const void* fn = mcb_prepare_fn(kind, dd);
+  CLP_BCUDA(b, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.total));
+  int occ = 0;
+  CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kBatchThreads, sm.total));
+  if (occ < 1) return bfail(b, CLP_ERR_CUDA, "batched maximum-clique kernel does not fit an SM");
+  long long grid = std::min<long long>(nprob, (long long)occ * b->sm_count);
+  size_t pstride = 0;
+  if (!graph) {
+    pstride = mcb_layout(max_m, dd).total;
+    size_t free_b = 0, total_b = 0;
+    CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
+    const long long by_mem = (long long)((double)(free_b + b->mc_pscratch.cap) * 0.8 / (double)pstride);
+    if (by_mem < 1) return bfail(b, CLP_ERR_ALLOC, "batched maximum clique: not enough device memory for one problem's scoring scratch");
+    grid = std::min(grid, by_mem);
+    CLP_BCUDA(b, b->mc_pscratch.ensure((size_t)grid * pstride));
+  }
+  McBatchArgs ba;
+  std::memset(&ba, 0, sizeof(ba));
+  ba.prob = b->mc_probs.as<McBatchProblem>(); ba.nprob = nprob; ba.run_heu = method != CLP_MC_KCORE ? 1 : 0; ba.build_tasks = search ? 1 : 0;
+  ba.next = reinterpret_cast<int*>(&b->sync.as<SyncBlock>()->counts[0]);
+  ba.adj = b->mc_adj.as<unsigned>(); ba.vint = b->mc_vint.as<int>(); ba.tpre = b->mc_tpre.as<long long>();
+  ba.out = b->mc_out.as<McBatchOut>(); ba.edges = b->mc_edges.as<int>();
+  ba.D1 = b->in_d1.as<double>(); ba.D2 = b->in_d2.as<double>(); ba.A = b->in_a.as<int>();
+  ba.p0 = in.p[0]; ba.p1 = in.p[1]; ba.p2 = in.p[2]; ba.p3 = in.p[3]; ba.affinityeps = b->prm.affinityeps;
+  ba.error = &b->sync.as<SyncBlock>()->error;
+  ba.scratch = b->mc_pscratch.as<unsigned char>(); ba.scratch_stride = pstride; ba.max_m = max_m;
+  McEvents ev;
+  for (cudaEvent_t& x : ev.e) CLP_BCUDA(b, cudaEventCreate(&x));
+  CLP_BCUDA(b, cudaEventRecord(ev.e[0], b->stream));
+  {
+    void* args[] = {&ba};
+    CLP_BCUDA(b, cudaLaunchKernel(fn, dim3((unsigned)grid), dim3(kBatchThreads), args, sm.total, b->stream));
+  }
+  CLP_BCUDA(b, cudaEventRecord(ev.e[1], b->stream));
+  std::vector<McBatchOut> outs((size_t)nprob);
+  SyncBlock h_sb;
+  CLP_BCUDA(b, cudaMemcpyAsync(outs.data(), b->mc_out.p, (size_t)nprob * sizeof(McBatchOut), cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
+  if (h_sb.error == 2) return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
+  b->last_ctas = (int)grid;
+  b->last_scratch = (long long)grid * (long long)pstride;
+
+  // ---- phases B and C: the search over the tasks of every problem, then the replays
+  int* h_v = reinterpret_cast<int*>(hp);
+  unsigned long long* h_best = reinterpret_cast<unsigned long long*>(hp + (((size_t)nv * 4 + 15) & ~(size_t)15));
+  unsigned long long* h_br = h_best + nprob;
+  unsigned long long* h_done = h_br + nprob;
+  int* h_flags = reinterpret_cast<int*>(h_done + nprob);
+  float search_ms = 0.f;
+  long long total = 0;
+  if (search) {
+    std::vector<int> porder;
+    for (int p = 0; p < nprob; ++p) if (outs[(size_t)p].ntasks > 0) porder.push_back(p);
+    std::stable_sort(porder.begin(), porder.end(), [&](int x, int y) { return outs[(size_t)x].ntasks > outs[(size_t)y].ntasks; });
+    // rounds: round k holds task k of the first w problems of porder (those with more than k tasks); equal widths
+    // form one segment
+    std::vector<long long> seg_start, seg_k0;
+    std::vector<int> seg_width;
+    long long k0 = 0;
+    for (int i = (int)porder.size() - 1; i >= 0; --i) {
+      const long long kend = outs[(size_t)porder[(size_t)i]].ntasks;
+      if (kend <= k0) continue;
+      seg_start.push_back(total); seg_k0.push_back(k0); seg_width.push_back(i + 1);
+      total += (kend - k0) * (i + 1);
+      k0 = kend;
+    }
+    seg_start.push_back(total);
+    if (total > 0) {
+      int K = 1;
+      for (int p : porder) K = std::max(K, outs[(size_t)p].K);
+      const int KW = (K + 31) / 32;
+      const unsigned arena_cap = (unsigned)std::min<long long>((long long)K * (K + 1) / 2 + 64, 1ll << 18);
+      const size_t stride = mc_scratch_bytes(K, KW, arena_cap);
+      size_t free_b = 0, total_b = 0;
+      CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
+      const long long want = (long long)b->sm_count * 2 * kMcSearchWarps;
+      long long nworkers = std::min<long long>(want, (long long)((free_b + b->mc_sscratch.cap) / 2 / stride));
+      nworkers = nworkers / kMcSearchWarps * kMcSearchWarps;
+      if (nworkers < kMcSearchWarps) return bfail(b, CLP_ERR_ALLOC, "batched maximum clique EXACT: not enough device memory for the search scratch");
+      CLP_BCUDA(b, b->mc_sscratch.ensure((size_t)nworkers * stride));
+      const int nseg = (int)seg_width.size();
+      // device state: best | branches | done [nprob] 8-byte, next, deadline, flags [2 nprob]; rounds: porder, segments
+      CLP_BCUDA(b, b->mc_state.ensure((size_t)nprob * 3 * 8 + 16 + (size_t)nprob * 8 + 16));
+      CLP_BCUDA(b, b->mc_rounds.ensure((size_t)(nprob + 1) * 4 + (size_t)(2 * nseg + 1) * 8 + (size_t)nseg * 4 + 64));
+      unsigned long long* d_best = b->mc_state.as<unsigned long long>();
+      unsigned long long* d_br = d_best + nprob;
+      unsigned long long* d_done = d_br + nprob;
+      unsigned long long* d_next = d_done + nprob;
+      unsigned long long* d_deadline = d_next + 1;
+      int* d_flags = reinterpret_cast<int*>(d_deadline + 1);
+      long long* d_seg_start = b->mc_rounds.as<long long>();
+      long long* d_seg_k0 = d_seg_start + nseg + 1;
+      int* d_seg_width = reinterpret_cast<int*>(d_seg_k0 + nseg);
+      int* d_porder = d_seg_width + nseg;
+      std::vector<unsigned long long> best0((size_t)nprob);
+      for (int p = 0; p < nprob; ++p) best0[(size_t)p] = mc_key((unsigned)outs[(size_t)p].lb, 0u);
+      CLP_BCUDA(b, cudaMemcpyAsync(d_best, best0.data(), (size_t)nprob * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_BCUDA(b, cudaMemsetAsync(d_br, 0, (size_t)nprob * 2 * 8 + 16 + (size_t)nprob * 8, b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_start, seg_start.data(), seg_start.size() * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_k0, seg_k0.data(), seg_k0.size() * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_width, seg_width.data(), seg_width.size() * 4, cudaMemcpyHostToDevice, b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(d_porder, porder.data(), porder.size() * 4, cudaMemcpyHostToDevice, b->stream));
+      const double left = time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+      const double left_ns = std::max(0.0, left) * 1e9;
+      const unsigned long long limit_ns = left_ns >= 1.8e19 ? ~0ull : (unsigned long long)left_ns;
+      McBatchSearchArgs sa;
+      sa.prob = b->mc_probs.as<McBatchProblem>(); sa.out = b->mc_out.as<McBatchOut>();
+      sa.adj = b->mc_adj.as<unsigned>(); sa.vint = b->mc_vint.as<int>(); sa.tpre = b->mc_tpre.as<long long>();
+      sa.porder = d_porder; sa.seg_start = d_seg_start; sa.seg_k0 = d_seg_k0; sa.seg_width = d_seg_width; sa.nseg = nseg;
+      sa.total = total; sa.K = K; sa.KW = KW; sa.arena_cap = arena_cap;
+      sa.scratch = b->mc_sscratch.as<unsigned char>(); sa.stride = stride;
+      sa.best = d_best; sa.branches = d_br; sa.done = d_done; sa.flags = d_flags; sa.next = d_next; sa.deadline = d_deadline;
+      const size_t ssmem = (size_t)kMcSearchWarps * 2 * KW * sizeof(unsigned);
+      CLP_BCUDA(b, cudaFuncSetAttribute(mc_batch_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+      CLP_BCUDA(b, cudaFuncSetAttribute(mc_batch_replay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+      CLP_BCUDA(b, cudaEventRecord(ev.e[2], b->stream));
+      mc_deadline_kernel<<<1, 1, 0, b->stream>>>(d_deadline, limit_ns);
+      mc_batch_search_kernel<<<(unsigned)(nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, b->stream>>>(sa);
+      CLP_BCUDA(b, cudaGetLastError());
+      const long long rgrid = std::min<long long>(nworkers / kMcSearchWarps, (nprob + kMcSearchWarps - 1) / kMcSearchWarps);
+      mc_batch_replay_kernel<<<(unsigned)rgrid, kMcSearchWarps * 32, ssmem, b->stream>>>(sa, nprob);
+      CLP_BCUDA(b, cudaGetLastError());
+      CLP_BCUDA(b, cudaEventRecord(ev.e[3], b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(h_best, d_best, (size_t)nprob * 3 * 8, cudaMemcpyDeviceToHost, b->stream));
+      CLP_BCUDA(b, cudaMemcpyAsync(h_flags, d_flags, (size_t)nprob * 8, cudaMemcpyDeviceToHost, b->stream));
+      b->last_scratch += (long long)nworkers * (long long)stride;
+    }
+  }
+  CLP_BCUDA(b, cudaMemcpyAsync(h_v, b->mc_vint.p, (size_t)nv * 4, cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
+  if (total > 0) search_ms = mc_elapsed(ev.e[2], ev.e[3]);
+
+  // ---- results per problem
+  const float phase_a_ms = mc_elapsed(ev.e[0], ev.e[1]);
+  double ns_sum[3] = {0.0, 0.0, 0.0};
+  for (const McBatchOut& o : outs) for (int q = 0; q < 3; ++q) ns_sum[q] += (double)o.ns[q];
+  const double ns_all = ns_sum[0] + ns_sum[1] + ns_sum[2];
+  double split[3] = {0.0, 0.0, 0.0};
+  for (int q = 0; q < 3; ++q) split[q] = ns_all > 0 ? phase_a_ms * ns_sum[q] / ns_all : 0.0;
+  std::vector<int32_t> nodes;
+  for (int p = 0; p < nprob; ++p) {
+    const McBatchProblem& q = probs[(size_t)p];
+    const McBatchOut& o = outs[(size_t)p];
+    const int m = q.sp.m;
+    const int* core = h_v + q.v_off;
+    const int* vnodes = core + 3 * m;
+    int lb = 0, proven = 0, timed_out = 0;
+    long long branches = 0;
+    nodes.clear();
+    if (method == CLP_MC_KCORE) {
+      for (int v = 0; v < m; ++v) if (core[v] >= o.max_core) nodes.push_back(v);
+    } else {
+      lb = o.lb;
+      int size = vnodes[m];  // the heuristic's replay, or the search's when it beat the heuristic
+      proven = (lb == o.max_core + 1) ? 1 : 0;
+      if (search && lb < o.max_core + 1) {
+        proven = 1;
+        if (o.ntasks > 0) {
+          const int s = (int)(h_best[p] >> 32);
+          branches = (long long)h_br[p];
+          timed_out = h_done[p] < (unsigned long long)o.ntasks ? 1 : 0;
+          proven = (!timed_out && h_flags[2 * p + 1] == 0) ? 1 : 0;
+          if (s > lb && (size < s || size > m))
+            return bfail(b, CLP_ERR_CUDA, "batched maximum clique: search replay did not reproduce its clique (problem " + std::to_string(p) + ")");
+          if (s <= lb && size != lb) return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+        } else if (size != lb) {
+          return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+        }
+      } else if (size != lb) {
+        return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+      }
+      nodes.assign(vnodes, vnodes + size);
+      std::sort(nodes.begin(), nodes.end());
+    }
+    if (nodes_out && nodes_out[p] && !nodes.empty()) std::memcpy(nodes_out[p], nodes.data(), nodes.size() * sizeof(int32_t));
+    if (core_out && core_out[p]) std::memcpy(core_out[p], core, (size_t)m * sizeof(int32_t));
+    clp_mc_info& info = infos[p];
+    std::memset(&info, 0, sizeof(info));
+    info.n_nodes = (int32_t)nodes.size();
+    info.max_core = o.max_core;
+    info.lower_bound = lb;
+    info.upper_bound = o.max_core + 1;
+    info.proven = proven;
+    info.timed_out = timed_out;
+    info.n_edges = (int64_t)o.n_edges;
+    info.n_branches = branches;
+    info.adjacency_ms = split[0]; info.peel_ms = split[1]; info.heuristic_ms = split[2]; info.search_ms = search_ms;
+    info.kernel_ms = phase_a_ms + search_ms;
+  }
+  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  for (int p = 0; p < nprob; ++p) infos[p].t = wall / nprob;
+  return CLP_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1928,7 +2251,10 @@ int clp_batch_create(int device, clp_batch* out) {
 int clp_batch_destroy(clp_batch b) {
   if (!b) return CLP_OK;
   cudaSetDevice(b->device);
-  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof}) d->release();
+  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof,
+                    &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
+                    &b->mc_pscratch, &b->mc_sscratch})
+    d->release();
   if (b->pinned) cudaFreeHost(b->pinned);
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
@@ -1970,6 +2296,40 @@ int clp_batch_info(clp_batch b, int32_t* n_ctas, int64_t* scratch_bytes, int64_t
   if (scratch_bytes) *scratch_bytes = b->last_scratch;
   if (nnz_upper_total) *nnz_upper_total = b->last_nnz;
   return CLP_OK;
+}
+
+int clp_batch_max_clique_euclidean(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                                   const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                   double sigma, double epsilon, double mindist, int method, double time_limit_s,
+                                   clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  McBatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
+  in.p[0] = sigma; in.p[1] = epsilon; in.p[2] = mindist;
+  try { return batch_max_clique(b, 0, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
+  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
+  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+}
+
+int clp_batch_max_clique_pointnormal(clp_batch b, int32_t nprob, const double* const* D1, const int64_t* n1,
+                                     const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                     double sigp, double epsp, double sign, double epsn, int method, double time_limit_s,
+                                     clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  McBatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
+  in.p[0] = sigp; in.p[1] = epsp; in.p[2] = sign; in.p[3] = epsn;
+  try { return batch_max_clique(b, 1, 6, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
+  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
+  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+}
+
+int clp_batch_max_clique_graphs(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* colptr,
+                                const int32_t* const* rowidx, int method, double time_limit_s, clp_mc_info* infos,
+                                int32_t* const* nodes_out, int32_t* const* core_out) {
+  McBatchInput in;
+  in.m = m; in.colptr = colptr; in.rowidx = rowidx;
+  try { return batch_max_clique(b, kMcbKindGraph, 0, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
+  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
+  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
 }
 
 }  // extern "C"

@@ -130,47 +130,58 @@ __global__ void __launch_bounds__(kMcPeelThreads) mc_peel_kernel(McPeelArgs a) {
 // K += u, P &= N(u).  The largest K wins, ties to the smaller seed.  A seed is skipped when core(v) + 1 < best size and
 // abandoned when |K| + |P| cannot beat the incumbent key: neither can change the winner, whatever the schedule.
 // replay_seed >= 0: one warp re-runs that seed and writes its nodes in the order they were taken.
+// One seed of the heuristic, run by one warp; P is the warp's W-word bitset.  best is the incumbent key: global memory
+// (read through L2) for mc_heu_kernel, shared memory (SHARED_BEST) for the batched path.
+template <bool SHARED_BEST>
+__device__ __forceinline__ unsigned long long mc_load_best(const unsigned long long* best) {
+  return SHARED_BEST ? *(const volatile unsigned long long*)best : __ldcg(best);
+}
+template <bool SHARED_BEST>
+__device__ __forceinline__ void mc_heu_seed(const unsigned* __restrict__ adj, int m, int W, const int* __restrict__ core,
+                                            int v, unsigned long long* best, bool replay, int* nodes_out, unsigned* P) {
+  const int lane = threadIdx.x & 31;
+  if (!replay && core[v] + 1 < (int)(mc_load_best<SHARED_BEST>(best) >> 32)) return;
+  int psize = 0;
+  for (int w = lane; w < W; w += 32) { const unsigned x = adj[(size_t)v * W + w]; P[w] = x; psize += __popc(x); }
+  psize = mc_warp_sum(psize);
+  int ksz = 1;
+  if (replay && lane == 0) nodes_out[0] = v;
+  bool abandoned = false;
+  while (psize > 0) {  // |P| shrinks by at least one per step
+    if (!replay && mc_key((unsigned)(ksz + psize), (unsigned)v) <= mc_load_best<SHARED_BEST>(best)) { abandoned = true; break; }
+    unsigned long long bk = 0ull;
+    for (int w = lane; w < W; w += 32) {
+      unsigned bits = P[w];
+      while (bits) {
+        const int u = w * 32 + __ffs(bits) - 1;
+        bits &= bits - 1u;
+        const unsigned long long c = mc_key((unsigned)core[u], (unsigned)u);
+        bk = c > bk ? c : bk;
+      }
+    }
+    bk = mc_warp_max(bk);
+    const int u = (int)(0xffffffffu - (unsigned)(bk & 0xffffffffull));
+    if (replay && lane == 0) nodes_out[ksz] = u;
+    ++ksz;
+    psize = 0;
+    for (int w = lane; w < W; w += 32) { const unsigned x = P[w] & adj[(size_t)u * W + w]; P[w] = x; psize += __popc(x); }
+    psize = mc_warp_sum(psize);
+  }
+  if (!replay && !abandoned && lane == 0) atomicMax(best, mc_key((unsigned)ksz, (unsigned)v));
+  if (replay && lane == 0) nodes_out[m] = ksz;  // size after the m node slots
+}
+
 __global__ void __launch_bounds__(kMcThreads) mc_heu_kernel(const unsigned* __restrict__ adj, int m, int W,
                                                             const int* __restrict__ core, const int* __restrict__ seeds,
                                                             unsigned long long* best, int replay_seed, int* nodes_out) {
   extern __shared__ unsigned mc_smem[];
-  const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
+  const int wib = threadIdx.x >> 5;
   unsigned* P = mc_smem + (size_t)wib * W;  // word w is only ever touched by lane w % 32
   const bool replay = replay_seed >= 0;
   const int nwarps = gridDim.x * (blockDim.x >> 5);
   const int n = replay ? 1 : m;
-  for (int s = blockIdx.x * (blockDim.x >> 5) + wib; s < n; s += nwarps) {
-    const int v = replay ? replay_seed : seeds[s];
-    if (!replay && core[v] + 1 < (int)(__ldcg(best) >> 32)) continue;
-    int psize = 0;
-    for (int w = lane; w < W; w += 32) { const unsigned x = adj[(size_t)v * W + w]; P[w] = x; psize += __popc(x); }
-    psize = mc_warp_sum(psize);
-    int ksz = 1;
-    if (replay && lane == 0) nodes_out[0] = v;
-    bool abandoned = false;
-    while (psize > 0) {  // |P| shrinks by at least one per step
-      if (!replay && mc_key((unsigned)(ksz + psize), (unsigned)v) <= __ldcg(best)) { abandoned = true; break; }
-      unsigned long long bk = 0ull;
-      for (int w = lane; w < W; w += 32) {
-        unsigned bits = P[w];
-        while (bits) {
-          const int u = w * 32 + __ffs(bits) - 1;
-          bits &= bits - 1u;
-          const unsigned long long c = mc_key((unsigned)core[u], (unsigned)u);
-          bk = c > bk ? c : bk;
-        }
-      }
-      bk = mc_warp_max(bk);
-      const int u = (int)(0xffffffffu - (unsigned)(bk & 0xffffffffull));
-      if (replay && lane == 0) nodes_out[ksz] = u;
-      ++ksz;
-      psize = 0;
-      for (int w = lane; w < W; w += 32) { const unsigned x = P[w] & adj[(size_t)u * W + w]; P[w] = x; psize += __popc(x); }
-      psize = mc_warp_sum(psize);
-    }
-    if (!replay && !abandoned && lane == 0) atomicMax(best, mc_key((unsigned)ksz, (unsigned)v));
-    if (replay && lane == 0) nodes_out[m] = ksz;  // size after the m node slots
-  }
+  for (int s = blockIdx.x * (blockDim.x >> 5) + wib; s < n; s += nwarps)
+    mc_heu_seed<false>(adj, m, W, core, replay ? replay_seed : seeds[s], best, replay, nodes_out, P);
 }
 
 // number of later neighbours (in degeneracy order) of every vertex: the candidate count of a search root

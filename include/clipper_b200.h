@@ -265,6 +265,37 @@ int clp_batch_solve_pointnormal(clp_batch b, int32_t nprob, const double* const*
 /* diagnostics of the last batch: CTAs of the launch, HBM scratch bytes, stored affinities (i<j) over all problems */
 int clp_batch_info(clp_batch b, int32_t* n_ctas, int64_t* scratch_bytes, int64_t* nnz_upper_total);
 
+/* ---- batched maximum clique: many small graphs in a constant number of launches -----------------------------------
+ * Problem p gets exactly what clp_max_clique returns on an fp32 handle holding the same graph (scored from the same
+ * inputs with clp_batch_set_params' affinityeps; rounding plays no part): the same core numbers, max_core, n_edges,
+ * lower and upper bounds, KCORE and HEU nodes, and -- when both are proven -- the same EXACT nodes.  m <= 4096 per
+ * problem; scored problems take the arguments of clp_batch_solve_* (A[p] == NULL: all-to-all).
+ * clp_batch_max_clique_graphs takes problem p's graph as a strictly-upper CSC pattern of m[p] columns (colptr[p]:
+ * m[p] + 1 entries from 0, rowidx[p]: row < column); every listed pair is an edge.
+ * The device work: one CTA per problem builds the adjacency, peels the k-cores, runs the heuristic and lists the
+ * search tasks; for EXACT one launch then searches the tasks of all problems, drawn so that task k of every problem
+ * comes before task k + 1 of any; one warp per improved problem replays its winner.  time_limit_s bounds the whole call
+ * from its start; <= 0 returns the HEU cliques without searching (proven = lower_bound == upper_bound).  A problem
+ * whose tasks all completed is proven whatever happened to the others; one whose tasks did not comes back with its
+ * best clique, proven = 0, timed_out = 1.
+ * infos[p] holds the fields of clp_mc_info for problem p; kernel_ms and the phase times are those of the whole batch
+ * (adjacency_ms, peel_ms and heuristic_ms split the first launch by in-kernel time, search_ms covers the search and the
+ * replays), t the wall-clock time of the call divided by nprob.  nodes_out[p] (m[p] int32, ascending) and core_out[p]
+ * (m[p] int32 core numbers) may be NULL arrays or NULL entries.  CLP_ERR_INVALID: m > 4096, an unknown method, a CSC
+ * entry with row >= column or out of range, association indices out of range.  CLP_ERR_ALLOC: the scratch does not
+ * fit the free device memory. */
+int clp_batch_max_clique_euclidean(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                                   const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                   double sigma, double epsilon, double mindist, int method, double time_limit_s,
+                                   clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
+int clp_batch_max_clique_pointnormal(clp_batch b, int32_t nprob, const double* const* D1, const int64_t* n1,
+                                     const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                     double sigp, double epsp, double sign, double epsn, int method, double time_limit_s,
+                                     clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
+int clp_batch_max_clique_graphs(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* colptr,
+                                const int32_t* const* rowidx, int method, double time_limit_s, clp_mc_info* infos,
+                                int32_t* const* nodes_out, int32_t* const* core_out);
+
 #ifdef __cplusplus
 }
 #endif
