@@ -16,7 +16,7 @@ from . import _capi
 from ._capi import ClipperError, STORE_F32, STORE_F64
 from .api import (CLIPPER, Params, Solution, Rounding, MCMethod, MCParams, SDPParams, invariants, utils, dsd,
                   __version__)
-from .batch import BatchCLIPPER, maxclique_many
+from .batch import BatchCLIPPER, MatrixBatchCLIPPER, maxclique_many
 
 __all__ = ["CLIPPER", "Params", "Solution", "Rounding", "MCMethod", "MCParams", "SDPParams", "invariants", "utils",
-           "dsd", "BatchCLIPPER", "maxclique_many", "ClipperError", "STORE_F32", "STORE_F64", "__version__"]
+           "dsd", "BatchCLIPPER", "MatrixBatchCLIPPER", "maxclique_many", "ClipperError", "STORE_F32", "STORE_F64", "__version__"]

@@ -29,6 +29,7 @@ SYMBOLS = [
     "clp_batch_solve_euclidean", "clp_batch_solve_pointnormal", "clp_batch_info",
     "clp_max_clique", "clp_core_numbers",
     "clp_batch_max_clique_euclidean", "clp_batch_max_clique_pointnormal", "clp_batch_max_clique_graphs",
+    "clp_batch_solve_matrices",
 ]
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 
@@ -137,6 +138,7 @@ def load():
                                             C.POINTER(ClpSolution), pp, pp]
     L.clp_batch_solve_pointnormal.argtypes = [vp, i32, pp, lp, pp, lp, pp, lp, pp, dbl, dbl, dbl, dbl,
                                               C.POINTER(ClpSolution), pp, pp]
+    L.clp_batch_solve_matrices.argtypes = [vp, i32, lp, pp, pp, pp, pp, pp, pp, pp, C.POINTER(ClpSolution), pp, pp]
     L.clp_batch_info.argtypes = [vp, ip, lp, lp]
     L.clp_max_clique.argtypes = [vp, C.c_int, dbl, ip, C.POINTER(ClpMcInfo)]
     L.clp_core_numbers.argtypes = [vp, ip]

@@ -6,6 +6,8 @@ takes the whole list: one CTA per problem scores the pairs, builds the compact c
 synchronisation anywhere; results per problem are those of ``CLIPPER.score_pairwise_consistency`` + ``solve``.
 ``BatchCLIPPER.max_clique_many`` and ``maxclique_many`` solve each problem of such a list as a maximum clique
 (clp_batch_max_clique_*): per problem the answer of ``CLIPPER.solve_as_maximum_clique`` on an fp32 handle.
+``MatrixBatchCLIPPER`` solves problems whose (M, C) the caller gives (clp_batch_solve_matrices): per problem the
+result of ``CLIPPER.set_sparse_matrix_data`` / ``set_matrix_data`` + ``solve`` on an fp32 handle.
 """
 import ctypes as C
 
@@ -165,6 +167,107 @@ class BatchCLIPPER:
             o.prof_ms = (s.prof_matvec_ms, s.prof_combine_ms, s.prof_exchange_ms)
             out.append(o)
         return out
+
+
+def _solutions(sols, n, u0s, us, nodes):
+    """api.Solution per problem from the clp_solution array of a batched solve"""
+    out = []
+    for k in range(n):
+        s = sols[k]
+        o = Solution()
+        o.t, o.ifinal, o.score = s.t, s.ifinal, s.score
+        o.nodes = nodes[k][: s.n_nodes].tolist()
+        o.u0, o.u = u0s[k], us[k]
+        o.d_final, o.n_evals, o.n_matvec, o.n_inner, o.kernel_ms = s.d_final, s.n_evals, s.n_matvec, s.n_inner, s.kernel_ms
+        o.prof_ms = (s.prof_matvec_ms, s.prof_combine_ms, s.prof_exchange_ms)
+        out.append(o)
+    return out
+
+
+def matrices_to_csc(M, C_):
+    """(m, colptrM, rowidxM, valM, colptrC, rowidxC, valC) of one problem, in the form clp_set_sparse_upper and
+    clp_batch_solve_matrices take (colptr int64, rowidx int32, val float64).
+    Dense M and C (square arrays of equal shape) follow set_matrix_data: only the strict upper triangle is read; the
+    entries of M that are non-zero (NaN included) and of C that are non-zero become CSC entries, with C's values kept as
+    given so that the library checks them.  scipy sparse M and C follow set_sparse_matrix_data: CSC with sorted indices,
+    entries on or below the diagonal passed through (the library refuses them)."""
+    import scipy.sparse as sp
+    if sp.issparse(M) != sp.issparse(C_):
+        raise ValueError("M and C must both be dense arrays or both scipy sparse matrices")
+    if sp.issparse(M):
+        if M.shape != C_.shape or len(M.shape) != 2 or M.shape[0] != M.shape[1]:
+            raise ValueError("M and C must be square and of equal shape, got %s and %s" % (M.shape, C_.shape))
+        arrs = []
+        for X in (M, C_):
+            S = sp.csc_matrix(X, dtype=np.float64)   # shares the arrays of a float64 CSC input
+            if not S.has_sorted_indices:
+                S = S.copy(); S.sort_indices()         # never reorders the caller's matrix in place
+            arrs += [np.ascontiguousarray(S.indptr, np.int64), np.ascontiguousarray(S.indices, np.int32),
+                     np.ascontiguousarray(S.data, np.float64)]
+        return (M.shape[0],) + tuple(arrs)
+    Md = np.asarray(_check_f64(M, "M")); Cd = np.asarray(_check_f64(C_, "C"))
+    if Md.shape != Cd.shape or Md.ndim != 2 or Md.shape[0] != Md.shape[1]:
+        raise ValueError("M and C must be square and of equal shape, got %s and %s" % (Md.shape, Cd.shape))
+    m = Md.shape[0]
+    upper = np.triu(np.ones((m, m), bool), 1)
+    arrs = []
+    for X in (Md, Cd):
+        cols, rows = np.nonzero((upper & (X != 0)).T)   # column-major order: rows ascending within a column
+        colptr = np.zeros(m + 1, np.int64)
+        np.cumsum(np.bincount(cols, minlength=m), out=colptr[1:])
+        arrs += [colptr, rows.astype(np.int32), np.ascontiguousarray(X[rows, cols], np.float64)]
+    return (m,) + tuple(arrs)
+
+
+class MatrixBatchCLIPPER:
+    """Many problems given as affinity and constraint matrices, solved in one launch (clp_batch_solve_matrices): the
+    batched form of set_matrix_data / set_sparse_matrix_data + solve, for affinities that do not come from the built-in
+    invariants (a custom PairwiseInvariant, another consistency measure, a matrix read back with get_affinity_matrix).
+    params: Params (rounding NONZERO or DSD_HEU).  The handle keeps its device buffers between calls."""
+
+    def __init__(self, params=None, device=0):
+        self._lib = _capi.load()
+        self._b = C.c_void_p()
+        rc = self._lib.clp_batch_create(int(device), C.byref(self._b))
+        if rc != _capi.OK:
+            msg = self._lib.clp_batch_last_error(None)
+            raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+        self._params = params if params is not None else Params()
+
+    __del__ = BatchCLIPPER.__del__
+    _check = BatchCLIPPER._check
+    info = BatchCLIPPER.info
+
+    def solve_many(self, problems):
+        """problems: sequence of dicts with M and C (both square dense arrays or both scipy sparse matrices, m <= 4096,
+        see matrices_to_csc) and u0 (m,) float64.  Returns the list of api.Solution in input order, as
+        BatchCLIPPER.solve_many fills it."""
+        problems = list(problems)
+        n = len(problems)
+        if n == 0:
+            return []
+        self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
+        vp = C.c_void_p
+        ptrs = [(vp * n)() for _ in range(6)]
+        u0p, up, np_ = (vp * n)(), (vp * n)(), (vp * n)()
+        m = (C.c_int64 * n)()
+        keep, u0s, us, nodes = [], [], [], []
+        for k, p in enumerate(problems):
+            csc = matrices_to_csc(p["M"], p["C"])
+            mk = csc[0]
+            u0 = np.ascontiguousarray(_check_f64(p["u0"], "u0")).reshape(-1)
+            if u0.size != mk:
+                raise ValueError("problem %d: u0 has %d entries, expected %d" % (k, u0.size, mk))
+            uk = np.zeros(mk, np.float64); nk = np.zeros(max(mk, 1), np.int32)
+            keep.append(csc); u0s.append(u0); us.append(uk); nodes.append(nk)
+            m[k] = mk
+            for q in range(6):
+                a = csc[1 + q]
+                ptrs[q][k] = a.ctypes.data if a.size else None
+            u0p[k], up[k], np_[k] = u0.ctypes.data, uk.ctypes.data, nk.ctypes.data
+        sols = (_capi.ClpSolution * n)()
+        self._check(self._lib.clp_batch_solve_matrices(self._b, n, m, *ptrs, u0p, sols, up, np_))
+        return _solutions(sols, n, u0s, us, nodes)
 
 
 def _mc_outputs(ms, params):

@@ -28,24 +28,26 @@ struct BatchProblem {       // device array, one per problem; offsets into the c
   int n1, n2, m, pad_;
 };
 
-// per-CTA scratch in HBM, sized for the largest problem of the batch
+// per-CTA scratch in HBM, sized for the largest problem of the batch.  points = false (matrices given by the caller,
+// clp_batch_matrix.cuh): the endpoint, fp32 position and association regions are empty
 struct BatchLayout {
   size_t E1, E2, F1, F2, A, M, rowid, itemptr, ctafirst, val, idx, vecs, cand, pieces, total;
   int ld_max, rows_pad_max;
 };
 __host__ __device__ inline size_t batch_align(size_t x) { return (x + 255) & ~(size_t)255; }
-__host__ __device__ inline BatchLayout batch_layout(int max_m, int dd) {
+__host__ __device__ inline BatchLayout batch_layout(int max_m, int dd, bool points = true) {
   BatchLayout L;
   const size_t mm = (size_t)max_m;
+  const size_t mp = points ? mm : 0;
   L.ld_max = (int)((mm + 127) / 128 * 128);
   L.rows_pad_max = (int)((mm + 3) / 4 * 4);
   const size_t ni = (size_t)L.rows_pad_max / 4;
   size_t o = 0;
-  L.E1 = o; o = batch_align(o + mm * dd * 8);
-  L.E2 = o; o = batch_align(o + mm * dd * 8);
-  L.F1 = o; o = batch_align(o + mm * 16);
-  L.F2 = o; o = batch_align(o + mm * 16);
-  L.A = o; o = batch_align(o + 2 * mm * 4);
+  L.E1 = o; o = batch_align(o + mp * dd * 8);
+  L.E2 = o; o = batch_align(o + mp * dd * 8);
+  L.F1 = o; o = batch_align(o + mp * 16);
+  L.F2 = o; o = batch_align(o + mp * 16);
+  L.A = o; o = batch_align(o + 2 * mp * 4);
   L.M = o; o = batch_align(o + (size_t)L.rows_pad_max * L.ld_max * 4);
   L.rowid = o; o = batch_align(o + (size_t)L.rows_pad_max * 4);
   L.itemptr = o; o = batch_align(o + (ni + 1) * 4);
@@ -251,6 +253,122 @@ __device__ __forceinline__ void batch_score_pairs(const BatchProblem& P, const d
   __syncthreads();
 }
 
+// steps 3-4 of a batched problem, shared by batch_solve_kernel and batch_matrix_solve_kernel (clp_batch_matrix.cuh): from
+// the fp32 matrix M (leading dimension ld) and the kept entries per row in cnt, build the full-row sliced-ELL copy and
+// run the solver on it.  plain: every kept entry has M > 0 and C = 1 (the sweep may skip the constraint bit).  The
+// kept entries of the problem are added to nnz_out[p]; prof (nullable) gets [t_scored - t_begin, build, solve, total].
+__device__ __forceinline__ void batch_build_solve(int p, int m, int ld, int rows_pad, int NI, long long u_off, int plain,
+                                                  const float* M, unsigned int* rowid, unsigned int* itemptr,
+                                                  unsigned int* ctafirst, float* val, unsigned short* idx, unsigned char* sc,
+                                                  const BatchLayout& L, unsigned char* smem, const BatchSmem& bs,
+                                                  const unsigned int* cnt, unsigned int* nnz_out, const SolverParams& prm,
+                                                  const double* u0, double* u_out, SolverOut* out, SyncBlock* sb,
+                                                  long long spin_limit, unsigned long long* prof, unsigned long long t_begin,
+                                                  unsigned long long t_scored, ResArgs& sa) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  // ---- 3. full-row sliced-ELL copy: sort rows by length (longest first), items of four, scan, fill
+  const int nb = ld / 4 + 2;
+  unsigned int* hist = reinterpret_cast<unsigned int*>(smem + bs.hist);                         // [nb + 1]
+  unsigned int* scs = reinterpret_cast<unsigned int*>(smem + bs.scan);
+  {
+    unsigned int mine = 0;
+    for (int i = tid; i <= nb; i += kBatchThreads) hist[i] = 0u;
+    __syncthreads();
+    for (int r = tid; r < rows_pad; r += kBatchThreads) { mine += cnt[r]; atomicAdd(&hist[min((cnt[r] + 3u) >> 2, (unsigned int)(nb - 1))], 1u); }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+    if (lane == 0 && mine) atomicAdd(&nnz_out[p], mine);
+    __syncthreads();
+    // start of every length class, longest first: exclusive scan of the histogram read backwards
+    const int per = (nb + kBatchThreads - 1) / kBatchThreads;
+    const int r0 = tid * per;
+    unsigned int local = 0;
+    for (int q = 0; q < per; ++q) { const int r = r0 + q; if (r < nb) local += hist[nb - 1 - r]; }
+    unsigned int run = batch_block_exscan(local, scs);
+    for (int q = 0; q < per; ++q) {
+      const int r = r0 + q;
+      if (r < nb) { const unsigned int hc = hist[nb - 1 - r]; hist[nb - 1 - r] = run; run += hc; }
+    }
+    __syncthreads();
+    // stable placement, as in sell_sort_kernel: tiles of 256 rows in row order, the warps take turns
+    for (int base = 0; base < rows_pad; base += kBatchThreads) {
+      const int r = base + tid;
+      const bool have = r < rows_pad;
+      const unsigned int cls = have ? min((cnt[r] + 3u) >> 2, (unsigned int)(nb - 1)) : 0xffffffffu;
+      const unsigned int peers = __match_any_sync(0xffffffffu, cls);
+      const int leader = __ffs(peers) - 1;
+      const unsigned int before = __popc(peers & ((1u << lane) - 1u));
+      unsigned int start = 0u;
+      for (int w = 0; w < kBatchWarps; ++w) {
+        if (warp == w && have && lane == leader) { start = hist[cls]; hist[cls] = start + __popc(peers); }
+        __syncthreads();
+      }
+      start = __shfl_sync(0xffffffffu, start, leader);
+      if (have) rowid[start + before] = (unsigned int)r;
+    }
+    __syncthreads();
+    // item lengths (4 x the longest = first member), exclusive scan into itemptr[0..NI]
+    const int peri = (NI + 1 + kBatchThreads - 1) / kBatchThreads;
+    const int i0 = tid * peri;
+    unsigned int loc = 0;
+    for (int q = 0; q < peri; ++q) { const int it = i0 + q; if (it < NI) loc += 4u * ((cnt[rowid[4 * it]] + 3u) >> 2); }
+    unsigned int runi = batch_block_exscan(loc, scs);
+    for (int q = 0; q < peri; ++q) {
+      const int it = i0 + q;
+      if (it <= NI) { itemptr[it] = runi; if (it < NI) runi += 4u * ((cnt[rowid[4 * it]] + 3u) >> 2); }
+    }
+    if (tid == 0) { ctafirst[0] = 0u; ctafirst[1] = (unsigned int)NI; }
+    __syncthreads();
+  }
+  {
+    // item-wise fill by the first kFillWarps warps
+    unsigned char* ringbase = smem + bs.ring;
+    float (*ringv)[4][kRing] = reinterpret_cast<float (*)[4][kRing]>(ringbase);
+    unsigned short (*ringo)[4][kRing] = reinterpret_cast<unsigned short (*)[4][kRing]>(ringbase + (size_t)kFillWarps * 4 * kRing * 4);
+    if (warp < kFillWarps) {
+      for (int it = warp; it < NI; it += kFillWarps) {
+        unsigned int r[4];
+#pragma unroll
+        for (int s_ = 0; s_ < 4; ++s_) r[s_] = rowid[4 * it + s_];
+        sell_fill_item_warp<float>(M, ld, m, 0, m, itemptr[it], itemptr[it + 1], r, val, idx, 0, (unsigned int)m,
+                                   ringv[warp], ringo[warp]);
+      }
+    }
+  }
+  __threadfence_block();
+  __syncthreads();
+
+  // ---- 4. the solver (clp_resident.cuh, SOLO): arguments in shared memory
+  if (tid == 0) {
+    ResArgs a;
+    a.sp.val = val; a.sp.off16 = idx; a.sp.itemptr = itemptr; a.sp.rowid = rowid; a.sp.rows_pad = rows_pad; a.sp.plain = plain;
+    a.sp.cta_first = ctafirst;
+    a.m = m; a.row0 = 0; a.rows = m; a.rows_pad = rows_pad; a.NI = NI; a.G = 1;
+    a.prm = prm;
+    a.u0 = u0 + u_off;
+    a.vecs = reinterpret_cast<double*>(sc + L.vecs);
+    a.cand = reinterpret_cast<double*>(sc + L.cand);
+    a.ll = nullptr;
+    a.mpad = (long long)ld;
+    a.pieces = reinterpret_cast<double*>(sc + L.pieces);
+    a.sb = sb;
+    a.u_final = u_out + u_off;
+    a.out = out + p;
+    a.rank = 0; a.world = 1;
+    for (int r = 0; r < kMaxPeers; ++r) { a.peer_ll[r] = nullptr; a.peer_comm[r] = nullptr; }
+    a.comm = nullptr; a.seq0 = 0; a.spin_limit = spin_limit; a.pieces_cap = 0u; a.state_cap = 0u; a.redll = nullptr; a.prof_cta = nullptr; a.prof_laps = 0;
+    sa = a;
+  }
+  __syncthreads();
+  const unsigned long long t_built = global_ns();
+  res_solve_body<float, kBatchThreads, kBatchU, kBatchD, false, true, /*coherent loads*/ true>(sa, smem);
+  if (prof && tid == 0) {
+    const unsigned long long t_end = global_ns();
+    prof[(size_t)p * 4 + 0] = t_scored - t_begin; prof[(size_t)p * 4 + 1] = t_built - t_scored;
+    prof[(size_t)p * 4 + 2] = t_end - t_built; prof[(size_t)p * 4 + 3] = t_end - t_begin;
+  }
+}
+
 template <int KIND, int DD>
 __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs ba) {
   extern __shared__ __align__(128) unsigned char clp_batch_smem[];
@@ -258,7 +376,7 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
   __shared__ ResArgs sa;
   __shared__ int s_p;
   __shared__ float s_R;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int tid = threadIdx.x;
   const BatchLayout L = batch_layout(ba.max_m, DD);
   unsigned char* sc = ba.scratch + (size_t)blockIdx.x * ba.scratch_stride;
   double* E1 = reinterpret_cast<double*>(sc + L.E1);
@@ -295,107 +413,9 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
                                 reinterpret_cast<float*>(smem + bs.tile), reinterpret_cast<float*>(smem + bs.scan), s_R);
 
     const unsigned long long t_scored = global_ns();
-    // ---- 3. full-row sliced-ELL copy: sort rows by length (longest first), items of four, scan, fill
-    const int nb = ld / 4 + 2;
-    unsigned int* hist = reinterpret_cast<unsigned int*>(smem + bs.hist);                         // [nb + 1]
-    unsigned int* scs = reinterpret_cast<unsigned int*>(smem + bs.scan);
-    {
-      unsigned int mine = 0;
-      for (int i = tid; i <= nb; i += kBatchThreads) hist[i] = 0u;
-      __syncthreads();
-      for (int r = tid; r < rows_pad; r += kBatchThreads) { mine += cnt[r]; atomicAdd(&hist[min((cnt[r] + 3u) >> 2, (unsigned int)(nb - 1))], 1u); }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
-      if (lane == 0 && mine) atomicAdd(&ba.nnz_out[p], mine);
-      __syncthreads();
-      // start of every length class, longest first: exclusive scan of the histogram read backwards
-      const int per = (nb + kBatchThreads - 1) / kBatchThreads;
-      const int r0 = tid * per;
-      unsigned int local = 0;
-      for (int q = 0; q < per; ++q) { const int r = r0 + q; if (r < nb) local += hist[nb - 1 - r]; }
-      unsigned int run = batch_block_exscan(local, scs);
-      for (int q = 0; q < per; ++q) {
-        const int r = r0 + q;
-        if (r < nb) { const unsigned int hc = hist[nb - 1 - r]; hist[nb - 1 - r] = run; run += hc; }
-      }
-      __syncthreads();
-      // stable placement, as in sell_sort_kernel: tiles of 256 rows in row order, the warps take turns
-      for (int base = 0; base < rows_pad; base += kBatchThreads) {
-        const int r = base + tid;
-        const bool have = r < rows_pad;
-        const unsigned int cls = have ? min((cnt[r] + 3u) >> 2, (unsigned int)(nb - 1)) : 0xffffffffu;
-        const unsigned int peers = __match_any_sync(0xffffffffu, cls);
-        const int leader = __ffs(peers) - 1;
-        const unsigned int before = __popc(peers & ((1u << lane) - 1u));
-        unsigned int start = 0u;
-        for (int w = 0; w < kBatchWarps; ++w) {
-          if (warp == w && have && lane == leader) { start = hist[cls]; hist[cls] = start + __popc(peers); }
-          __syncthreads();
-        }
-        start = __shfl_sync(0xffffffffu, start, leader);
-        if (have) rowid[start + before] = (unsigned int)r;
-      }
-      __syncthreads();
-      // item lengths (4 x the longest = first member), exclusive scan into itemptr[0..NI]
-      const int peri = (NI + 1 + kBatchThreads - 1) / kBatchThreads;
-      const int i0 = tid * peri;
-      unsigned int loc = 0;
-      for (int q = 0; q < peri; ++q) { const int it = i0 + q; if (it < NI) loc += 4u * ((cnt[rowid[4 * it]] + 3u) >> 2); }
-      unsigned int runi = batch_block_exscan(loc, scs);
-      for (int q = 0; q < peri; ++q) {
-        const int it = i0 + q;
-        if (it <= NI) { itemptr[it] = runi; if (it < NI) runi += 4u * ((cnt[rowid[4 * it]] + 3u) >> 2); }
-      }
-      if (tid == 0) { ctafirst[0] = 0u; ctafirst[1] = (unsigned int)NI; }
-      __syncthreads();
-    }
-    {
-      // item-wise fill by the first kFillWarps warps
-      unsigned char* ringbase = smem + bs.ring;
-      float (*ringv)[4][kRing] = reinterpret_cast<float (*)[4][kRing]>(ringbase);
-      unsigned short (*ringo)[4][kRing] = reinterpret_cast<unsigned short (*)[4][kRing]>(ringbase + (size_t)kFillWarps * 4 * kRing * 4);
-      if (warp < kFillWarps) {
-        for (int it = warp; it < NI; it += kFillWarps) {
-          unsigned int r[4];
-#pragma unroll
-          for (int s_ = 0; s_ < 4; ++s_) r[s_] = rowid[4 * it + s_];
-          sell_fill_item_warp<float>(M, ld, m, 0, m, itemptr[it], itemptr[it + 1], r, val, idx, 0, (unsigned int)m,
-                                     ringv[warp], ringo[warp]);
-        }
-      }
-    }
-    __threadfence_block();
-    __syncthreads();
-
-    // ---- 4. the solver (clp_resident.cuh, SOLO): arguments in shared memory
-    if (tid == 0) {
-      ResArgs a;
-      a.sp.val = val; a.sp.off16 = idx; a.sp.itemptr = itemptr; a.sp.rowid = rowid; a.sp.rows_pad = rows_pad; a.sp.plain = 1;
-      a.sp.cta_first = ctafirst;
-      a.m = m; a.row0 = 0; a.rows = m; a.rows_pad = rows_pad; a.NI = NI; a.G = 1;
-      a.prm = ba.prm;
-      a.u0 = ba.u0 + P.u_off;
-      a.vecs = reinterpret_cast<double*>(sc + L.vecs);
-      a.cand = reinterpret_cast<double*>(sc + L.cand);
-      a.ll = nullptr;
-      a.mpad = (long long)ld;
-      a.pieces = reinterpret_cast<double*>(sc + L.pieces);
-      a.sb = ba.sb;
-      a.u_final = ba.u_out + P.u_off;
-      a.out = ba.out + p;
-      a.rank = 0; a.world = 1;
-      for (int r = 0; r < kMaxPeers; ++r) { a.peer_ll[r] = nullptr; a.peer_comm[r] = nullptr; }
-      a.comm = nullptr; a.seq0 = 0; a.spin_limit = ba.spin_limit; a.pieces_cap = 0u; a.state_cap = 0u; a.redll = nullptr; a.prof_cta = nullptr; a.prof_laps = 0;
-      sa = a;
-    }
-    __syncthreads();
-    const unsigned long long t_built = global_ns();
-    res_solve_body<float, kBatchThreads, kBatchU, kBatchD, false, true, /*coherent loads*/ true>(sa, smem);
-    if (ba.prof && tid == 0) {
-      const unsigned long long t_end = global_ns();
-      ba.prof[(size_t)p * 4 + 0] = t_scored - t_begin; ba.prof[(size_t)p * 4 + 1] = t_built - t_scored;
-      ba.prof[(size_t)p * 4 + 2] = t_end - t_built; ba.prof[(size_t)p * 4 + 3] = t_end - t_begin;
-    }
+    batch_build_solve(p, m, ld, rows_pad, NI, P.u_off, /*plain: every scored entry has M > 0 and C = 1*/ 1, M, rowid, itemptr,
+                      ctafirst, val, idx, sc, L, smem, bs, cnt, ba.nnz_out, ba.prm, ba.u0, ba.u_out, ba.out, ba.sb,
+                      ba.spin_limit, ba.prof, t_begin, t_scored, sa);
   }
 }
 

@@ -6,6 +6,7 @@
 #include "clp_kernels.cuh"
 #include "clp_clique.cuh"
 #include "clp_batch_clique.cuh"
+#include "clp_batch_matrix.cuh"
 #include "clp_host_utils.h"
 #include "../../include/clipper_b200.h"
 
@@ -17,6 +18,7 @@
 #include <cstring>
 #include <random>
 #include <string>
+#include <thread>
 #include <vector>
 #include <unistd.h>
 
@@ -1704,11 +1706,12 @@ int clp_set_dense_mode(clp_handle h, int mode) {
 struct clp_batch_s {
   int device = 0;
   cudaStream_t stream = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_up = nullptr;
   clp_params prm;
   std::string err;
   int sm_count = 0, smem_optin = 0;
   DevBuf in_d1, in_d2, in_a, in_u0, out_u, probs, outs, nnz, sync, scratch, prof;
+  DevBuf mat_in;  // batched matrices: column pointers | values | u0 | row indices | problem table
   // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
   DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
   int prof_on = env_int("CLP_PROF_BATCH", 0);
@@ -1742,6 +1745,38 @@ int batch_occupancy(clp_batch b, size_t smem, int* occ) {
   CLP_BCUDA(b, cudaFuncSetAttribute(batch_solve_kernel<KIND, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, batch_solve_kernel<KIND, DD>, kBatchThreads, smem));
   return CLP_OK;
+}
+
+// per-problem results of a batched solve: rounding (NONZERO or DSD_HEU) and the outputs of clp_batch_solve_*.
+// Prob: BatchProblem or BatchMatProblem (m, u_off).  sols[p].t is left to the caller.
+template <typename Prob>
+void batch_results(const clp_params& P, const std::vector<Prob>& probs, const double* h_u, const SolverOut* h_out, float ms,
+                   clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
+  std::vector<int32_t> nodes;
+  for (int p = 0; p < (int)probs.size(); ++p) {
+    const Prob& q = probs[(size_t)p];
+    const SolverOut& so = h_out[p];
+    const double* u = h_u + q.u_off;
+    nodes.clear();
+    if (P.rounding == CLP_ROUND_NONZERO) {
+      nodes.resize((size_t)q.m);
+      nodes.resize((size_t)clp_find_above(u, q.m, 0.0, nodes.data()));
+    } else {  // DSD_HEU, ref clipper.cpp:302-308
+      const int omega = (int)std::round(so.F);
+      if (omega >= 1) {
+        nodes.resize((size_t)std::min<long long>(omega, q.m));
+        nodes.resize((size_t)clp_find_k_largest(u, q.m, omega, nodes.data()));
+      }
+    }
+    clp_solution& s = sols[p];
+    std::memset(&s, 0, sizeof(s));
+    s.ifinal = so.ifinal; s.n_nodes = (int32_t)nodes.size(); s.score = so.F; s.d_final = so.d;
+    s.n_evals = so.n_evals; s.n_matvec = so.n_matvec; s.n_inner = so.n_inner; s.kernel_ms = ms;
+    s.prof_matvec_ms = 1e-6 * (double)so.ns_matvec; s.prof_combine_ms = 1e-6 * (double)so.ns_combine;
+    s.prof_exchange_ms = 1e-6 * (double)so.ns_exchange;
+    if (u_out && u_out[p]) std::memcpy(u_out[p], u, (size_t)q.m * 8);
+    if (nodes_out && nodes_out[p] && !nodes.empty()) std::memcpy(nodes_out[p], nodes.data(), nodes.size() * 4);
+  }
 }
 
 int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const double* const* D1, const int64_t* n1,
@@ -1865,32 +1900,207 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const double* cons
   if (h_sb.error == 2) return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
   if (h_sb.error != 0) return bfail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
   b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)L.total; b->last_nnz = 0;
-  std::vector<int32_t> nodes;
-  for (int p = 0; p < nprob; ++p) {
-    const BatchProblem& q = probs[(size_t)p];
-    const SolverOut& so = h_out[p];
-    const double* u = h_u + q.u_off;
-    b->last_nnz += h_nnz[p] / 2;
-    nodes.clear();
-    if (P.rounding == CLP_ROUND_NONZERO) {
-      nodes.resize((size_t)q.m);
-      nodes.resize((size_t)clp_find_above(u, q.m, 0.0, nodes.data()));
-    } else {  // DSD_HEU, ref clipper.cpp:302-308
-      const int omega = (int)std::round(so.F);
-      if (omega >= 1) {
-        nodes.resize((size_t)std::min<long long>(omega, q.m));
-        nodes.resize((size_t)clp_find_k_largest(u, q.m, omega, nodes.data()));
+  for (int p = 0; p < nprob; ++p) b->last_nnz += h_nnz[p] / 2;
+  batch_results(P, probs, h_u, h_out, ms, sols, u_out, nodes_out);
+  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
+  return CLP_OK;
+}
+
+// ---- batched solve of given matrices (clp_batch_matrix.cuh) -------------------------------------------------------
+// Problem p: strictly-upper CSC M and C of m[p] columns, as clp_set_sparse_upper takes them.  Validated on the host with
+// that call's predicates while the entries are copied into the pinned staging buffer; the error of the whole call is
+// the first structural error of any problem (CLP_ERR_INVALID), else the first negative affinity, else the first
+// constraint value outside {0, 1} (CLP_ERR_UNSUPPORTED): the single path's order, flag 4 before 1 before 2.
+struct MatCheck { int kind = -1; std::string msg; };  // kind 0: structure, 1: M value, 2: C value
+
+// validate one CSC matrix of problem p and copy its row indices and values to ri_dst / v_dst; sets chk on the first
+// problem found (structure errors replace a value error found earlier)
+void mat_check_copy(int p, const char* what, int which, long long m, const int64_t* cp, const int32_t* ri, const double* v,
+                    int32_t* ri_dst, double* v_dst, MatCheck& chk) {
+  const std::string tag = "problem " + std::to_string(p) + ", " + what + ": ";
+  for (long long c = 0; c < m; ++c) {
+    long long prev = -1;
+    for (int64_t k = cp[c]; k < cp[c + 1]; ++k) {
+      const int32_t r = ri[k];
+      if (r < 0 || r >= c) {
+        chk.kind = 0;
+        chk.msg = tag + "entry (" + std::to_string(r) + ", " + std::to_string(c) + ") is not strictly upper triangular (row < column)";
+        return;
       }
+      if (r <= prev) {
+        chk.kind = 0;
+        chk.msg = tag + "rows of column " + std::to_string(c) + " are not strictly ascending (row " + std::to_string(r) + ")";
+        return;
+      }
+      prev = r;
+      const double x = v[k];
+      if (chk.kind < 0 && (which == 0 ? (x < 0.0) : (x != 0.0 && x != 1.0))) {
+        chk.kind = which + 1;
+        chk.msg = tag + (which == 0 ? "affinity matrix has negative entries" : "constraint matrix is not binary");
+      }
+      ri_dst[k] = r; v_dst[k] = x;
     }
-    clp_solution& s = sols[p];
-    std::memset(&s, 0, sizeof(s));
-    s.ifinal = so.ifinal; s.n_nodes = (int32_t)nodes.size(); s.score = so.F; s.d_final = so.d;
-    s.n_evals = so.n_evals; s.n_matvec = so.n_matvec; s.n_inner = so.n_inner; s.kernel_ms = ms;
-    s.prof_matvec_ms = 1e-6 * (double)so.ns_matvec; s.prof_combine_ms = 1e-6 * (double)so.ns_combine;
-    s.prof_exchange_ms = 1e-6 * (double)so.ns_exchange;
-    if (u_out && u_out[p]) std::memcpy(u_out[p], u, (size_t)q.m * 8);
-    if (nodes_out && nodes_out[p] && !nodes.empty()) std::memcpy(nodes_out[p], nodes.data(), nodes.size() * 4);
   }
+}
+
+int batch_launch_matrices(clp_batch b, BatchMatArgs& ba, int grid, size_t smem) {
+  CLP_BCUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  batch_matrix_solve_kernel<<<grid, kBatchThreads, smem, b->stream>>>(ba);
+  CLP_BCUDA(b, cudaGetLastError());
+  return CLP_OK;
+}
+
+int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* cpM, const int32_t* const* riM,
+                         const double* const* vM, const int64_t* const* cpC, const int32_t* const* riC,
+                         const double* const* vC, const double* const* u0, clp_solution* sols, double* const* u_out,
+                         int32_t* const* nodes_out) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC || !u0 || !sols) return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
+  const clp_params& P = b->prm;
+  if (P.rounding == CLP_ROUND_DSD) return bfail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
+  if (P.maxlsiters < 1) return bfail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
+  const auto t_begin = std::chrono::steady_clock::now();
+  CLP_BCUDA(b, cudaSetDevice(b->device));
+  // ---- problem table: sizes and column pointers (the entries are checked while they are copied)
+  std::vector<BatchMatProblem> probs((size_t)nprob);
+  long long ncp = 0, ne = 0, nu = 0;
+  int max_m = 1;
+  for (int p = 0; p < nprob; ++p) {
+    BatchMatProblem& q = probs[(size_t)p];
+    const std::string tag = "problem " + std::to_string(p) + ": ";
+    const long long mp = (long long)m[p];
+    if (mp < 1 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, tag + "batched problems need 1 <= m <= 4096");
+    if (!u0[p]) return bfail(b, CLP_ERR_INVALID, tag + "null u0");
+    long long nz[2] = {0, 0};
+    for (int which = 0; which < 2; ++which) {
+      const int64_t* cp = which ? cpC[p] : cpM[p];
+      const char* what = which ? "C" : "M";
+      if (!cp || cp[0] != 0) return bfail(b, CLP_ERR_INVALID, tag + what + " column pointer must start at 0");
+      for (long long c = 0; c < mp; ++c)
+        if (cp[c + 1] < cp[c]) return bfail(b, CLP_ERR_INVALID, tag + what + " column pointer decreases at column " + std::to_string(c));
+      nz[which] = cp[mp];
+      if (nz[which] > 0 && (which ? (!riC[p] || !vC[p]) : (!riM[p] || !vM[p])))
+        return bfail(b, CLP_ERR_INVALID, tag + what + " has entries but null row indices or values");
+    }
+    q.cpM_off = ncp; q.cpC_off = ncp + mp + 1; ncp += 2 * (mp + 1);
+    q.eM_off = ne; q.eC_off = ne + nz[0]; ne += nz[0] + nz[1];
+    q.u_off = nu; nu += (mp + 1) & ~1LL;  // 16-byte aligned u0 / u slots (the kernels use 16-byte loads)
+    q.m = (int)mp; q.pad_ = 0;
+    max_m = std::max(max_m, (int)mp);
+  }
+  // ---- staging: column pointers | values | u0 | row indices | problem table, one upload
+  const size_t o_val = (size_t)ncp * 8, o_u0 = (o_val + (size_t)ne * 8 + 15) & ~(size_t)15, o_ri = o_u0 + (size_t)nu * 8;
+  const size_t o_pr = (o_ri + (size_t)ne * 4 + 15) & ~(size_t)15;
+  const size_t bytes_in = o_pr + (size_t)nprob * sizeof(BatchMatProblem);
+  const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
+  const size_t need = std::max(bytes_in, bytes_out) + 4096;
+  if (need > b->pinned_cap) {
+    if (b->pinned) { cudaFreeHost(b->pinned); b->pinned = nullptr; b->pinned_cap = 0; }
+    CLP_BCUDA(b, cudaMallocHost(&b->pinned, need));
+    b->pinned_cap = need;
+  }
+  char* hp = reinterpret_cast<char*>(b->pinned);
+  int64_t* h_cp = reinterpret_cast<int64_t*>(hp);
+  double* h_val = reinterpret_cast<double*>(hp + o_val);
+  double* h_u0 = reinterpret_cast<double*>(hp + o_u0);
+  int32_t* h_ri = reinterpret_cast<int32_t*>(hp + o_ri);
+  // validate and copy, problems spread over host threads; the verdict does not depend on the split
+  std::vector<MatCheck> chk((size_t)nprob);
+  auto work = [&](int p0, int p1) {
+    for (int p = p0; p < p1; ++p) {
+      const BatchMatProblem& q = probs[(size_t)p];
+      std::memcpy(h_cp + q.cpM_off, cpM[p], (size_t)(q.m + 1) * 8);
+      std::memcpy(h_cp + q.cpC_off, cpC[p], (size_t)(q.m + 1) * 8);
+      std::memcpy(h_u0 + q.u_off, u0[p], (size_t)q.m * 8);
+      MatCheck cm, cc;
+      mat_check_copy(p, "M", 0, q.m, cpM[p], riM[p], vM[p], h_ri + q.eM_off, h_val + q.eM_off, cm);
+      if (cm.kind != 0) mat_check_copy(p, "C", 1, q.m, cpC[p], riC[p], vC[p], h_ri + q.eC_off, h_val + q.eC_off, cc);
+      chk[(size_t)p] = (cm.kind == 0 || cc.kind == 0) ? (cm.kind == 0 ? cm : cc) : (cm.kind >= 0 ? cm : cc);
+    }
+  };
+  {
+    const unsigned hw = std::max(1u, std::min(16u, std::thread::hardware_concurrency()));
+    const int nth = (int)std::min<long long>(hw, std::max<long long>(1, ne / (1 << 20)));  // ~1M entries per thread at least
+    if (nth <= 1 || nprob == 1) work(0, nprob);
+    else {
+      std::vector<std::thread> th;
+      for (int t = 0; t < nth; ++t) th.emplace_back(work, (int)((long long)nprob * t / nth), (int)((long long)nprob * (t + 1) / nth));
+      for (std::thread& x : th) x.join();
+    }
+  }
+  for (int kind = 0; kind < 3; ++kind)
+    for (int p = 0; p < nprob; ++p)
+      if (chk[(size_t)p].kind == kind) return bfail(b, kind == 0 ? CLP_ERR_INVALID : CLP_ERR_UNSUPPORTED, chk[(size_t)p].msg);
+  std::memcpy(hp + o_pr, probs.data(), (size_t)nprob * sizeof(BatchMatProblem));
+  // the device copy keeps the staging offsets (u0 starts on a 16-byte boundary, the base is cudaMalloc-aligned)
+  CLP_BCUDA(b, b->mat_in.ensure(bytes_in + 16));
+  CLP_BCUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
+  CLP_BCUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
+  CLP_BCUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
+  CLP_BCUDA(b, cudaEventRecord(b->ev_up, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(b->mat_in.p, hp, bytes_in, cudaMemcpyHostToDevice, b->stream));
+  CLP_BCUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
+  CLP_BCUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
+  CLP_BCUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  // ---- grid: as many CTAs as are co-resident (and as there are problems), each with its own scratch slot
+  const BatchSmem bs = batch_smem_plan(max_m);
+  if ((long long)bs.total > (long long)b->smem_optin) return bfail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
+  int occ = 0;
+  CLP_BCUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs.total));
+  CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, batch_matrix_solve_kernel, kBatchThreads, bs.total));
+  if (occ < 1) return bfail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
+  const BatchLayout L = batch_layout(max_m, 0, /*points*/ false);
+  size_t free_b = 0, total_b = 0;
+  CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
+  const long long by_mem = (long long)((double)(free_b + b->scratch.cap) * 0.8 / (double)L.total);
+  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(nprob, (long long)occ * b->sm_count), by_mem));
+  CLP_BCUDA(b, b->scratch.ensure((size_t)grid * L.total));
+  const char* din = b->mat_in.as<char>();
+  BatchMatArgs ba;
+  std::memset(&ba, 0, sizeof(ba));
+  ba.prob = reinterpret_cast<const BatchMatProblem*>(din + o_pr); ba.nprob = nprob;
+  ba.colptr = reinterpret_cast<const long long*>(din); ba.val = reinterpret_cast<const double*>(din + o_val);
+  ba.u0 = reinterpret_cast<const double*>(din + o_u0); ba.rowidx = reinterpret_cast<const int*>(din + o_ri);
+  ba.u_out = b->out_u.as<double>(); ba.out = b->outs.as<SolverOut>(); ba.nnz_out = b->nnz.as<unsigned int>();
+  ba.next = reinterpret_cast<int*>(&b->sync.as<SyncBlock>()->counts[0]);
+  ba.scratch = b->scratch.as<unsigned char>(); ba.scratch_stride = L.total;
+  ba.max_m = max_m;
+  ba.prm.tol_u = P.tol_u; ba.prm.tol_F = P.tol_F; ba.prm.beta = P.beta; ba.prm.eps = P.eps;
+  ba.prm.maxiniters = P.maxiniters; ba.prm.maxoliters = P.maxoliters; ba.prm.maxlsiters = P.maxlsiters;
+  ba.prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
+  ba.sb = b->sync.as<SyncBlock>(); ba.spin_limit = 4LL * 1900000000LL;
+  if (b->prof_on) { CLP_BCUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  CLP_BCUDA(b, cudaEventRecord(b->ev0, b->stream));
+  if (int rc = batch_launch_matrices(b, ba, grid, bs.total)) return rc;
+  CLP_BCUDA(b, cudaEventRecord(b->ev1, b->stream));
+  // ---- results
+  double* h_u = reinterpret_cast<double*>(hp);
+  SolverOut* h_out = reinterpret_cast<SolverOut*>(h_u + nu);
+  unsigned int* h_nnz = reinterpret_cast<unsigned int*>(h_out + nprob);
+  SyncBlock h_sb;
+  CLP_BCUDA(b, cudaMemcpyAsync(h_u, b->out_u.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(h_out, b->outs.p, (size_t)nprob * sizeof(SolverOut), cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(h_nnz, b->nnz.p, (size_t)nprob * 4, cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
+  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
+  float ms = 0.f, up_ms = 0.f;
+  CLP_BCUDA(b, cudaEventElapsedTime(&ms, b->ev0, b->ev1));
+  CLP_BCUDA(b, cudaEventElapsedTime(&up_ms, b->ev_up, b->ev0));
+  if (b->prof_on) {
+    std::vector<unsigned long long> pr((size_t)nprob * 4);
+    CLP_BCUDA(b, cudaMemcpy(pr.data(), b->prof.p, pr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    double acc[4] = {0, 0, 0, 0};
+    for (int p = 0; p < nprob; ++p) for (int q = 0; q < 4; ++q) acc[q] += 1e-6 * (double)pr[(size_t)p * 4 + q];
+    std::fprintf(stderr, "[clp batch matrices prof] %d problems (max m %d), %d CTAs, upload %zu bytes %.3f ms, kernel %.3f ms; "
+                 "mean per problem: scatter %.3f  build %.3f  solve %.3f  total %.3f ms\n",
+                 nprob, max_m, grid, bytes_in, up_ms, ms, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
+  }
+  if (h_sb.flags != 0) return bfail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
+  if (h_sb.error != 0) return bfail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
+  b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)L.total; b->last_nnz = 0;
+  for (int p = 0; p < nprob; ++p) b->last_nnz += h_nnz[p] / 2;
+  batch_results(P, probs, h_u, h_out, ms, sols, u_out, nodes_out);
   const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
   for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
   return CLP_OK;
@@ -2242,6 +2452,7 @@ int clp_batch_create(int device, clp_batch* out) {
   if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
   if ((e = cudaEventCreate(&b->ev0)) != cudaSuccess) return bail("cudaEventCreate", e);
   if ((e = cudaEventCreate(&b->ev1)) != cudaSuccess) return bail("cudaEventCreate", e);
+  if ((e = cudaEventCreate(&b->ev_up)) != cudaSuccess) return bail("cudaEventCreate", e);
   if ((e = b->sync.ensure(sizeof(SyncBlock))) != cudaSuccess) return bail("cudaMalloc", e);
   if ((e = cudaDeviceGetAttribute(&b->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device)) != cudaSuccess) return bail("cudaDeviceGetAttribute", e);
   *out = b;
@@ -2251,13 +2462,14 @@ int clp_batch_create(int device, clp_batch* out) {
 int clp_batch_destroy(clp_batch b) {
   if (!b) return CLP_OK;
   cudaSetDevice(b->device);
-  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof,
+  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in,
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
                     &b->mc_pscratch, &b->mc_sscratch})
     d->release();
   if (b->pinned) cudaFreeHost(b->pinned);
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
+  if (b->ev_up) cudaEventDestroy(b->ev_up);
   if (b->stream) cudaStreamDestroy(b->stream);
   delete b;
   return CLP_OK;
@@ -2286,6 +2498,15 @@ int clp_batch_solve_pointnormal(clp_batch b, int32_t nprob, const double* const*
                                 const double* const* u0, double sigp, double epsp, double sign, double epsn,
                                 clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
   try { return batch_solve(b, 1, 6, nprob, D1, n1, D2, n2, A, m, u0, sigp, epsp, sign, epsn, sols, u_out, nodes_out); }
+  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
+  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+}
+
+int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
+                             const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
+                             const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
+                             const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
+  try { return batch_solve_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, u0, sols, u_out, nodes_out); }
   catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
   catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
 }

@@ -1364,33 +1364,39 @@ __global__ void encode_dense_panel_kernel(const double* Mp, const double* Cp, in
 
 // strictly-upper CSC -> HBM layout.  pass 0: M values (sign cleared => C=1 provisional is wrong),
 // so the host runs: fill neutral; pass A writes |M| with C=0 (negative sign); pass B sets C bits.
+// The per-entry bodies are shared with the batched matrix path (clp_batch_matrix.cuh): the storage rule of a CSC
+// entry (i, j) lives here only.
+template <typename T>
+__device__ __forceinline__ void scatter_csc_M_entry(int i, int j, const double* vq, T* M, long long ld, int row0, int rows, int* flags) {
+  if (i < 0 || i >= j) { atomicOr(flags, 4); return; }
+  const double v = *vq;
+  if (v < 0.0) atomicOr(flags, 1);
+  const T e = encode<T>(v, false);
+  if (i >= row0 && i < row0 + rows) M[(size_t)(i - row0) * ld + j] = e;
+  if (j >= row0 && j < row0 + rows) M[(size_t)(j - row0) * ld + i] = e;
+}
+template <typename T>
+__device__ __forceinline__ void scatter_csc_C_entry(int i, int j, const double* vq, T* M, long long ld, int row0, int rows, int* flags) {
+  if (i < 0 || i >= j) { atomicOr(flags, 4); return; }
+  const double v = *vq;
+  if (v == 0.0) return;
+  if (v != 1.0) atomicOr(flags, 2);
+  if (i >= row0 && i < row0 + rows) { T* p = M + (size_t)(i - row0) * ld + j; double a; bool c; decode(*p, a, c); *p = encode<T>(a, true); }
+  if (j >= row0 && j < row0 + rows) { T* p = M + (size_t)(j - row0) * ld + i; double a; bool c; decode(*p, a, c); *p = encode<T>(a, true); }
+}
 template <typename T>
 __global__ void scatter_csc_M_kernel(const long long* colptr, const int* rowidx, const double* val, int m,
                                      T* M, long long ld, int row0, int rows, int* flags) {
   const int j = blockIdx.x;
-  for (long long q = colptr[j] + threadIdx.x; q < colptr[j + 1]; q += blockDim.x) {
-    const int i = rowidx[q];
-    if (i < 0 || i >= j) { atomicOr(flags, 4); continue; }
-    const double v = val[q];
-    if (v < 0.0) atomicOr(flags, 1);
-    const T e = encode<T>(v, false);
-    if (i >= row0 && i < row0 + rows) M[(size_t)(i - row0) * ld + j] = e;
-    if (j >= row0 && j < row0 + rows) M[(size_t)(j - row0) * ld + i] = e;
-  }
+  for (long long q = colptr[j] + threadIdx.x; q < colptr[j + 1]; q += blockDim.x)
+    scatter_csc_M_entry<T>(rowidx[q], j, val + q, M, ld, row0, rows, flags);
 }
 template <typename T>
 __global__ void scatter_csc_C_kernel(const long long* colptr, const int* rowidx, const double* val, int m,
                                      T* M, long long ld, int row0, int rows, int* flags) {
   const int j = blockIdx.x;
-  for (long long q = colptr[j] + threadIdx.x; q < colptr[j + 1]; q += blockDim.x) {
-    const int i = rowidx[q];
-    if (i < 0 || i >= j) { atomicOr(flags, 4); continue; }
-    const double v = val[q];
-    if (v == 0.0) continue;
-    if (v != 1.0) atomicOr(flags, 2);
-    if (i >= row0 && i < row0 + rows) { T* p = M + (size_t)(i - row0) * ld + j; double a; bool c; decode(*p, a, c); *p = encode<T>(a, true); }
-    if (j >= row0 && j < row0 + rows) { T* p = M + (size_t)(j - row0) * ld + i; double a; bool c; decode(*p, a, c); *p = encode<T>(a, true); }
-  }
+  for (long long q = colptr[j] + threadIdx.x; q < colptr[j + 1]; q += blockDim.x)
+    scatter_csc_C_entry<T>(rowidx[q], j, val + q, M, ld, row0, rows, flags);
 }
 
 // columns [j0,j1) of getAffinityMatrix()/getConstraintMatrix(): out[(j-j0)*m + i], sym + I.

@@ -165,3 +165,34 @@ def config_problem(name, m=None):
         prob = pointnormal_problem(cfg["m"], cfg["rho"], cfg["seed"])
     prob["cfg"] = cfg
     return prob
+
+
+def weighted_matrix_problem(m, density, seed, odd=0.0):
+    """Seeded weighted problem given as matrices (MatrixBatchCLIPPER, CLIPPER.set_sparse_matrix_data): random pairs
+    i < j at about the given density with weights U[0.05, 0.9), plus a planted cluster of max(3, m // 16) vertices whose
+    pairs weigh U[0.9, 1.0); a fraction `odd` of the random pairs is split evenly into (M = 0, C = 1) and (M > 0, C = 0)
+    pairs.  Returns dict(M, C) strictly upper scipy CSC and u0 (m draws of U[0, 1))."""
+    import scipy.sparse as sp
+    rng = np.random.default_rng(seed)
+    want = int(density * m * (m - 1) / 2)
+    a = rng.integers(0, m, 2 * want + 8); b = rng.integers(0, m, a.size)
+    keep = a != b
+    key = np.unique(np.minimum(a[keep], b[keep]).astype(np.int64) * m + np.maximum(a[keep], b[keep]))
+    key = key[rng.permutation(key.size)[:want]]
+    w = rng.uniform(0.05, 0.9, key.size)
+    c = np.ones(key.size)
+    n_odd = int(odd * key.size) // 2
+    w[:n_odd] = 0.0                       # no affinity, constraint set
+    c[n_odd:2 * n_odd] = 0.0              # affinity without constraint
+    S = np.sort(rng.choice(m, size=min(m, max(3, m // 16)), replace=False))
+    si, sj = np.triu_indices(S.size, 1)
+    ckey = S[si].astype(np.int64) * m + S[sj]
+    other = ~np.isin(key, ckey)
+    key = np.concatenate([key[other], ckey])
+    w = np.concatenate([w[other], rng.uniform(0.9, 1.0, ckey.size)])
+    c = np.concatenate([c[other], np.ones(ckey.size)])
+    i, j = key // m, key % m
+    km, kc = w != 0, c != 0
+    M = sp.csc_matrix((w[km], (i[km], j[km])), shape=(m, m)); M.sort_indices()
+    C = sp.csc_matrix((c[kc], (i[kc], j[kc])), shape=(m, m)); C.sort_indices()
+    return dict(M=M, C=C, u0=rng.random(m))

@@ -262,7 +262,21 @@ int clp_batch_solve_pointnormal(clp_batch b, int32_t nprob, const double* const*
                                 const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
                                 const double* const* u0, double sigp, double epsp, double sign, double epsn,
                                 clp_solution* sols, double* const* u_out, int32_t* const* nodes_out);
-/* diagnostics of the last batch: CTAs of the launch, HBM scratch bytes, stored affinities (i<j) over all problems */
+/* Problems given as matrices (the batched form of setSparseMatrixData, ref clipper.h:132-143): problem p is two
+ * strictly-upper CSC matrices M and C of m[p] columns (colptr m[p] + 1 int64 from 0, rowidx int32, val double), exactly
+ * as clp_set_sparse_upper takes them, and gets the result of an fp32 handle after clp_set_sparse_upper(h, m[p], ...) +
+ * clp_solve(h, u0[p], ...) with the batch's parameters (affinityeps plays no part).  The input is checked on the host
+ * before anything is uploaded, with clp_set_sparse_upper's predicates: CLP_ERR_INVALID for a bad structure (m[p]
+ * outside [1, 4096], colptr not starting at 0 or decreasing, a row < 0 or >= its column, rows not strictly ascending
+ * within a column -- duplicates included -- or a NULL u0[p]); then CLP_ERR_UNSUPPORTED for a negative M value, then
+ * for a C value other than 0 and 1 (NaN included).  The first problem with an error of the first kind found is named
+ * in clp_batch_last_error; the handle stays usable.  Outputs as for clp_batch_solve_*. */
+int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
+                             const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
+                             const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
+                             const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out);
+/* diagnostics of the last batch: CTAs of the launch, HBM scratch bytes, and the kept entries i<j over all problems
+ * (entries whose stored affinity is non-zero or whose C bit is set; for scored problems: the stored affinities) */
 int clp_batch_info(clp_batch b, int32_t* n_ctas, int64_t* scratch_bytes, int64_t* nnz_upper_total);
 
 /* ---- batched maximum clique: many small graphs in a constant number of launches -----------------------------------
