@@ -290,7 +290,7 @@ __device__ __forceinline__ void batch_build_solve(int p, int m, int ld, int rows
       if (r < nb) { const unsigned int hc = hist[nb - 1 - r]; hist[nb - 1 - r] = run; run += hc; }
     }
     __syncthreads();
-    // stable placement, as in sell_sort_kernel: tiles of 256 rows in row order, the warps take turns
+    // stable placement, as in sell_place_kernel: tiles of 256 rows in row order, the warps take turns
     for (int base = 0; base < rows_pad; base += kBatchThreads) {
       const int r = base + tid;
       const bool have = r < rows_pad;

@@ -130,6 +130,7 @@ struct clp_handle_s {
   int dense_mode_eff = 2; // effective, decided when the matrix is finalised
   // compact-row copy (clp_sparse.cuh)
   DevBuf sp_val, sp_col, sp_ptr4, sp_part, sp_item, sp_rowid;  // sp_ptr4: kept entries per (segment, row)
+  DevBuf sp_hist, sp_bsum;  // compact build: class histograms of the row tiles | block sums of the scans
   DevBuf sp_win, res_wcol;  // packed layout: occupied 16-column windows per row | members' columns where every warp starts
   unsigned long long sp_nnz = 0, sp_nnz_real = 0;
   SparseView sp{};
@@ -394,6 +395,25 @@ cudaError_t launch_resident_matvec(clp_handle h, const double* v, double d, doub
 
 constexpr int kKeepDense = -1;  // build_sparse: the compact copy would not pay off (NOT an error code)
 
+// CTAs of the persistent packed fill (sparse_fill_items_kernel<float, true>): at most one wave, and only as many warps
+// as the items need in the rounds a full wave would take, so that every round is about equally full.  The occupancy is
+// asked once per device.
+unsigned packed_fill_grid(clp_handle h, long long items) {
+  static std::atomic<int> occ_of[8];  // 0: not asked yet
+  std::atomic<int>& slot = occ_of[h->device & 7];
+  int occ = slot.load(std::memory_order_relaxed);
+  if (occ == 0) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sparse_fill_items_kernel<float, true>, kDevFillWarps * 32, 0) != cudaSuccess ||
+        occ < 1)
+      occ = 1;
+    slot.store(occ, std::memory_order_relaxed);
+  }
+  const long long cap = (long long)occ * h->sm_count * kDevFillWarps;  // warps of one wave
+  const long long rounds = std::max<long long>(1, (items + cap - 1) / cap);
+  const long long warps = (items + rounds - 1) / rounds;
+  return (unsigned)std::max<long long>(1, (warps + kDevFillWarps - 1) / kDevFillWarps);
+}
+
 // Called once the dense store holds the new matrix: pick the sweep (dense mode) and build what it needs.
 template <typename T>
 int build_sparse(clp_handle h, bool force, bool resident) {
@@ -441,18 +461,31 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   CLP_CUDA(h, h->sp_rowid.ensure((size_t)nseg * h->rows_pad * sizeof(unsigned int)));
   CLP_CUDA(h, h->sp_item.ensure((size_t)nitem * sizeof(unsigned int)));
   const int nb = p.W / 4 + 2;  // possible slice lengths in chunks
-  sell_sort_kernel<<<nseg, 1024, (size_t)(nb + 1) * sizeof(unsigned int), h->stream>>>(
-      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, h->sp_rowid.as<unsigned int>(), fused ? &sb->counts[0] : nullptr, pc);
-  CLP_CUDA(h, cudaGetLastError());
-  sell_itemlen_kernel<<<(unsigned)((nitem + 255) / 256), 256, 0, h->stream>>>(h->sp_ptr4.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
-                                                                              h->rows_pad, nseg, h->sp_item.as<unsigned int>(), pc);
-  CLP_CUDA(h, cudaGetLastError());
+  const int ntile = (h->rows_pad + kSortTile - 1) / kSortTile;
+  const long long nhist = (long long)nseg * nb * ntile;
+  const long long nblk = (std::max(nhist, nitem) + kScanBlock - 1) / kScanBlock;
+  CLP_CUDA(h, h->sp_hist.ensure((size_t)nhist * sizeof(unsigned int)));
+  CLP_CUDA(h, h->sp_bsum.ensure((size_t)nblk * sizeof(unsigned long long)));
   unsigned long long* total4_d = reinterpret_cast<unsigned long long*>(&sb->leaf[0][0]);  // scratch words of the sync block
-  unsigned long long* segtot_d = reinterpret_cast<unsigned long long*>(&sb->leaf[1][0]);  // [<= 64] (leaf[1..4])
-  sparse_scan_seg_kernel<<<nseg, 1024, 0, h->stream>>>(h->sp_item.as<unsigned int>(), NI + 1, segtot_d);
+  // exclusive scan in place of n words; total: nullable
+  auto scan = [&](unsigned int* a, long long n, unsigned long long* total) -> int {
+    const unsigned g = (unsigned)((n + kScanBlock - 1) / kScanBlock);
+    sparse_scan_reduce_kernel<<<g, kScanThreads, 0, h->stream>>>(a, n, h->sp_bsum.as<unsigned long long>());
+    CLP_CUDA(h, cudaGetLastError());
+    sparse_scan_down_kernel<<<g, kScanThreads, 0, h->stream>>>(a, n, h->sp_bsum.as<unsigned long long>(), (int)g, total);
+    CLP_CUDA(h, cudaGetLastError());
+    return CLP_OK;
+  };
+  const dim3 tiles((unsigned)ntile, (unsigned)nseg);
+  sell_hist_kernel<<<tiles, kSortTile, (size_t)nb * sizeof(unsigned int), h->stream>>>(
+      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, ntile, h->sp_hist.as<unsigned int>(), fused ? &sb->counts[0] : nullptr, pc);
   CLP_CUDA(h, cudaGetLastError());
-  sparse_scan_fix_kernel<<<nseg, 1024, 0, h->stream>>>(h->sp_item.as<unsigned int>(), NI + 1, nseg, segtot_d, total4_d);
+  if (int rc = scan(h->sp_hist.as<unsigned int>(), nhist, nullptr)) return rc;
+  sell_place_kernel<<<tiles, kSortTile, (size_t)nb * sizeof(unsigned int), h->stream>>>(
+      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, ntile, h->sp_hist.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
+      h->sp_item.as<unsigned int>(), pc);
   CLP_CUDA(h, cudaGetLastError());
+  if (int rc = scan(h->sp_item.as<unsigned int>(), nitem, total4_d)) return rc;
   unsigned long long host[3] = {0, 0, 0};
   unsigned int hexpo[2] = {0u, 0u};
   int host_err = 0;
@@ -476,16 +509,17 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   if (!force && !(sparse_bytes < 0.8 * dense_bytes)) return kKeepDense;  // keep a dense sweep
   CLP_CUDA(h, h->sp_val.ensure((size_t)std::max<unsigned long long>(h->sp_nnz, 4) * sizeof(T)));
   if (!h->sp.packed) CLP_CUDA(h, h->sp_col.ensure((size_t)std::max<unsigned long long>(h->sp_nnz, 4) * sizeof(unsigned short)));
+  unsigned int* next_item = reinterpret_cast<unsigned int*>(&sb->leaf[5][0]);  // zeroed with the sync block
   if (h->sp.packed) {  // whole rows (nseg = 1), fp32 only
     if constexpr (sizeof(T) == 4)
-      sparse_fill_items_kernel<T, true><<<(unsigned)((NI + kFillWarps - 1) / kFillWarps), kFillWarps * 32, 0, h->stream>>>(
+      sparse_fill_items_kernel<T, true><<<packed_fill_grid(h, NI), kDevFillWarps * 32, 0, h->stream>>>(
           M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
-          h->sp_val.as<T>(), nullptr, 0, 0u, bias);
+          h->sp_val.as<T>(), nullptr, 0, 0u, next_item, bias);
   } else {
-    const long long nwarp = (long long)nseg * NI;
-    sparse_fill_items_kernel<T><<<(unsigned)((nwarp + kFillWarps - 1) / kFillWarps), kFillWarps * 32, 0, h->stream>>>(
+    const long long nwarp = (long long)nseg * NI;  // one warp per item
+    sparse_fill_items_kernel<T><<<(unsigned)((nwarp + kDevFillWarps - 1) / kDevFillWarps), kDevFillWarps * 32, 0, h->stream>>>(
         M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
-        h->sp_val.as<T>(), h->sp_col.as<unsigned short>(), resident ? 0 : 3, resident ? (unsigned int)h->m : kZeroSlot);
+        h->sp_val.as<T>(), h->sp_col.as<unsigned short>(), resident ? 0 : 3, resident ? (unsigned int)h->m : kZeroSlot, nullptr);
   }
   CLP_CUDA(h, cudaGetLastError());
   h->sp.val = h->sp_val.p; h->sp.off16 = h->sp.packed ? nullptr : h->sp_col.as<unsigned short>();

@@ -81,12 +81,6 @@ struct PackCount {
   __device__ __forceinline__ bool on() const {
     return win && sb->counts[1] == 0ull && pack_window(sb->expo[0], sb->expo[1], nullptr);
   }
-  __device__ __forceinline__ unsigned int fillers(int r) const {
-    if (r >= rows) return 0u;
-    unsigned int occ = 0u;
-    for (int k = 0; k < wwords; ++k) occ += __popc(win[(size_t)r * wwords + k]);
-    return (unsigned int)nwin - occ;
-  }
 };
 
 template <typename T> __device__ __forceinline__ void load4(const T* p, T (&x)[4]);
@@ -154,146 +148,161 @@ __global__ void sparse_count_kernel(const T* M, long long ld, int m, int rows, i
   }
 }
 
-// pass 2: one block (1024 threads) per column segment sorts the rows by slice length, longest first (counting sort
-// over the nb = W/4 + 2 possible lengths in chunks; ties in row order: a stable sort, so the layout is reproducible).
-//   rowid[seg][pos] = row at sorted position pos
-// Dynamic shared memory: (nb + 1) counters.
-// Packed builds (pc.on()) sort by kept entries + fillers: the stored length.
-__global__ void sell_sort_kernel(const unsigned int* cnt4, int rows_pad, int nb, unsigned int* rowid,
-                                 unsigned long long* total_entries /* nullable: += kept entries */, PackCount pc) {
-  extern __shared__ unsigned int hist[];
-  __shared__ unsigned int wsum[32];
-  const unsigned int* c = cnt4 + (size_t)blockIdx.x * (rows_pad + 1);
-  const bool pk = pc.on();
-  auto len = [&](int r) { return c[r] + (pk ? pc.fillers(r) : 0u); };
-  for (int i = threadIdx.x; i <= nb; i += blockDim.x) hist[i] = 0u;
+// pass 2: a device-wide stable counting sort of the rows of every segment by slice length, longest first (the
+// nb = W/4 + 2 possible lengths in chunks are the classes; ties in row order, so the layout -- hence the grouping of
+// every fp64 sum downstream -- is reproducible), in tiles of kSortTile rows, segment-major:
+//   sell_hist_kernel   class histogram of every (segment, tile) into hist[seg][nb - 1 - class][tile]
+//   sparse_scan_*      exclusive scan of hist in that order: the sorted position of the tile's first row of the class,
+//                      counted from the start of rowid (every segment holds rows_pad rows)
+//   sell_place_kernel  stable placement inside the tile: rowid[seg][pos] = row at sorted position pos; the first row of
+//                      every item also writes the item's length (4 x its chunks), scanned by sparse_scan_* into itemptr
+// Packed builds (pc.on()) sort by kept entries + fillers: the stored length.  The class of a row is its stored length
+// in chunks, at most ceil(W / 4) <= nb - 2 (a packed row holds at most one entry or filler per column).
+constexpr int kSortTile = 256;
+
+// class of row base + threadIdx.x (0xffffffff past rows_pad); occ: kSortTile shared words
+__device__ __forceinline__ unsigned int sell_tile_class(const unsigned int* c, int base, int rows_pad, int nb, const PackCount& pc,
+                                                        bool pk, unsigned int* occ) {
+  const int r = base + (int)threadIdx.x;
+  if (pk) {  // occupied windows of the tile's rows: the bitmap words are contiguous, read them coalesced
+    occ[threadIdx.x] = 0u;
+    __syncthreads();
+    const int nr = min(kSortTile, max(0, pc.rows - base));
+    const unsigned int* w = pc.win + (size_t)base * pc.wwords;
+    for (int k = threadIdx.x; k < nr * pc.wwords; k += blockDim.x) {
+      const unsigned int x = __popc(w[k]);
+      if (x) atomicAdd(&occ[k / pc.wwords], x);
+    }
+    __syncthreads();
+  }
+  if (r >= rows_pad) return 0xffffffffu;
+  const unsigned int len = c[r] + ((pk && r < pc.rows) ? (unsigned int)pc.nwin - occ[threadIdx.x] : 0u);
+  return min((len + 3u) >> 2, (unsigned int)(nb - 1));
+}
+
+// grid (tiles, nseg), kSortTile threads; dynamic shared memory: nb counters
+__global__ void __launch_bounds__(kSortTile) sell_hist_kernel(const unsigned int* cnt4, int rows_pad, int nb, int ntile, unsigned int* hist,
+                                                              unsigned long long* total_entries /* nullable: += kept entries */, PackCount pc) {
+  extern __shared__ unsigned int h[];
+  __shared__ unsigned int occ[kSortTile];
+  const int seg = blockIdx.y, base = blockIdx.x * kSortTile;
+  const unsigned int* c = cnt4 + (size_t)seg * (rows_pad + 1);
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) h[i] = 0u;
+  const unsigned int cls = sell_tile_class(c, base, rows_pad, nb, pc, pc.on(), occ);  // synchronises when packed
   __syncthreads();
-  unsigned long long mine = 0;
-  for (int r = threadIdx.x; r < rows_pad; r += blockDim.x) { mine += c[r]; atomicAdd(&hist[min((len(r) + 3u) >> 2, (unsigned int)(nb - 1))], 1u); }
+  if (cls != 0xffffffffu) atomicAdd(&h[cls], 1u);
   if (total_entries) {
+    unsigned long long mine = cls != 0xffffffffu ? c[base + threadIdx.x] : 0u;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
     if ((threadIdx.x & 31) == 0 && mine) atomicAdd(total_entries, mine);
   }
   __syncthreads();
-  {  // start of every length class, longest class first: exclusive scan of the histogram read backwards
-    const int per = (nb + (int)blockDim.x - 1) / (int)blockDim.x;
-    const int r0 = (int)threadIdx.x * per;          // reversed positions [r0, r0 + per): bin = nb - 1 - r
-    unsigned int local = 0;
-    for (int q = 0; q < per; ++q) { const int r = r0 + q; if (r < nb) local += hist[nb - 1 - r]; }
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned int inc = local;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) wsum[w] = inc;
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) hist[((size_t)seg * nb + (nb - 1 - i)) * ntile + blockIdx.x] = h[i];
+}
+
+// grid (tiles, nseg), kSortTile threads; dynamic shared memory: nb counters.  hist: scanned by sparse_scan_*.
+// items: [nseg][NI + 1] item lengths in chunks (entry NI = 0), scanned by sparse_scan_* into itemptr
+__global__ void __launch_bounds__(kSortTile) sell_place_kernel(const unsigned int* cnt4, int rows_pad, int nb, int ntile, const unsigned int* hist,
+                                                               unsigned int* rowid, unsigned int* items, PackCount pc) {
+  extern __shared__ unsigned int taken[];
+  __shared__ unsigned int occ[kSortTile];
+  const int seg = blockIdx.y, base = blockIdx.x * kSortTile;
+  const unsigned int* c = cnt4 + (size_t)seg * (rows_pad + 1);
+  const int NI = rows_pad >> 2;
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) taken[i] = 0u;
+  if (blockIdx.x == 0 && threadIdx.x == 0) items[(size_t)seg * (NI + 1) + NI] = 0u;
+  const unsigned int cls = sell_tile_class(c, base, rows_pad, nb, pc, pc.on(), occ);
+  __syncthreads();
+  // inside the tile the warps take turns in row order; __match_any_sync ranks the lanes of equal class
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned int peers = __match_any_sync(0xffffffffu, cls);
+  const int leader = __ffs(peers) - 1;
+  const unsigned int before = __popc(peers & ((1u << lane) - 1u));
+  unsigned int start = 0u;
+  for (int w = 0; w < kSortTile / 32; ++w) {
+    if (warp == w && cls != 0xffffffffu && lane == leader) { start = taken[cls]; taken[cls] = start + __popc(peers); }
     __syncthreads();
-    if (w == 0) {
-      unsigned int v = wsum[lane], t = v;
+  }
+  start = __shfl_sync(0xffffffffu, start, leader);
+  if (cls == 0xffffffffu) return;
+  const unsigned int pos = hist[((size_t)seg * nb + (nb - 1 - cls)) * ntile + blockIdx.x] + start + before - (unsigned int)seg * rows_pad;
+  rowid[(size_t)seg * rows_pad + pos] = (unsigned int)(base + threadIdx.x);
+  if ((pos & 3u) == 0u) items[(size_t)seg * (NI + 1) + (pos >> 2)] = 4u * cls;  // the longest member: chunks of the item
+}
+
+// pass 3: exclusive scan in place of a flat array of n words (sorted positions, then item pointers), in blocks of
+// kScanBlock words: sparse_scan_reduce_kernel sums every block, sparse_scan_down_kernel adds the sums of the blocks
+// before its own to the scan of its block; block 0 publishes the grand total.  Block sums and the total are 64-bit,
+// so a total past 2^32 (the scanned words wrap) is seen by the host, which then keeps the dense sweep
+constexpr int kScanThreads = 1024, kScanPer = 4, kScanBlock = kScanThreads * kScanPer;
+
+__device__ __forceinline__ unsigned long long block_sum_u64(unsigned long long x, unsigned long long* wsum) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
 #pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
-      wsum[lane] = t - v;
-    }
-    __syncthreads();
-    unsigned int run = wsum[w] + (inc - local);
-    for (int q = 0; q < per; ++q) {
-      const int r = r0 + q;
-      if (r < nb) { const unsigned int hcount = hist[nb - 1 - r]; hist[nb - 1 - r] = run; run += hcount; }
-    }
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  __syncthreads();
+  if (lane == 0) wsum[w] = x;
+  __syncthreads();
+  unsigned long long t = lane < (int)(blockDim.x >> 5) ? wsum[lane] : 0ull;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+  return t;
+}
+
+__global__ void __launch_bounds__(kScanThreads) sparse_scan_reduce_kernel(const unsigned int* a, long long n, unsigned long long* bsum) {
+  __shared__ unsigned long long wsum[32];
+  const long long i0 = (long long)blockIdx.x * kScanBlock + (long long)threadIdx.x * kScanPer;
+  unsigned long long x = 0;
+#pragma unroll
+  for (int q = 0; q < kScanPer; ++q) if (i0 + q < n) x += a[i0 + q];
+  x = block_sum_u64(x, wsum);
+  if (threadIdx.x == 0) bsum[blockIdx.x] = x;
+}
+
+__global__ void __launch_bounds__(kScanThreads) sparse_scan_down_kernel(unsigned int* a, long long n, const unsigned long long* bsum, int nblk,
+                                                                        unsigned long long* total /* nullable */) {
+  __shared__ unsigned long long wsum[32];
+  __shared__ unsigned int wex[32];
+  unsigned long long off = 0;  // sums of the blocks before this one (block 0: of all blocks, for the total)
+  const int upto = blockIdx.x == 0 ? nblk : (int)blockIdx.x;
+  for (int k = threadIdx.x; k < upto; k += blockDim.x) off += bsum[k];
+  off = block_sum_u64(off, wsum);
+  if (blockIdx.x == 0) { if (total && threadIdx.x == 0) *total = off; off = 0; }
+  const long long i0 = (long long)blockIdx.x * kScanBlock + (long long)threadIdx.x * kScanPer;
+  unsigned int x[kScanPer], mine = 0u;
+#pragma unroll
+  for (int q = 0; q < kScanPer; ++q) { x[q] = (i0 + q < n) ? a[i0 + q] : 0u; mine += x[q]; }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned int inc = mine;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+  if (lane == 31) wex[w] = inc;
+  __syncthreads();
+  if (w == 0) {
+    const unsigned int v = wex[lane];
+    unsigned int t = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, t, o); if (lane >= o) t += y; }
+    wex[lane] = t - v;
   }
   __syncthreads();
-  // STABLE placement (ties in row order): the layout -- hence the grouping of every fp64 sum downstream -- must not
-  // depend on the arrival order of atomics, or two runs on the same input differ in the last bit.  Rows are taken in
-  // tiles of blockDim.x in row order; inside a tile the warps take turns (one __syncthreads per turn); inside a warp
-  // __match_any_sync ranks the lanes of equal length class.
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = blockDim.x >> 5;
-  for (int base = 0; base < rows_pad; base += blockDim.x) {
-    const int r = base + threadIdx.x;
-    const bool have = r < rows_pad;
-    const unsigned int cls = have ? min((len(r) + 3u) >> 2, (unsigned int)(nb - 1)) : 0xffffffffu;
-    const unsigned int peers = __match_any_sync(0xffffffffu, cls);
-    const int leader = __ffs(peers) - 1;
-    const unsigned int before = __popc(peers & ((1u << lane) - 1u));
-    unsigned int start = 0u;
-    for (int w = 0; w < nwarp; ++w) {   // the warps of the tile take turns (passing a ticket through shared memory
-      if (warp == w && have && lane == leader) { start = hist[cls]; hist[cls] = start + __popc(peers); }  // with
-      __syncthreads();                  // spinning warps was several times slower)
-    }
-    start = __shfl_sync(0xffffffffu, start, leader);
-    if (have) rowid[(size_t)blockIdx.x * rows_pad + start + before] = (unsigned int)r;
-  }
-}
-
-// pass 3: chunks of every item = 4 x its longest member (the first one in sorted order); scanned in place by
-// the two scan kernels below into itemptr[seg][0..NI]
-__global__ void sell_itemlen_kernel(const unsigned int* cnt4, const unsigned int* rowid, int rows_pad, int nseg,
-                                    unsigned int* itemptr, PackCount pc) {
-  const int NI = rows_pad >> 2;
-  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= (long long)nseg * (NI + 1)) return;
-  const int seg = (int)(t / (NI + 1)), i = (int)(t - (long long)seg * (NI + 1));
-  unsigned int len = 0u;
-  if (i < NI) {
-    const unsigned int r = rowid[(size_t)seg * rows_pad + 4 * i];
-    len = 4u * ((cnt4[(size_t)seg * (rows_pad + 1) + r] + (pc.on() ? pc.fillers((int)r) : 0u) + 3u) >> 2);
-  }
-  itemptr[t] = len;
-}
-
-// pass 3a: one block per column segment: exclusive scan (in place) of that segment's item lengths, walking the
-// array in coalesced tiles of 1024; the segment total goes to segtot[seg]
-__global__ void sparse_scan_seg_kernel(unsigned int* cnt4, int n, unsigned long long* segtot) {
-  __shared__ unsigned int wsum[32];
-  __shared__ unsigned int carry_s;
-  unsigned int* a = cnt4 + (size_t)blockIdx.x * n;
-  const int t = threadIdx.x, lane = t & 31, w = t >> 5;
-  unsigned long long carry = 0;
-  for (int base = 0; base < n; base += 1024) {
-    const int i = base + t;
-    const unsigned int x = (i < n) ? a[i] : 0u;
-    unsigned int inc = x;
+  unsigned int run = (unsigned int)off + wex[w] + (inc - mine);
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
-    if (lane == 31) wsum[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-      unsigned int v = wsum[lane], s = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, s, o); if (lane >= o) s += y; }
-      wsum[lane] = s - v;                 // exclusive prefix of the warp sums
-      if (lane == 31) carry_s = s;        // tile total
-    }
-    __syncthreads();
-    if (i < n) a[i] = (unsigned int)(carry + wsum[w] + (inc - x));
-    carry += carry_s;
-    __syncthreads();
-  }
-  if (t == 0) segtot[blockIdx.x] = carry;
-}
-
-// pass 3b: add the start of each segment (prefix of the segment totals); block 0 also publishes the grand total
-__global__ void sparse_scan_fix_kernel(unsigned int* cnt4, int n, int nseg, const unsigned long long* segtot,
-                                       unsigned long long* total4) {
-  unsigned long long base = 0;
-  for (int s = 0; s < (int)blockIdx.x; ++s) base += segtot[s];
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    unsigned long long tot = 0;
-    for (int s = 0; s < nseg; ++s) tot += segtot[s];
-    *total4 = tot;
-  }
-  if (base == 0) return;
-  unsigned int* a = cnt4 + (size_t)blockIdx.x * n;
-  for (int i = threadIdx.x; i < n; i += blockDim.x) a[i] += (unsigned int)base;
+  for (int q = 0; q < kScanPer; ++q) if (i0 + q < n) { a[i0 + q] = run; run += x[q]; }
 }
 
 // pass 4: one warp per item reads its four member rows together and compacts them through four shared-memory
 // rings; chunk k of all four members is then 64 contiguous bytes of val (32 of off16), so a flush of 8 chunks per
 // member is one fully coalesced 512-byte store.
-constexpr int kFillWarps = 4;
+constexpr int kFillWarps = 4;  // warps of the batched solver's fill (clp_batch.cuh)
 constexpr int kRing = 256;  // entries per member ring: < 36 left after a flush + <= 128 new ones per step
 // one warp: the item whose chunks are [b, e) of the stream and whose members are rows r[0..3]; columns [c0, c1)
 // PACK (fp32, whole rows): one filler (+0.0) at the first column of every empty 16-column window of a real row, and
 // the chunks are written as packed words (pack_word; the column delta reads the previous entry from the ring)
-template <typename T, bool PACK = false>
+// PIPE: the loads of the next 128-column step are issued (streaming, no L1 allocation) before the current step is
+// scanned and flushed, so a warp always has one step of its rows in flight
+template <typename T, bool PACK = false, bool PIPE = false>
 __device__ __forceinline__ void sell_fill_item_warp(const T* M, long long ld, int rows, int c0, int c1, unsigned int b, unsigned int e,
                                                     const unsigned int (&r)[4], T* val, unsigned short* off16, int off_shift,
                                                     unsigned int pad_off, T (*rv)[kRing], unsigned short (*ro)[kRing],
@@ -301,6 +310,21 @@ __device__ __forceinline__ void sell_fill_item_warp(const T* M, long long ld, in
   const int lane = threadIdx.x & 31;
   const unsigned int L = (e - b) >> 2;  // chunks per member
   if (L == 0u) return;
+  T xn[4][4];  // PIPE: the step after the current one
+  auto load_step = [&](int jj, T (&y)[4][4]) {
+#pragma unroll
+    for (int s_ = 0; s_ < 4; ++s_) {
+      if (r[s_] < (unsigned int)rows) {  // jj + 3 < ld: ld is a multiple of 128
+        if constexpr (sizeof(T) == 4) {
+          const float4 v = ldg_stream(reinterpret_cast<const float4*>(M + (size_t)r[s_] * ld + jj));
+          y[s_][0] = v.x; y[s_][1] = v.y; y[s_][2] = v.z; y[s_][3] = v.w;
+        } else {
+          load4<T>(M + (size_t)r[s_] * ld + jj, y[s_]);
+        }
+      } else { y[s_][0] = y[s_][1] = y[s_][2] = y[s_][3] = encode<T>(0.0, false); }
+    }
+  };
+  if constexpr (PIPE) load_step(c0 + lane * 4, xn);
   unsigned int n[4] = {0u, 0u, 0u, 0u}, f[4] = {0u, 0u, 0u, 0u};
   const int g = lane >> 2, ms = lane & 3;  // flush role: chunk f + g of member ms
   // writes chunk k of member ms (entries beyond the member's n are neutral padding)
@@ -337,10 +361,18 @@ __device__ __forceinline__ void sell_fill_item_warp(const T* M, long long ld, in
     // as four 8-bit fields: a member keeps at most 128 entries per step)
     T x[4][4];
     unsigned int keep[4], packed = 0u;
+    if constexpr (PIPE) {
 #pragma unroll
-    for (int s_ = 0; s_ < 4; ++s_) {
-      if (r[s_] < (unsigned int)rows) load4<T>(M + (size_t)r[s_] * ld + j, x[s_]);  // j + 3 < ld: ld is a multiple of 128
-      else { x[s_][0] = x[s_][1] = x[s_][2] = x[s_][3] = encode<T>(0.0, false); }
+      for (int s_ = 0; s_ < 4; ++s_)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) x[s_][q] = xn[s_][q];
+      if (j0 + 128 < c1) load_step(j + 128, xn);
+    } else {
+#pragma unroll
+      for (int s_ = 0; s_ < 4; ++s_) {
+        if (r[s_] < (unsigned int)rows) load4<T>(M + (size_t)r[s_] * ld + j, x[s_]);  // j + 3 < ld: ld is a multiple of 128
+        else { x[s_][0] = x[s_][1] = x[s_][2] = x[s_][3] = encode<T>(0.0, false); }
+      }
     }
 #pragma unroll
     for (int s_ = 0; s_ < 4; ++s_) {
@@ -396,26 +428,46 @@ __device__ __forceinline__ void sell_fill_item_warp(const T* M, long long ld, in
   __syncwarp();
 }
 
+// One warp per item.  The packed whole-row build (PACK, config 2's) is PERSISTENT: the grid holds at most one wave of
+// CTAs, and every warp draws items in stream order from the zeroed counter next_item until none is left, loading the
+// next 128-column step while it scans and flushes the current one (sell_fill_item_warp<..., PIPE>).  Every item reads
+// whole rows of the dense store, so all cost about the same.  fill_grid (clp_capi.cu) keeps the number of rounds a
+// full wave would need but spreads the items over as few warps as that takes, so every round is about equally full:
+// at config 2 (5 000 items, 4 752 warps in a wave) about 2 500 warps take two items each, where one warp per item left
+// 248 items to a second wave on an idle GPU.  The 6-byte builds (column segments: config 4's 400 000 short items)
+// keep one CTA slot per item: there the persistent, pipelined variant measured 8 % slower (12.31 against 11.38 ms).
+// The ring size is shared with the batched solver's fill and already the smallest power of two above what a step
+// needs; the warps per CTA are this kernel's own (kDevFillWarps; 2 and 4 measured the same at config 2).
+constexpr int kDevFillWarps = 4;
 template <typename T, bool PACK = false>
-__global__ void __launch_bounds__(kFillWarps * 32)
+__global__ void __launch_bounds__(kDevFillWarps * 32)
 sparse_fill_items_kernel(const T* M, long long ld, int m, int rows, int rows_pad, int W, int nseg,
                          const unsigned int* itemptr, const unsigned int* rowid, T* val, unsigned short* off16,
                          int off_shift /* 3: byte offset of v[col] in the staged segment; 0: column index */,
                          unsigned int pad_off /* offset stored in padding entries: a slot that holds 0.0 */,
-                         unsigned int bias = 0u /* PACK: exponent bias of the codes */) {
-  __shared__ __align__(16) T ringv[kFillWarps][4][kRing];
-  __shared__ __align__(8) unsigned short ringo[kFillWarps][4][kRing];
-  const int wic = threadIdx.x >> 5;
+                         unsigned int* next_item /* PACK */, unsigned int bias = 0u /* PACK: exponent bias of the codes */) {
+  __shared__ __align__(16) T ringv[kDevFillWarps][4][kRing];
+  __shared__ __align__(8) unsigned short ringo[kDevFillWarps][4][kRing];
+  const int wic = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int NI = rows_pad >> 2;
-  const long long gw = (long long)blockIdx.x * kFillWarps + wic;
-  if (gw >= (long long)nseg * NI) return;
-  const int seg = (int)(gw / NI), it = (int)(gw - (long long)seg * NI);
-  const unsigned int b = itemptr[(size_t)seg * (NI + 1) + it], e = itemptr[(size_t)seg * (NI + 1) + it + 1];
-  unsigned int r[4];
+  const unsigned int N = (unsigned int)nseg * (unsigned int)NI;
+  unsigned int g = (unsigned int)blockIdx.x * kDevFillWarps + wic;
+  for (;;) {
+    if constexpr (PACK) {
+      g = 0u;
+      if (lane == 0) g = atomicAdd(next_item, 1u);
+      g = __shfl_sync(0xffffffffu, g, 0);
+    }
+    if (g >= N) return;
+    const int seg = (int)(g / (unsigned int)NI), it = (int)(g - (unsigned int)seg * NI);
+    const unsigned int b = itemptr[(size_t)seg * (NI + 1) + it], e = itemptr[(size_t)seg * (NI + 1) + it + 1];
+    unsigned int r[4];
 #pragma unroll
-  for (int s_ = 0; s_ < 4; ++s_) r[s_] = rowid[(size_t)seg * rows_pad + 4 * it + s_];
-  const int c0 = seg * W, c1 = min(m, c0 + W);
-  sell_fill_item_warp<T, PACK>(M, ld, rows, c0, c1, b, e, r, val, off16, off_shift, pad_off, ringv[wic], ringo[wic], bias);
+    for (int s_ = 0; s_ < 4; ++s_) r[s_] = rowid[(size_t)seg * rows_pad + 4 * it + s_];
+    const int c0 = seg * W, c1 = min(m, c0 + W);
+    sell_fill_item_warp<T, PACK, PACK>(M, ld, rows, c0, c1, b, e, r, val, off16, off_shift, pad_off, ringv[wic], ringo[wic], bias);
+    if constexpr (!PACK) return;
+  }
 }
 
 // 4 entries of one row slice
