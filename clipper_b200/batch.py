@@ -24,11 +24,7 @@ class BatchCLIPPER:
         if not isinstance(invariant, (EuclideanDistance, PointNormalDistance)):
             raise TypeError("a batch scores with the built-in invariants (EuclideanDistance, PointNormalDistance)")
         self._lib = _capi.load()
-        self._b = C.c_void_p()
-        rc = self._lib.clp_batch_create(int(device), C.byref(self._b))
-        if rc != _capi.OK:
-            msg = self._lib.clp_batch_last_error(None)
-            raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+        self._b = _new_batch(self._lib, device)
         self._invariant = invariant
         self._params = params if params is not None else Params()
 
@@ -62,44 +58,19 @@ class BatchCLIPPER:
             return []
         params = params if params is not None else MCParams()
         self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
-        keep = []
-        vp = C.c_void_p
-        D1p, D2p, Ap = (vp * n)(), (vp * n)(), (vp * n)()
-        n1, n2, m = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
-        ms = []
-        d = None
-        for k, p in enumerate(problems):
-            D1 = np.asfortranarray(_check_f64(p["D1"], "D1")); D2 = np.asfortranarray(_check_f64(p["D2"], "D2"))
-            if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
-                raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
-            if d is None:
-                d = D1.shape[0]
-            elif d != D1.shape[0]:
-                raise ValueError("all problems of a batch must have the same data dimension")
-            A = p.get("A")
-            if A is None or np.size(A) == 0:
-                mk = D1.shape[1] * D2.shape[1]; Ak = None
-            else:
-                if not isinstance(A, np.ndarray) or A.dtype != np.int32 or A.ndim != 2 or A.shape[1] != 2:
-                    raise TypeError("A must be an (m, 2) numpy int32 array")
-                Ak = np.asfortranarray(A); mk = Ak.shape[0]
-            keep += [D1, D2, Ak]
-            ms.append(mk)
-            D1p[k], D2p[k] = D1.ctypes.data, D2.ctypes.data
-            Ap[k] = Ak.ctypes.data if Ak is not None else None
-            n1[k], n2[k], m[k] = D1.shape[1], D2.shape[1], (mk if Ak is not None else 0)
+        d, pts, ms, keep = _point_problems(problems)  # keep: the arrays pts points into, alive during the call
         inv = self._invariant
         out, args = _mc_outputs(ms, params)
         if isinstance(inv, EuclideanDistance):
             q = inv.params()
-            rc = self._lib.clp_batch_max_clique_euclidean(self._b, n, int(d), D1p, n1, D2p, n2, Ap, m, float(q.sigma),
-                                                          float(q.epsilon), float(q.mindist), *args)
+            rc = self._lib.clp_batch_max_clique_euclidean(self._b, n, int(d), *pts, float(q.sigma), float(q.epsilon),
+                                                          float(q.mindist), *args)
         else:
             if d != 6:
                 raise ValueError("PointNormalDistance expects 6 x n data")
             q = inv.params()
-            rc = self._lib.clp_batch_max_clique_pointnormal(self._b, n, D1p, n1, D2p, n2, Ap, m, float(q.sigp),
-                                                            float(q.epsp), float(q.sign), float(q.epsn), *args)
+            rc = self._lib.clp_batch_max_clique_pointnormal(self._b, n, *pts, float(q.sigp), float(q.epsp), float(q.sign),
+                                                            float(q.epsn), *args)
         self._check(rc)
         return out()
 
@@ -112,61 +83,31 @@ class BatchCLIPPER:
         if n == 0:
             return []
         self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
-        keep = []  # keeps the converted arrays alive during the call
+        d, pts, ms, keep = _point_problems(problems)  # keep: the arrays pts points into, alive during the call
         vp = C.c_void_p
-        D1p, D2p, Ap, u0p, up, np_ = (vp * n)(), (vp * n)(), (vp * n)(), (vp * n)(), (vp * n)(), (vp * n)()
-        n1, n2, m = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
-        us, nodes = [], []
-        d = None
-        for k, p in enumerate(problems):
-            D1 = np.asfortranarray(_check_f64(p["D1"], "D1")); D2 = np.asfortranarray(_check_f64(p["D2"], "D2"))
-            if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
-                raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
-            if d is None:
-                d = D1.shape[0]
-            elif d != D1.shape[0]:
-                raise ValueError("all problems of a batch must have the same data dimension")
-            A = p.get("A")
-            if A is None or np.size(A) == 0:
-                mk = D1.shape[1] * D2.shape[1]; Ak = None
-            else:
-                if not isinstance(A, np.ndarray) or A.dtype != np.int32 or A.ndim != 2 or A.shape[1] != 2:
-                    raise TypeError("A must be an (m, 2) numpy int32 array")
-                Ak = np.asfortranarray(A); mk = Ak.shape[0]
+        u0p, up, np_ = (vp * n)(), (vp * n)(), (vp * n)()
+        u0s, us, nodes = [], [], []
+        for k, (p, mk) in enumerate(zip(problems, ms)):
             u0 = np.ascontiguousarray(_check_f64(p["u0"], "u0")).reshape(-1)
             if u0.size != mk:
                 raise ValueError("problem %d: u0 has %d entries, expected %d" % (k, u0.size, mk))
             uk = np.zeros(mk, np.float64); nk = np.zeros(max(mk, 1), np.int32)
-            keep += [D1, D2, Ak, u0]
-            us.append(uk); nodes.append(nk)
-            D1p[k], D2p[k], u0p[k] = D1.ctypes.data, D2.ctypes.data, u0.ctypes.data
-            Ap[k] = Ak.ctypes.data if Ak is not None else None
-            up[k], np_[k] = uk.ctypes.data, nk.ctypes.data
-            n1[k], n2[k], m[k] = D1.shape[1], D2.shape[1], (mk if Ak is not None else 0)
+            u0s.append(u0); us.append(uk); nodes.append(nk)
+            u0p[k], up[k], np_[k] = u0.ctypes.data, uk.ctypes.data, nk.ctypes.data
         sols = (_capi.ClpSolution * n)()
         inv = self._invariant
         if isinstance(inv, EuclideanDistance):
             q = inv.params()
-            rc = self._lib.clp_batch_solve_euclidean(self._b, n, int(d), D1p, n1, D2p, n2, Ap, m, u0p,
-                                                     float(q.sigma), float(q.epsilon), float(q.mindist), sols, up, np_)
+            rc = self._lib.clp_batch_solve_euclidean(self._b, n, int(d), *pts, u0p, float(q.sigma), float(q.epsilon),
+                                                     float(q.mindist), sols, up, np_)
         else:
             if d != 6:
                 raise ValueError("PointNormalDistance expects 6 x n data")
             q = inv.params()
-            rc = self._lib.clp_batch_solve_pointnormal(self._b, n, D1p, n1, D2p, n2, Ap, m, u0p,
-                                                       float(q.sigp), float(q.epsp), float(q.sign), float(q.epsn), sols, up, np_)
+            rc = self._lib.clp_batch_solve_pointnormal(self._b, n, *pts, u0p, float(q.sigp), float(q.epsp), float(q.sign),
+                                                       float(q.epsn), sols, up, np_)
         self._check(rc)
-        out = []
-        for k in range(n):
-            s = sols[k]
-            o = Solution()
-            o.t, o.ifinal, o.score = s.t, s.ifinal, s.score
-            o.nodes = nodes[k][: s.n_nodes].tolist()
-            o.u0, o.u = keep[4 * k + 3], us[k]
-            o.d_final, o.n_evals, o.n_matvec, o.n_inner, o.kernel_ms = s.d_final, s.n_evals, s.n_matvec, s.n_inner, s.kernel_ms
-            o.prof_ms = (s.prof_matvec_ms, s.prof_combine_ms, s.prof_exchange_ms)
-            out.append(o)
-        return out
+        return _solutions(sols, n, u0s, us, nodes)
 
 
 def _solutions(sols, n, u0s, us, nodes):
@@ -182,6 +123,49 @@ def _solutions(sols, n, u0s, us, nodes):
         o.prof_ms = (s.prof_matvec_ms, s.prof_combine_ms, s.prof_exchange_ms)
         out.append(o)
     return out
+
+
+def _new_batch(lib, device):
+    """a new clp_batch handle on the device; ClipperError with the library's reason when it cannot be made"""
+    b = C.c_void_p()
+    rc = lib.clp_batch_create(int(device), C.byref(b))
+    if rc != _capi.OK:
+        msg = lib.clp_batch_last_error(None)
+        raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+    return b
+
+
+def _point_problems(problems):
+    """the point clouds of scored problems (dicts with D1 (d, n1), D2 (d, n2) and A (m, 2) int32 or None) as the batch
+    C-ABI takes them: (d, (D1, n1, D2, n2, A, m) pointer arrays, the m of every problem, the converted arrays the
+    pointers point into).  A missing or empty A is the all-to-all hypothesis, passed as m = 0."""
+    n = len(problems)
+    vp = C.c_void_p
+    D1p, D2p, Ap = (vp * n)(), (vp * n)(), (vp * n)()
+    n1, n2, m = (C.c_int64 * n)(), (C.c_int64 * n)(), (C.c_int64 * n)()
+    keep, ms = [], []
+    d = None
+    for k, p in enumerate(problems):
+        D1 = np.asfortranarray(_check_f64(p["D1"], "D1")); D2 = np.asfortranarray(_check_f64(p["D2"], "D2"))
+        if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
+            raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+        if d is None:
+            d = D1.shape[0]
+        elif d != D1.shape[0]:
+            raise ValueError("all problems of a batch must have the same data dimension")
+        A = p.get("A")
+        if A is None or np.size(A) == 0:
+            mk = D1.shape[1] * D2.shape[1]; Ak = None
+        else:
+            if not isinstance(A, np.ndarray) or A.dtype != np.int32 or A.ndim != 2 or A.shape[1] != 2:
+                raise TypeError("A must be an (m, 2) numpy int32 array")
+            Ak = np.asfortranarray(A); mk = Ak.shape[0]
+        keep += [D1, D2, Ak]
+        ms.append(mk)
+        D1p[k], D2p[k] = D1.ctypes.data, D2.ctypes.data
+        Ap[k] = Ak.ctypes.data if Ak is not None else None
+        n1[k], n2[k], m[k] = D1.shape[1], D2.shape[1], (mk if Ak is not None else 0)
+    return d, (D1p, n1, D2p, n2, Ap, m), ms, keep
 
 
 def matrices_to_csc(M, C_):
@@ -227,11 +211,7 @@ class MatrixBatchCLIPPER:
 
     def __init__(self, params=None, device=0):
         self._lib = _capi.load()
-        self._b = C.c_void_p()
-        rc = self._lib.clp_batch_create(int(device), C.byref(self._b))
-        if rc != _capi.OK:
-            msg = self._lib.clp_batch_last_error(None)
-            raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+        self._b = _new_batch(self._lib, device)
         self._params = params if params is not None else Params()
 
     __del__ = BatchCLIPPER.__del__
@@ -348,11 +328,7 @@ def maxclique_many(graphs, params=None, device=0):
     params = params if params is not None else MCParams()
     csc = [graph_to_csc(G) for G in graphs]
     lib = _capi.load()
-    b = C.c_void_p()
-    rc = lib.clp_batch_create(int(device), C.byref(b))
-    if rc != _capi.OK:
-        msg = lib.clp_batch_last_error(None)
-        raise _capi.ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+    b = _new_batch(lib, device)
     try:
         vp = C.c_void_p
         m = (C.c_int64 * n)(*[c[0] for c in csc])

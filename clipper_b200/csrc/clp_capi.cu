@@ -30,8 +30,6 @@ using namespace clp;
 
 namespace {
 
-thread_local std::string g_create_error;
-
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
@@ -43,6 +41,20 @@ struct DevBuf {
     return e;
   }
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
+};
+
+struct PinnedBuf {  // page-locked host staging: the asynchronous copies from and to it do not wait for the host
+  void* p = nullptr;
+  size_t cap = 0;
+  cudaError_t ensure(size_t bytes) {
+    if (bytes <= cap) return cudaSuccess;
+    if (p) { cudaFreeHost(p); p = nullptr; cap = 0; }
+    cudaError_t e = cudaMallocHost(&p, bytes);
+    if (e == cudaSuccess) cap = bytes;
+    return e;
+  }
+  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
   template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
 };
 
@@ -119,8 +131,7 @@ struct clp_handle_s {
   DevBuf res_vecs, res_cand, res_pieces, res_redll;  // resident solver: plain vectors | candidate points | piece table | LL sums
   DevBuf panel;   // staging panels for get/set dense
   DevBuf cscbuf;
-  void* pinned = nullptr;
-  size_t pinned_cap = 0;
+  PinnedBuf pinned;
   Plan plan{};
   long long mpad = 0;
   // stripe decomposition (clp_dense2.cuh)
@@ -150,8 +161,18 @@ struct clp_handle_s {
 
 namespace {
 
-int fail(clp_handle h, int code, const std::string& msg) {
-  if (h) h->err = msg; else g_create_error = msg;
+// the message of the last failed create on this thread, one per handle type (clp_handle_s, clp_batch_s): what
+// clp_last_error(nullptr) and clp_batch_last_error(nullptr) return
+template <typename H>
+std::string& create_error() {
+  thread_local std::string msg;
+  return msg;
+}
+
+// records msg on the handle (or, without one, as the failed create's message) and returns code
+template <typename H>
+int fail(H* h, int code, const std::string& msg) {
+  (h ? h->err : create_error<H>()) = msg;
   return code;
 }
 
@@ -167,20 +188,35 @@ inline long long round_up(long long x, long long q) { return (x + q - 1) / q * q
 int reset_sync(clp_handle h);
 
 // nothing may propagate out of an extern "C" entry point (the library is loaded into Python and into C callers)
-template <typename F>
-int guarded(clp_handle h, F&& f) {
+template <typename H, typename F>
+int guarded(H* h, F&& f) {
   try { return f(); }
   catch (const std::bad_alloc&) { return fail(h, CLP_ERR_ALLOC, "host allocation failed"); }
   catch (const std::exception& e) { return fail(h, CLP_ERR_INVALID, std::string("internal error: ") + e.what()); }
   catch (...) { return fail(h, CLP_ERR_INVALID, "internal error"); }
 }
 
-int ensure_pinned(clp_handle h, size_t bytes) {
-  if (bytes <= h->pinned_cap) return CLP_OK;
-  if (h->pinned) { cudaFreeHost(h->pinned); h->pinned = nullptr; h->pinned_cap = 0; }
-  CLP_CUDA(h, cudaMallocHost(&h->pinned, bytes));
-  h->pinned_cap = bytes;
+// the checks clp_create and clp_batch_create share: the ordinal names a device, and that device is an sm_90
+template <typename H>
+int probe_device(int device, cudaDeviceProp* prop) {
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return fail<H>(nullptr, CLP_ERR_CUDA, std::string("no usable CUDA device: ") + cudaGetErrorString(e));
+  if (device < 0 || device >= ndev) return fail<H>(nullptr, CLP_ERR_INVALID, "device ordinal out of range");
+  if ((e = cudaGetDeviceProperties(prop, device)) != cudaSuccess) return fail<H>(nullptr, CLP_ERR_CUDA, cudaGetErrorString(e));
+  if (prop->major != 9 || prop->minor != 0)
+    return fail<H>(nullptr, CLP_ERR_CUDA, "clipper_b200 is built for sm_90a only; device is sm_" + std::to_string(prop->major) +
+                                              std::to_string(prop->minor));
   return CLP_OK;
+}
+
+SolverParams solver_params(const clp_params& P) {
+  SolverParams prm;
+  prm.tol_u = P.tol_u; prm.tol_F = P.tol_F; prm.beta = P.beta; prm.eps = P.eps;
+  prm.maxiniters = P.maxiniters; prm.maxoliters = P.maxoliters; prm.maxlsiters = P.maxlsiters;
+  prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
+  return prm;
 }
 
 void shard_rows(long long m, int rank, int world, int* row0, int* rows) {
@@ -353,10 +389,7 @@ ResArgs res_args(clp_handle h) {
   std::memset(&a, 0, sizeof(a));
   a.sp = h->sp;
   a.m = (int)h->m; a.row0 = h->row0; a.rows = h->rows; a.rows_pad = h->rows_pad; a.NI = h->res_NI; a.G = h->res_G;
-  const clp_params& P = h->prm;
-  a.prm.tol_u = P.tol_u; a.prm.tol_F = P.tol_F; a.prm.beta = P.beta; a.prm.eps = P.eps;
-  a.prm.maxiniters = P.maxiniters; a.prm.maxoliters = P.maxoliters; a.prm.maxlsiters = P.maxlsiters;
-  a.prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
+  a.prm = solver_params(h->prm);
   a.u0 = h->u0dev.as<double>();
   a.vecs = h->res_vecs.as<double>();
   a.cand = h->res_cand.as<double>();
@@ -622,7 +655,7 @@ int ensure_matrix(clp_handle h, long long m) {
   CLP_CUDA(h, h->result.ensure(256 + (size_t)h->mpad * sizeof(double)));
   CLP_CUDA(h, h->u0dev.ensure((size_t)h->mpad * sizeof(double)));
   CLP_CUDA(h, h->ybuf.ensure((size_t)4 * h->mpad * sizeof(double)));
-  if (int rc = ensure_pinned(h, 256 + (size_t)h->mpad * sizeof(double))) return rc;
+  CLP_CUDA(h, h->pinned.ensure(256 + (size_t)h->mpad * sizeof(double)));
   h->has_matrix = false;
   return CLP_OK;
 }
@@ -841,9 +874,7 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
   SolverArgs a;
   a.mv = mat_view(h);
   a.plan = h->plan;
-  a.prm.tol_u = P.tol_u; a.prm.tol_F = P.tol_F; a.prm.beta = P.beta; a.prm.eps = P.eps;
-  a.prm.maxiniters = P.maxiniters; a.prm.maxoliters = P.maxoliters; a.prm.maxlsiters = P.maxlsiters;
-  a.prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
+  a.prm = solver_params(P);
   SyncBlock* sb = h->sync.as<SyncBlock>();
   a.bar.sb = sb; a.bar.nleaf = std::min(32, h->plan.G); a.bar.G = h->plan.G;
   a.u0 = h->u0dev.as<double>();
@@ -880,7 +911,7 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
   CLP_CUDA(h, le);
   CLP_CUDA(h, cudaEventRecord(h->ev1, h->stream));
   const size_t rbytes = 256 + (size_t)h->m * sizeof(double);
-  CLP_CUDA(h, cudaMemcpyAsync(h->pinned, h->result.p, rbytes, cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaMemcpyAsync(h->pinned.p, h->result.p, rbytes, cudaMemcpyDeviceToHost, h->stream));
   if (u_out_dev)
     CLP_CUDA(h, cudaMemcpyAsync(u_out_dev, a.u_final, (size_t)h->m * sizeof(double), cudaMemcpyDeviceToDevice, h->stream));
   CLP_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -888,7 +919,7 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
   float ms = 0.f;
   CLP_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
 
-  const SolverOut so = *reinterpret_cast<const SolverOut*>(h->pinned);
+  const SolverOut so = *h->pinned.as<const SolverOut>();
   h->seq = so.seq_end;
   if (h->prof_ctas && h->dense_mode_eff == 6) {  // diagnostics: spread of the per-CTA phase times
     std::vector<double> pc((size_t)h->res_G * 8);
@@ -910,7 +941,7 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
     h->shard_ready = false;  // sequence numbers may have diverged between ranks
     return fail(h, CLP_ERR_TIMEOUT, "solver kernel: device-wide barrier / peer exchange timed out");
   }
-  const double* u = reinterpret_cast<const double*>(reinterpret_cast<const char*>(h->pinned) + 256);
+  const double* u = reinterpret_cast<const double*>(h->pinned.as<const char>() + 256);
 
   // rounding (ref clipper.cpp:287-310) on the device-produced u
   std::vector<int32_t> nodes;
@@ -1009,6 +1040,31 @@ struct McEvents {  // timing of one call; destroyed with the call
 float mc_elapsed(cudaEvent_t a, cudaEvent_t b) {
   float ms = 0.f;
   return cudaEventElapsedTime(&ms, a, b) == cudaSuccess ? ms : 0.f;
+}
+
+// EXACT search over tasks of at most K candidates (mc_search_kernel, mc_batch_search_kernel): words of a candidate
+// bitset, node arena, scratch bytes per worker, workers (two per SM warp slot, no more than half of free_b holds, whole
+// CTAs; fewer than one CTA means the scratch does not fit) and the nanoseconds left of time_limit_s since t0.
+struct McSearchSetup {
+  int KW;
+  unsigned arena_cap;
+  size_t stride;
+  long long nworkers;
+  unsigned long long limit_ns;
+};
+
+McSearchSetup mc_search_setup(int K, size_t free_b, int sm_count, double time_limit_s, std::chrono::steady_clock::time_point t0) {
+  McSearchSetup s;
+  s.KW = (K + 31) / 32;
+  s.arena_cap = (unsigned)std::min<long long>((long long)K * (K + 1) / 2 + 64, 1ll << 18);
+  s.stride = mc_scratch_bytes(K, s.KW, s.arena_cap);
+  const long long want = (long long)sm_count * 2 * kMcSearchWarps;
+  s.nworkers = std::min<long long>(want, (long long)(free_b / 2 / s.stride));
+  s.nworkers = s.nworkers / kMcSearchWarps * kMcSearchWarps;
+  const double left = time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  const double left_ns = std::max(0.0, left) * 1e9;
+  s.limit_ns = left_ns >= 1.8e19 ? ~0ull : (unsigned long long)left_ns;
+  return s;
 }
 
 // bitset adjacency (built once per matrix) + k-core peel; core numbers and removal iterations come back to the host
@@ -1145,37 +1201,29 @@ int mc_solve(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, 
       if (ntasks > 0) {
         int K = 1;
         for (int32_t v : roots) K = std::max(K, (int)later[(size_t)v]);
-        const int KW = (K + 31) / 32;
-        const unsigned arena_cap = (unsigned)std::min<long long>((long long)K * (K + 1) / 2 + 64, 1ll << 18);
-        const size_t stride = mc_scratch_bytes(K, KW, arena_cap);
         size_t free_b = 0, total_b = 0;
         CLP_CUDA(h, cudaMemGetInfo(&free_b, &total_b));
-        const long long want = (long long)h->sm_count * 2 * kMcSearchWarps;
-        long long nworkers = std::min<long long>(want, (long long)(free_b / 2 / stride));
-        nworkers = nworkers / kMcSearchWarps * kMcSearchWarps;
-        if (nworkers < kMcSearchWarps)
+        const McSearchSetup ss = mc_search_setup(K, free_b, h->sm_count, time_limit_s, t0);
+        if (ss.nworkers < kMcSearchWarps)
           return fail(h, CLP_ERR_ALLOC, "maximum clique EXACT: not enough device memory for the search scratch");
-        CLP_CUDA(h, h->mc_scratch.ensure((size_t)nworkers * stride));
+        CLP_CUDA(h, h->mc_scratch.ensure((size_t)ss.nworkers * ss.stride));
         CLP_CUDA(h, cudaMemcpyAsync(L.roots, roots.data(), roots.size() * sizeof(int), cudaMemcpyHostToDevice, h->stream));
         CLP_CUDA(h, cudaMemcpyAsync(L.tprefix, tprefix.data(), tprefix.size() * sizeof(long long), cudaMemcpyHostToDevice, h->stream));
         CLP_CUDA(h, cudaMemcpyAsync(L.best, &best_s, sizeof(best_s), cudaMemcpyHostToDevice, h->stream));
         CLP_CUDA(h, cudaMemsetAsync(L.next, 0, sizeof(unsigned long long), h->stream));
         CLP_CUDA(h, cudaMemsetAsync(L.branches, 0, sizeof(unsigned long long), h->stream));
         CLP_CUDA(h, cudaMemsetAsync(L.flags, 0, 4 * sizeof(int), h->stream));
-        const double left = time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-        const double left_ns = std::max(0.0, left) * 1e9;
-        const unsigned long long limit_ns = left_ns >= 1.8e19 ? ~0ull : (unsigned long long)left_ns;
         McSearchArgs sa;
         sa.adj = adj; sa.m = (int)m; sa.W = W; sa.rnd = L.rnd; sa.roots = L.roots; sa.tprefix = L.tprefix;
-        sa.nroots = (int)roots.size(); sa.ntasks = ntasks; sa.K = K; sa.KW = KW; sa.arena_cap = arena_cap;
-        sa.scratch = h->mc_scratch.as<unsigned char>(); sa.stride = stride;
+        sa.nroots = (int)roots.size(); sa.ntasks = ntasks; sa.K = K; sa.KW = ss.KW; sa.arena_cap = ss.arena_cap;
+        sa.scratch = h->mc_scratch.as<unsigned char>(); sa.stride = ss.stride;
         sa.best = L.best; sa.next_task = L.next; sa.n_branches = L.branches; sa.flags = L.flags; sa.deadline = L.deadline;
         sa.replay_task = -1; sa.replay_size = 0; sa.nodes_out = L.nodes;
-        const size_t ssmem = (size_t)kMcSearchWarps * 2 * KW * sizeof(unsigned);
+        const size_t ssmem = (size_t)kMcSearchWarps * 2 * ss.KW * sizeof(unsigned);
         CLP_CUDA(h, cudaFuncSetAttribute(mc_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
         CLP_CUDA(h, cudaEventRecord(ev.e[5], h->stream));
-        mc_deadline_kernel<<<1, 1, 0, h->stream>>>(L.deadline, limit_ns);
-        mc_search_kernel<<<(unsigned)(nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, h->stream>>>(sa);
+        mc_deadline_kernel<<<1, 1, 0, h->stream>>>(L.deadline, ss.limit_ns);
+        mc_search_kernel<<<(unsigned)(ss.nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, h->stream>>>(sa);
         CLP_CUDA(h, cudaGetLastError());
         unsigned long long hb[2] = {0ull, 0ull};
         CLP_CUDA(h, cudaMemcpyAsync(&hb[0], L.best, 8, cudaMemcpyDeviceToHost, h->stream));
@@ -1187,7 +1235,7 @@ int mc_solve(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, 
         if (s > lb) {  // a task beat the heuristic: replay it for the nodes
           sa.replay_task = (long long)(0xffffffffu - (unsigned)(best_s & 0xffffffffull));
           sa.replay_size = s;
-          mc_search_kernel<<<1, 32, 2 * KW * sizeof(unsigned), h->stream>>>(sa);
+          mc_search_kernel<<<1, 32, 2 * ss.KW * sizeof(unsigned), h->stream>>>(sa);
           CLP_CUDA(h, cudaGetLastError());
           int got = 0;
           CLP_CUDA(h, cudaMemcpyAsync(&got, L.nodes + m, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
@@ -1243,26 +1291,19 @@ void clp_default_params(clp_params* p) {
 int clp_create(int device, int storage, clp_handle* out) {
   if (!out) return CLP_ERR_INVALID;
   *out = nullptr;
-  if (storage != CLP_STORE_F32 && storage != CLP_STORE_F64) return fail(nullptr, CLP_ERR_INVALID, "unknown storage type");
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0)
-    return fail(nullptr, CLP_ERR_CUDA, std::string("no usable CUDA device: ") + cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return fail(nullptr, CLP_ERR_INVALID, "device ordinal out of range");
+  if (storage != CLP_STORE_F32 && storage != CLP_STORE_F64) return fail<clp_handle_s>(nullptr, CLP_ERR_INVALID, "unknown storage type");
   cudaDeviceProp prop;
-  if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return fail(nullptr, CLP_ERR_CUDA, cudaGetErrorString(e));
-  if (prop.major != 9 || prop.minor != 0)
-    return fail(nullptr, CLP_ERR_CUDA, "clipper_b200 is built for sm_90a only; device is sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
-  if (!prop.cooperativeLaunch) return fail(nullptr, CLP_ERR_CUDA, "device lacks cooperative launch");
+  if (int rc = probe_device<clp_handle_s>(device, &prop)) return rc;
+  if (!prop.cooperativeLaunch) return fail<clp_handle_s>(nullptr, CLP_ERR_CUDA, "device lacks cooperative launch");
   clp_handle h = new (std::nothrow) clp_handle_s();
-  if (!h) return fail(nullptr, CLP_ERR_ALLOC, "host allocation failed");
+  if (!h) return fail<clp_handle_s>(nullptr, CLP_ERR_ALLOC, "host allocation failed");
   h->device = device; h->storage = storage; h->sm_count = prop.multiProcessorCount;
   clp_default_params(&h->prm);
   auto bail = [&](const char* what, cudaError_t ce) {
-    g_create_error = std::string(what) + ": " + cudaGetErrorString(ce);
     clp_destroy(h);
-    return CLP_ERR_CUDA;
+    return fail<clp_handle_s>(nullptr, CLP_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(ce));
   };
+  cudaError_t e;
   if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
   if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
   if ((e = cudaEventCreate(&h->ev0)) != cudaSuccess) return bail("cudaEventCreate", e);
@@ -1302,7 +1343,7 @@ int clp_destroy(clp_handle h) {
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
                     &h->mc_adj, &h->mc_work, &h->mc_scratch})
     b->release();
-  if (h->pinned) cudaFreeHost(h->pinned);
+  h->pinned.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream && h->own_stream) cudaStreamDestroy(h->stream);
@@ -1310,7 +1351,7 @@ int clp_destroy(clp_handle h) {
   return CLP_OK;
 }
 
-const char* clp_last_error(clp_handle h) { return h ? h->err.c_str() : g_create_error.c_str(); }
+const char* clp_last_error(clp_handle h) { return h ? h->err.c_str() : create_error<clp_handle_s>().c_str(); }
 
 int clp_set_params(clp_handle h, const clp_params* p) {
   if (!h || !p) return CLP_ERR_INVALID;
@@ -1500,7 +1541,7 @@ int clp_solve(clp_handle h, const double* u0, clp_solution* out, double* u_out, 
   const auto t0 = std::chrono::steady_clock::now();
   if (!h->has_matrix) return fail(h, CLP_ERR_INVALID, "solve() before any affinity matrix was scored or set");
   CLP_CUDA(h, cudaSetDevice(h->device));
-  double* stage = reinterpret_cast<double*>(reinterpret_cast<char*>(h->pinned) + 256);
+  double* stage = reinterpret_cast<double*>(h->pinned.as<char>() + 256);
   if (u0) {
     std::memcpy(stage, u0, (size_t)h->m * sizeof(double));
   } else {  // utils::randvec (ref utils.cpp:22-29): U[0,1) seeded from std::random_device
@@ -1749,35 +1790,24 @@ struct clp_batch_s {
   // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
   DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
   int prof_on = env_int("CLP_PROF_BATCH", 0);
-  void* pinned = nullptr; size_t pinned_cap = 0;
+  PinnedBuf pinned;         // the caller's other inputs, then the results
+  PinnedBuf pinned_points;  // D1 | D2 | A of scored problems (stage_points)
   int last_ctas = 0; long long last_scratch = 0, last_nnz = 0;
 };
 
 namespace {
-thread_local std::string g_batch_create_error;
-int bfail(clp_batch b, int code, const std::string& msg) {
-  if (b) b->err = msg; else g_batch_create_error = msg;
-  return code;
-}
-#define CLP_BCUDA(b, call)                                                                 \
-  do {                                                                                     \
-    cudaError_t e__ = (call);                                                              \
-    if (e__ != cudaSuccess)                                                                \
-      return bfail(b, e__ == cudaErrorMemoryAllocation ? CLP_ERR_ALLOC : CLP_ERR_CUDA,     \
-                   std::string(#call) + ": " + cudaGetErrorString(e__));                   \
-  } while (0)
 
 template <int KIND, int DD>
 int batch_launch(clp_batch b, BatchArgs& ba, int grid, size_t smem) {
-  CLP_BCUDA(b, cudaFuncSetAttribute(batch_solve_kernel<KIND, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CLP_CUDA(b, cudaFuncSetAttribute(batch_solve_kernel<KIND, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   batch_solve_kernel<KIND, DD><<<grid, kBatchThreads, smem, b->stream>>>(ba);
-  CLP_BCUDA(b, cudaGetLastError());
+  CLP_CUDA(b, cudaGetLastError());
   return CLP_OK;
 }
 template <int KIND, int DD>
 int batch_occupancy(clp_batch b, size_t smem, int* occ) {
-  CLP_BCUDA(b, cudaFuncSetAttribute(batch_solve_kernel<KIND, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, batch_solve_kernel<KIND, DD>, kBatchThreads, smem));
+  CLP_CUDA(b, cudaFuncSetAttribute(batch_solve_kernel<KIND, DD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, batch_solve_kernel<KIND, DD>, kBatchThreads, smem));
   return CLP_OK;
 }
 
@@ -1813,86 +1843,172 @@ void batch_results(const clp_params& P, const std::vector<Prob>& probs, const do
   }
 }
 
-int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const double* const* D1, const int64_t* n1,
-                const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
-                const double* const* u0, double p0, double p1, double p2, double p3, clp_solution* sols,
-                double* const* u_out, int32_t* const* nodes_out) {
-  if (!b) return CLP_ERR_INVALID;
-  if (nprob <= 0 || !D1 || !n1 || !D2 || !n2 || !m || !u0 || !sols) return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
-  if (!((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
-    return bfail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
-  const clp_params& P = b->prm;
-  if (P.rounding == CLP_ROUND_DSD) return bfail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
-  if (P.maxlsiters < 1) return bfail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
-  const auto t_begin = std::chrono::steady_clock::now();
-  CLP_BCUDA(b, cudaSetDevice(b->device));
-  // ---- problem table and concatenated inputs
-  std::vector<BatchProblem> probs((size_t)nprob);
-  long long nd1 = 0, nd2 = 0, na = 0, nu = 0;
-  int max_m = 1;
+// Inputs of the batch C-ABI calls.  Scored problems: D1, n1, D2, n2, A, m and the invariant's parameters p; graphs
+// given as strictly-upper CSC patterns: m, colptr and rowidx.
+struct BatchInput {
+  const double* const* D1 = nullptr; const int64_t* n1 = nullptr;
+  const double* const* D2 = nullptr; const int64_t* n2 = nullptr;
+  const int32_t* const* A = nullptr; const int64_t* m = nullptr;
+  const int64_t* const* colptr = nullptr; const int32_t* const* rowidx = nullptr;
+  double p[4] = {0.0, 0.0, 0.0, 0.0};
+};
+
+// Point clouds of a scored batch: checks every problem (association indices included), fills its BatchProblem (offsets
+// of D1, D2 and A; m = n1 n2 where A, A[p] or m[p] is empty: the all-to-all hypothesis; u_off 0) and uploads D1, D2
+// and A to in_d1, in_d2 and in_a through pinned_points.  *bytes: the bytes uploaded.
+int stage_points(clp_batch b, int dd, int32_t nprob, const BatchInput& in, std::vector<BatchProblem>& probs, size_t* bytes) {
+  probs.assign((size_t)nprob, BatchProblem{});
+  long long nd1 = 0, nd2 = 0, na = 0;
   for (int p = 0; p < nprob; ++p) {
     BatchProblem& q = probs[(size_t)p];
-    if (!D1[p] || !D2[p] || !u0[p] || n1[p] <= 0 || n2[p] <= 0) return bfail(b, CLP_ERR_INVALID, "bad problem in the batch (null data or u0)");
-    const bool a2a = (A == nullptr || A[p] == nullptr || m[p] == 0);
-    const long long mp = a2a ? (long long)n1[p] * n2[p] : (long long)m[p];
-    if (mp <= 0 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
-    q.d1_off = nd1; q.d2_off = nd2; q.a_off = a2a ? -1 : na; q.u_off = nu;
-    q.n1 = (int)n1[p]; q.n2 = (int)n2[p]; q.m = (int)mp; q.pad_ = 0;
-    nd1 += (long long)dd * n1[p]; nd2 += (long long)dd * n2[p]; if (!a2a) na += 2 * mp;
-    nu += (mp + 1) & ~1LL;  // every problem's u0 / u slot starts on a 16-byte boundary (the kernels use 16-byte loads)
-    max_m = std::max(max_m, (int)mp);
+    if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
+    const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
+    const long long mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
+    if (mp <= 0 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
+    if (!a2a)
+      for (long long i = 0; i < mp; ++i) {
+        const int32_t a0 = in.A[p][i], a1 = in.A[p][mp + i];
+        if (a0 < 0 || a0 >= in.n1[p] || a1 < 0 || a1 >= in.n2[p])
+          return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
+      }
+    q.d1_off = nd1; q.d2_off = nd2; q.a_off = a2a ? -1 : na;
+    q.n1 = (int)in.n1[p]; q.n2 = (int)in.n2[p]; q.m = (int)mp;
+    nd1 += (long long)dd * in.n1[p]; nd2 += (long long)dd * in.n2[p]; if (!a2a) na += 2 * mp;
   }
-  const size_t bytes_in = (size_t)(nd1 + nd2 + nu) * 8 + (size_t)na * 4 + (size_t)nprob * sizeof(BatchProblem);
-  const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
-  const size_t need = std::max(bytes_in, bytes_out) + 4096;
-  if (need > b->pinned_cap) {
-    if (b->pinned) { cudaFreeHost(b->pinned); b->pinned = nullptr; b->pinned_cap = 0; }
-    CLP_BCUDA(b, cudaMallocHost(&b->pinned, need));
-    b->pinned_cap = need;
-  }
-  char* hp = reinterpret_cast<char*>(b->pinned);
-  double* h_d1 = reinterpret_cast<double*>(hp);
+  *bytes = (size_t)(nd1 + nd2) * 8 + (size_t)na * 4;
+  CLP_CUDA(b, b->pinned_points.ensure(*bytes + 16));
+  double* h_d1 = b->pinned_points.as<double>();
   double* h_d2 = h_d1 + nd1;
-  double* h_u0 = h_d2 + nd2;
-  int32_t* h_a = reinterpret_cast<int32_t*>(h_u0 + nu);
-  BatchProblem* h_pr = reinterpret_cast<BatchProblem*>(reinterpret_cast<char*>(h_a) + (((size_t)na * 4 + 15) & ~(size_t)15));
+  int32_t* h_a = reinterpret_cast<int32_t*>(h_d2 + nd2);
   for (int p = 0; p < nprob; ++p) {
     const BatchProblem& q = probs[(size_t)p];
-    std::memcpy(h_d1 + q.d1_off, D1[p], (size_t)dd * q.n1 * 8);
-    std::memcpy(h_d2 + q.d2_off, D2[p], (size_t)dd * q.n2 * 8);
-    std::memcpy(h_u0 + q.u_off, u0[p], (size_t)q.m * 8);
-    if (q.a_off >= 0) std::memcpy(h_a + q.a_off, A[p], (size_t)2 * q.m * 4);
+    std::memcpy(h_d1 + q.d1_off, in.D1[p], (size_t)dd * q.n1 * 8);
+    std::memcpy(h_d2 + q.d2_off, in.D2[p], (size_t)dd * q.n2 * 8);
+    if (q.a_off >= 0) std::memcpy(h_a + q.a_off, in.A[p], (size_t)2 * q.m * 4);
   }
+  CLP_CUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
+  CLP_CUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
+  CLP_CUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
+  CLP_CUDA(b, cudaMemcpyAsync(b->in_d1.p, h_d1, (size_t)nd1 * 8, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->in_d2.p, h_d2, (size_t)nd2 * 8, cudaMemcpyHostToDevice, b->stream));
+  if (na) CLP_CUDA(b, cudaMemcpyAsync(b->in_a.p, h_a, (size_t)na * 4, cudaMemcpyHostToDevice, b->stream));
+  return CLP_OK;
+}
+
+// CTAs of a persistent batch launch, each with a scratch slot of `stride` bytes in `scratch` (stride 0: none): as many
+// as are co-resident at occ per SM, no more than there are problems, and no more than 80 % of the free device memory
+// holds slots for (the slots `scratch` holds count as free).  Ensures the scratch.  When not one slot fits, no_room is
+// the CLP_ERR_ALLOC message, or without one, one CTA is tried.
+int batch_grid(clp_batch b, int occ, int32_t nprob, size_t stride, DevBuf& scratch, const char* no_room, int* grid) {
+  long long g = std::min<long long>(nprob, (long long)occ * b->sm_count);
+  if (stride > 0) {
+    size_t free_b = 0, total_b = 0;
+    CLP_CUDA(b, cudaMemGetInfo(&free_b, &total_b));
+    const long long by_mem = (long long)((double)(free_b + scratch.cap) * 0.8 / (double)stride);
+    if (by_mem < 1 && no_room) return fail(b, CLP_ERR_ALLOC, no_room);
+    g = std::max<long long>(1, std::min(g, by_mem));
+    CLP_CUDA(b, scratch.ensure((size_t)g * stride));
+  }
+  *grid = (int)g;
+  return CLP_OK;
+}
+
+// Tail of the batched solves, from the launch on: reads u (nu doubles), the SolverOut and the kept-entry count of every
+// problem and the sync block into the staging buffer with one synchronisation, prints the CLP_PROF_BATCH line, maps the
+// device's error words (batch_matrix_solve_kernel sets flags, batch_solve_kernel error 2, both time out with error 1),
+// and fills the results.  `label` names the call and `first` its first in-kernel phase in the profile line.
+template <typename Prob>
+int batch_finish(clp_batch b, const char* label, const char* first, const std::vector<Prob>& probs, long long nu, int max_m,
+                 int grid, size_t stride, size_t bytes_in, std::chrono::steady_clock::time_point t_begin, clp_solution* sols,
+                 double* const* u_out, int32_t* const* nodes_out) {
+  const int nprob = (int)probs.size();
+  CLP_CUDA(b, cudaEventRecord(b->ev1, b->stream));
+  double* h_u = b->pinned.as<double>();
+  SolverOut* h_out = reinterpret_cast<SolverOut*>(h_u + nu);
+  unsigned int* h_nnz = reinterpret_cast<unsigned int*>(h_out + nprob);
+  SyncBlock h_sb;
+  CLP_CUDA(b, cudaMemcpyAsync(h_u, b->out_u.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(h_out, b->outs.p, (size_t)nprob * sizeof(SolverOut), cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(h_nnz, b->nnz.p, (size_t)nprob * 4, cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaStreamSynchronize(b->stream));
+  float ms = 0.f, up_ms = 0.f;
+  CLP_CUDA(b, cudaEventElapsedTime(&ms, b->ev0, b->ev1));
+  CLP_CUDA(b, cudaEventElapsedTime(&up_ms, b->ev_up, b->ev0));
+  if (b->prof_on) {
+    std::vector<unsigned long long> pr((size_t)nprob * 4);
+    CLP_CUDA(b, cudaMemcpy(pr.data(), b->prof.p, pr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    double acc[4] = {0, 0, 0, 0};
+    for (int p = 0; p < nprob; ++p) for (int q = 0; q < 4; ++q) acc[q] += 1e-6 * (double)pr[(size_t)p * 4 + q];
+    std::fprintf(stderr, "[clp %s prof] %d problems (max m %d), %d CTAs, upload %zu bytes %.3f ms, kernel %.3f ms; "
+                 "mean per problem: %s %.3f  build %.3f  solve %.3f  total %.3f ms\n",
+                 label, nprob, max_m, grid, bytes_in, up_ms, ms, first, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
+  }
+  if (h_sb.flags != 0) return fail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
+  if (h_sb.error == 2) return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
+  if (h_sb.error != 0) return fail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
+  b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)stride; b->last_nnz = 0;
+  for (int p = 0; p < nprob; ++p) b->last_nnz += h_nnz[p] / 2;
+  batch_results(b->prm, probs, h_u, h_out, ms, sols, u_out, nodes_out);
+  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
+  return CLP_OK;
+}
+
+int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& in, const double* const* u0, clp_solution* sols,
+                double* const* u_out, int32_t* const* nodes_out) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !in.D1 || !in.n1 || !in.D2 || !in.n2 || !in.m || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (!((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
+    return fail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
+  const clp_params& P = b->prm;
+  if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
+  if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
+  const auto t_begin = std::chrono::steady_clock::now();
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  // ---- problem table and concatenated inputs
+  for (int p = 0; p < nprob; ++p)
+    if (!u0[p]) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null u0)");
+  CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
+  std::vector<BatchProblem> probs;
+  size_t bytes_in = 0;
+  if (int rc = stage_points(b, dd, nprob, in, probs, &bytes_in)) return rc;
+  long long nu = 0;
+  int max_m = 1;
+  for (BatchProblem& q : probs) {
+    q.u_off = nu;
+    nu += (q.m + 1) & ~1LL;  // every problem's u0 / u slot starts on a 16-byte boundary (the kernels use 16-byte loads)
+    max_m = std::max(max_m, q.m);
+  }
+  const size_t bytes_table = (size_t)nu * 8 + (size_t)nprob * sizeof(BatchProblem);
+  const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
+  bytes_in += bytes_table;
+  CLP_CUDA(b, b->pinned.ensure(std::max(bytes_table, bytes_out) + 4096));
+  double* h_u0 = b->pinned.as<double>();
+  BatchProblem* h_pr = reinterpret_cast<BatchProblem*>(h_u0 + nu);
+  for (int p = 0; p < nprob; ++p) std::memcpy(h_u0 + probs[(size_t)p].u_off, u0[p], (size_t)probs[(size_t)p].m * 8);
   std::memcpy(h_pr, probs.data(), (size_t)nprob * sizeof(BatchProblem));
-  CLP_BCUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
-  CLP_BCUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
-  CLP_BCUDA(b, b->in_u0.ensure((size_t)nu * 8 + 16));
-  CLP_BCUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
-  CLP_BCUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
-  CLP_BCUDA(b, b->probs.ensure((size_t)nprob * sizeof(BatchProblem)));
-  CLP_BCUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
-  CLP_BCUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->in_d1.p, h_d1, (size_t)nd1 * 8, cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->in_d2.p, h_d2, (size_t)nd2 * 8, cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->in_u0.p, h_u0, (size_t)nu * 8, cudaMemcpyHostToDevice, b->stream));
-  if (na) CLP_BCUDA(b, cudaMemcpyAsync(b->in_a.p, h_a, (size_t)na * 4, cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->probs.p, h_pr, (size_t)nprob * sizeof(BatchProblem), cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  CLP_CUDA(b, b->in_u0.ensure((size_t)nu * 8 + 16));
+  CLP_CUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
+  CLP_CUDA(b, b->probs.ensure((size_t)nprob * sizeof(BatchProblem)));
+  CLP_CUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
+  CLP_CUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
+  CLP_CUDA(b, cudaMemcpyAsync(b->in_u0.p, h_u0, (size_t)nu * 8, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->probs.p, h_pr, (size_t)nprob * sizeof(BatchProblem), cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
   // ---- grid: as many CTAs as are co-resident (and as there are problems), each with its own scratch slot
   const BatchSmem bs = batch_smem_plan(max_m);
-  if ((long long)bs.total > (long long)b->smem_optin) return bfail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
+  if ((long long)bs.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
   int occ = 0;
   int rc = (kind == 1) ? batch_occupancy<1, 6>(b, bs.total, &occ) : (dd == 3 ? batch_occupancy<0, 3>(b, bs.total, &occ) : batch_occupancy<0, 2>(b, bs.total, &occ));
   if (rc) return rc;
-  if (occ < 1) return bfail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
+  if (occ < 1) return fail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
   const BatchLayout L = batch_layout(max_m, dd);
-  size_t free_b = 0, total_b = 0;
-  CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
-  const long long by_mem = (long long)((double)(free_b + b->scratch.cap) * 0.8 / (double)L.total);
-  int grid = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(nprob, (long long)occ * b->sm_count), by_mem));
-  CLP_BCUDA(b, b->scratch.ensure((size_t)grid * L.total));
+  int grid = 0;
+  rc = batch_grid(b, occ, nprob, L.total, b->scratch, nullptr, &grid);
+  if (rc) return rc;
   BatchArgs ba;
   std::memset(&ba, 0, sizeof(ba));
   ba.prob = b->probs.as<BatchProblem>(); ba.nprob = nprob;
@@ -1901,44 +2017,14 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const double* cons
   ba.next = reinterpret_cast<int*>(&b->sync.as<SyncBlock>()->counts[0]);
   ba.scratch = b->scratch.as<unsigned char>(); ba.scratch_stride = L.total;
   ba.max_m = max_m; ba.kind = kind; ba.dd = dd;
-  ba.prm.tol_u = P.tol_u; ba.prm.tol_F = P.tol_F; ba.prm.beta = P.beta; ba.prm.eps = P.eps;
-  ba.prm.maxiniters = P.maxiniters; ba.prm.maxoliters = P.maxoliters; ba.prm.maxlsiters = P.maxlsiters;
-  ba.prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
-  ba.p0 = p0; ba.p1 = p1; ba.p2 = p2; ba.p3 = p3; ba.affinityeps = P.affinityeps;
+  ba.prm = solver_params(P);
+  ba.p0 = in.p[0]; ba.p1 = in.p[1]; ba.p2 = in.p[2]; ba.p3 = in.p[3]; ba.affinityeps = P.affinityeps;
   ba.sb = b->sync.as<SyncBlock>(); ba.spin_limit = 4LL * 1900000000LL;
-  if (b->prof_on) { CLP_BCUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
-  CLP_BCUDA(b, cudaEventRecord(b->ev0, b->stream));
+  if (b->prof_on) { CLP_CUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   rc = (kind == 1) ? batch_launch<1, 6>(b, ba, grid, bs.total) : (dd == 3 ? batch_launch<0, 3>(b, ba, grid, bs.total) : batch_launch<0, 2>(b, ba, grid, bs.total));
   if (rc) return rc;
-  CLP_BCUDA(b, cudaEventRecord(b->ev1, b->stream));
-  // ---- results
-  double* h_u = reinterpret_cast<double*>(hp);
-  SolverOut* h_out = reinterpret_cast<SolverOut*>(h_u + nu);
-  unsigned int* h_nnz = reinterpret_cast<unsigned int*>(h_out + nprob);
-  SyncBlock h_sb;
-  CLP_BCUDA(b, cudaMemcpyAsync(h_u, b->out_u.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(h_out, b->outs.p, (size_t)nprob * sizeof(SolverOut), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(h_nnz, b->nnz.p, (size_t)nprob * 4, cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
-  float ms = 0.f;
-  CLP_BCUDA(b, cudaEventElapsedTime(&ms, b->ev0, b->ev1));
-  if (b->prof_on) {
-    std::vector<unsigned long long> pr((size_t)nprob * 4);
-    CLP_BCUDA(b, cudaMemcpy(pr.data(), b->prof.p, pr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    double acc[4] = {0, 0, 0, 0};
-    for (int p = 0; p < nprob; ++p) for (int q = 0; q < 4; ++q) acc[q] += 1e-6 * (double)pr[(size_t)p * 4 + q];
-    std::fprintf(stderr, "[clp batch prof] %d problems (max m %d), %d CTAs, kernel %.3f ms; mean per problem: score %.3f  build %.3f  solve %.3f  total %.3f ms\n",
-                 nprob, max_m, grid, ms, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
-  }
-  if (h_sb.error == 2) return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
-  if (h_sb.error != 0) return bfail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
-  b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)L.total; b->last_nnz = 0;
-  for (int p = 0; p < nprob; ++p) b->last_nnz += h_nnz[p] / 2;
-  batch_results(P, probs, h_u, h_out, ms, sols, u_out, nodes_out);
-  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
-  for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
-  return CLP_OK;
+  return batch_finish(b, "batch", "score", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
 }
 
 // ---- batched solve of given matrices (clp_batch_matrix.cuh) -------------------------------------------------------
@@ -1979,9 +2065,9 @@ void mat_check_copy(int p, const char* what, int which, long long m, const int64
 }
 
 int batch_launch_matrices(clp_batch b, BatchMatArgs& ba, int grid, size_t smem) {
-  CLP_BCUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CLP_CUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   batch_matrix_solve_kernel<<<grid, kBatchThreads, smem, b->stream>>>(ba);
-  CLP_BCUDA(b, cudaGetLastError());
+  CLP_CUDA(b, cudaGetLastError());
   return CLP_OK;
 }
 
@@ -1990,12 +2076,12 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
                          const double* const* vC, const double* const* u0, clp_solution* sols, double* const* u_out,
                          int32_t* const* nodes_out) {
   if (!b) return CLP_ERR_INVALID;
-  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC || !u0 || !sols) return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   const clp_params& P = b->prm;
-  if (P.rounding == CLP_ROUND_DSD) return bfail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
-  if (P.maxlsiters < 1) return bfail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
+  if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
+  if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
   const auto t_begin = std::chrono::steady_clock::now();
-  CLP_BCUDA(b, cudaSetDevice(b->device));
+  CLP_CUDA(b, cudaSetDevice(b->device));
   // ---- problem table: sizes and column pointers (the entries are checked while they are copied)
   std::vector<BatchMatProblem> probs((size_t)nprob);
   long long ncp = 0, ne = 0, nu = 0;
@@ -2004,18 +2090,18 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
     BatchMatProblem& q = probs[(size_t)p];
     const std::string tag = "problem " + std::to_string(p) + ": ";
     const long long mp = (long long)m[p];
-    if (mp < 1 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, tag + "batched problems need 1 <= m <= 4096");
-    if (!u0[p]) return bfail(b, CLP_ERR_INVALID, tag + "null u0");
+    if (mp < 1 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, tag + "batched problems need 1 <= m <= 4096");
+    if (!u0[p]) return fail(b, CLP_ERR_INVALID, tag + "null u0");
     long long nz[2] = {0, 0};
     for (int which = 0; which < 2; ++which) {
       const int64_t* cp = which ? cpC[p] : cpM[p];
       const char* what = which ? "C" : "M";
-      if (!cp || cp[0] != 0) return bfail(b, CLP_ERR_INVALID, tag + what + " column pointer must start at 0");
+      if (!cp || cp[0] != 0) return fail(b, CLP_ERR_INVALID, tag + what + " column pointer must start at 0");
       for (long long c = 0; c < mp; ++c)
-        if (cp[c + 1] < cp[c]) return bfail(b, CLP_ERR_INVALID, tag + what + " column pointer decreases at column " + std::to_string(c));
+        if (cp[c + 1] < cp[c]) return fail(b, CLP_ERR_INVALID, tag + what + " column pointer decreases at column " + std::to_string(c));
       nz[which] = cp[mp];
       if (nz[which] > 0 && (which ? (!riC[p] || !vC[p]) : (!riM[p] || !vM[p])))
-        return bfail(b, CLP_ERR_INVALID, tag + what + " has entries but null row indices or values");
+        return fail(b, CLP_ERR_INVALID, tag + what + " has entries but null row indices or values");
     }
     q.cpM_off = ncp; q.cpC_off = ncp + mp + 1; ncp += 2 * (mp + 1);
     q.eM_off = ne; q.eC_off = ne + nz[0]; ne += nz[0] + nz[1];
@@ -2028,13 +2114,8 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   const size_t o_pr = (o_ri + (size_t)ne * 4 + 15) & ~(size_t)15;
   const size_t bytes_in = o_pr + (size_t)nprob * sizeof(BatchMatProblem);
   const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
-  const size_t need = std::max(bytes_in, bytes_out) + 4096;
-  if (need > b->pinned_cap) {
-    if (b->pinned) { cudaFreeHost(b->pinned); b->pinned = nullptr; b->pinned_cap = 0; }
-    CLP_BCUDA(b, cudaMallocHost(&b->pinned, need));
-    b->pinned_cap = need;
-  }
-  char* hp = reinterpret_cast<char*>(b->pinned);
+  CLP_CUDA(b, b->pinned.ensure(std::max(bytes_in, bytes_out) + 4096));
+  char* hp = b->pinned.as<char>();
   int64_t* h_cp = reinterpret_cast<int64_t*>(hp);
   double* h_val = reinterpret_cast<double*>(hp + o_val);
   double* h_u0 = reinterpret_cast<double*>(hp + o_u0);
@@ -2065,31 +2146,28 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   }
   for (int kind = 0; kind < 3; ++kind)
     for (int p = 0; p < nprob; ++p)
-      if (chk[(size_t)p].kind == kind) return bfail(b, kind == 0 ? CLP_ERR_INVALID : CLP_ERR_UNSUPPORTED, chk[(size_t)p].msg);
+      if (chk[(size_t)p].kind == kind) return fail(b, kind == 0 ? CLP_ERR_INVALID : CLP_ERR_UNSUPPORTED, chk[(size_t)p].msg);
   std::memcpy(hp + o_pr, probs.data(), (size_t)nprob * sizeof(BatchMatProblem));
   // the device copy keeps the staging offsets (u0 starts on a 16-byte boundary, the base is cudaMalloc-aligned)
-  CLP_BCUDA(b, b->mat_in.ensure(bytes_in + 16));
-  CLP_BCUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
-  CLP_BCUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
-  CLP_BCUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
-  CLP_BCUDA(b, cudaEventRecord(b->ev_up, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->mat_in.p, hp, bytes_in, cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  CLP_CUDA(b, b->mat_in.ensure(bytes_in + 16));
+  CLP_CUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
+  CLP_CUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
+  CLP_CUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
+  CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->mat_in.p, hp, bytes_in, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
   // ---- grid: as many CTAs as are co-resident (and as there are problems), each with its own scratch slot
   const BatchSmem bs = batch_smem_plan(max_m);
-  if ((long long)bs.total > (long long)b->smem_optin) return bfail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
+  if ((long long)bs.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
   int occ = 0;
-  CLP_BCUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs.total));
-  CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, batch_matrix_solve_kernel, kBatchThreads, bs.total));
-  if (occ < 1) return bfail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
+  CLP_CUDA(b, cudaFuncSetAttribute(batch_matrix_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs.total));
+  CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, batch_matrix_solve_kernel, kBatchThreads, bs.total));
+  if (occ < 1) return fail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
   const BatchLayout L = batch_layout(max_m, 0, /*points*/ false);
-  size_t free_b = 0, total_b = 0;
-  CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
-  const long long by_mem = (long long)((double)(free_b + b->scratch.cap) * 0.8 / (double)L.total);
-  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(nprob, (long long)occ * b->sm_count), by_mem));
-  CLP_BCUDA(b, b->scratch.ensure((size_t)grid * L.total));
+  int grid = 0;
+  if (int rc = batch_grid(b, occ, nprob, L.total, b->scratch, nullptr, &grid)) return rc;
   const char* din = b->mat_in.as<char>();
   BatchMatArgs ba;
   std::memset(&ba, 0, sizeof(ba));
@@ -2100,187 +2178,113 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   ba.next = reinterpret_cast<int*>(&b->sync.as<SyncBlock>()->counts[0]);
   ba.scratch = b->scratch.as<unsigned char>(); ba.scratch_stride = L.total;
   ba.max_m = max_m;
-  ba.prm.tol_u = P.tol_u; ba.prm.tol_F = P.tol_F; ba.prm.beta = P.beta; ba.prm.eps = P.eps;
-  ba.prm.maxiniters = P.maxiniters; ba.prm.maxoliters = P.maxoliters; ba.prm.maxlsiters = P.maxlsiters;
-  ba.prm.rescale_u0 = P.rescale_u0 ? 1 : 0;
+  ba.prm = solver_params(P);
   ba.sb = b->sync.as<SyncBlock>(); ba.spin_limit = 4LL * 1900000000LL;
-  if (b->prof_on) { CLP_BCUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
-  CLP_BCUDA(b, cudaEventRecord(b->ev0, b->stream));
+  if (b->prof_on) { CLP_CUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   if (int rc = batch_launch_matrices(b, ba, grid, bs.total)) return rc;
-  CLP_BCUDA(b, cudaEventRecord(b->ev1, b->stream));
-  // ---- results
-  double* h_u = reinterpret_cast<double*>(hp);
-  SolverOut* h_out = reinterpret_cast<SolverOut*>(h_u + nu);
-  unsigned int* h_nnz = reinterpret_cast<unsigned int*>(h_out + nprob);
-  SyncBlock h_sb;
-  CLP_BCUDA(b, cudaMemcpyAsync(h_u, b->out_u.p, (size_t)nu * 8, cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(h_out, b->outs.p, (size_t)nprob * sizeof(SolverOut), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(h_nnz, b->nnz.p, (size_t)nprob * 4, cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
-  float ms = 0.f, up_ms = 0.f;
-  CLP_BCUDA(b, cudaEventElapsedTime(&ms, b->ev0, b->ev1));
-  CLP_BCUDA(b, cudaEventElapsedTime(&up_ms, b->ev_up, b->ev0));
-  if (b->prof_on) {
-    std::vector<unsigned long long> pr((size_t)nprob * 4);
-    CLP_BCUDA(b, cudaMemcpy(pr.data(), b->prof.p, pr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    double acc[4] = {0, 0, 0, 0};
-    for (int p = 0; p < nprob; ++p) for (int q = 0; q < 4; ++q) acc[q] += 1e-6 * (double)pr[(size_t)p * 4 + q];
-    std::fprintf(stderr, "[clp batch matrices prof] %d problems (max m %d), %d CTAs, upload %zu bytes %.3f ms, kernel %.3f ms; "
-                 "mean per problem: scatter %.3f  build %.3f  solve %.3f  total %.3f ms\n",
-                 nprob, max_m, grid, bytes_in, up_ms, ms, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
-  }
-  if (h_sb.flags != 0) return bfail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
-  if (h_sb.error != 0) return bfail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
-  b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)L.total; b->last_nnz = 0;
-  for (int p = 0; p < nprob; ++p) b->last_nnz += h_nnz[p] / 2;
-  batch_results(P, probs, h_u, h_out, ms, sols, u_out, nodes_out);
-  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
-  for (int p = 0; p < nprob; ++p) sols[p].t = wall / nprob;
-  return CLP_OK;
+  return batch_finish(b, "batch matrices", "scatter", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
 }
 
 // ---- batched maximum clique (clp_batch_clique.cuh) ----------------------------------------------------------------
 // kind 0 / 1: scored problems (EuclideanDistance d = 2, 3 / PointNormalDistance); kind 2: graphs given as strictly-upper
 // CSC patterns.  Phase A, then for EXACT with a positive time limit phases B and C: two host synchronisations.
-struct McBatchInput {
-  const double* const* D1 = nullptr; const int64_t* n1 = nullptr;
-  const double* const* D2 = nullptr; const int64_t* n2 = nullptr;
-  const int32_t* const* A = nullptr; const int64_t* m = nullptr;
-  const int64_t* const* colptr = nullptr; const int32_t* const* rowidx = nullptr;
-  double p[4] = {0.0, 0.0, 0.0, 0.0};
-};
-
 const void* mcb_prepare_fn(int kind, int dd) {
   if (kind == kMcbKindGraph) return (const void*)mc_batch_prepare_kernel<kMcbKindGraph, 1>;
   if (kind == 1) return (const void*)mc_batch_prepare_kernel<1, 6>;
   return dd == 3 ? (const void*)mc_batch_prepare_kernel<0, 3> : (const void*)mc_batch_prepare_kernel<0, 2>;
 }
 
-int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatchInput& in, int method, double time_limit_s,
+int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& in, int method, double time_limit_s,
                      clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
   if (!b) return CLP_ERR_INVALID;
   const auto t_begin = std::chrono::steady_clock::now();
-  if (nprob <= 0 || !infos || !in.m) return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
-  if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return bfail(b, CLP_ERR_INVALID, "unknown maximum-clique method");
+  if (nprob <= 0 || !infos || !in.m) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return fail(b, CLP_ERR_INVALID, "unknown maximum-clique method");
   const bool graph = kind == kMcbKindGraph;
   if (graph ? (!in.colptr || !in.rowidx) : (!in.D1 || !in.n1 || !in.D2 || !in.n2))
-    return bfail(b, CLP_ERR_INVALID, "bad batch arguments");
+    return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   if (!graph && !((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
-    return bfail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
+    return fail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
   const bool search = method == CLP_MC_EXACT && time_limit_s > 0;
-  CLP_BCUDA(b, cudaSetDevice(b->device));
-  // ---- problem table, per-problem regions and the concatenated inputs, validated here
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  // ---- problem table and per-problem regions; scored inputs are checked and uploaded by stage_points, graphs here
   std::vector<McBatchProblem> probs((size_t)nprob);
-  long long nd1 = 0, nd2 = 0, na = 0, ne = 0, nadj = 0, nv = 0, nt = 0;
+  if (!graph) {
+    std::vector<BatchProblem> pts;
+    size_t bytes_pts = 0;
+    if (int rc = stage_points(b, dd, nprob, in, pts, &bytes_pts)) return rc;
+    for (int p = 0; p < nprob; ++p) probs[(size_t)p].sp = pts[(size_t)p];
+  }
+  long long ne = 0, nadj = 0, nv = 0, nt = 0;
   int max_m = 1;
   for (int p = 0; p < nprob; ++p) {
     McBatchProblem& q = probs[(size_t)p];
-    std::memset(&q, 0, sizeof(q));
-    long long mp = 0;
     if (graph) {
-      mp = (long long)in.m[p];
-      if (mp <= 0 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 vertices");
+      const long long mp = (long long)in.m[p];
+      if (mp <= 0 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 vertices");
       const int64_t* cp = in.colptr[p];
       const int32_t* ri = in.rowidx[p];
-      if (!cp || cp[0] != 0) return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr must start at 0");
+      if (!cp || cp[0] != 0) return fail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr must start at 0");
       for (long long c = 0; c < mp; ++c) {
-        if (cp[c + 1] < cp[c]) return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr decreases");
+        if (cp[c + 1] < cp[c]) return fail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": colptr decreases");
         for (int64_t k = cp[c]; k < cp[c + 1]; ++k)
           if (!ri || ri[k] < 0 || ri[k] >= c)
-            return bfail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": entry (" + std::to_string(ri ? ri[k] : -1) + ", " +
-                                                  std::to_string(c) + ") is not strictly upper (row < column)");
+            return fail(b, CLP_ERR_INVALID, "graph " + std::to_string(p) + ": entry (" + std::to_string(ri ? ri[k] : -1) + ", " +
+                                                std::to_string(c) + ") is not strictly upper (row < column)");
       }
       q.e_off = ne; q.ne = cp[mp];
       ne += cp[mp];
-    } else {
-      if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return bfail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
-      const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
-      mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
-      if (mp <= 0 || mp > kBatchMaxM) return bfail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
-      if (!a2a)
-        for (long long i = 0; i < mp; ++i) {
-          const int32_t a0 = in.A[p][i], a1 = in.A[p][mp + i];
-          if (a0 < 0 || a0 >= in.n1[p] || a1 < 0 || a1 >= in.n2[p])
-            return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
-        }
-      q.sp.d1_off = nd1; q.sp.d2_off = nd2; q.sp.a_off = a2a ? -1 : na; q.sp.u_off = 0;
-      q.sp.n1 = (int)in.n1[p]; q.sp.n2 = (int)in.n2[p];
-      nd1 += (long long)dd * in.n1[p]; nd2 += (long long)dd * in.n2[p]; if (!a2a) na += 2 * mp;
+      q.sp.m = (int)mp;
     }
-    q.sp.m = (int)mp;
+    const long long mp = q.sp.m;
     const long long W = (mp + 31) / 32;
     q.adj_off = nadj; nadj += mp * W;
     q.v_off = nv; nv += (4 * mp + 1 + 3) & ~3LL;
     q.t_off = nt; nt += mp + 1;
     max_m = std::max(max_m, (int)mp);
   }
-  // ---- inputs through the pinned staging buffer
-  const size_t bytes_in = (size_t)(nd1 + nd2) * 8 + (size_t)(na + 2 * ne) * 4 + (size_t)nprob * sizeof(McBatchProblem) + 64;
+  // ---- edges and the problem table through the pinned staging buffer
+  const size_t bytes_in = (size_t)(2 * ne) * 4 + (size_t)nprob * sizeof(McBatchProblem) + 64;
   const size_t bytes_out = (size_t)nv * 4 + (size_t)nprob * (sizeof(McBatchOut) + 3 * 8 + 2 * 4) + 64;
-  const size_t need = std::max(bytes_in, bytes_out) + 4096;
-  if (need > b->pinned_cap) {
-    if (b->pinned) { cudaFreeHost(b->pinned); b->pinned = nullptr; b->pinned_cap = 0; }
-    CLP_BCUDA(b, cudaMallocHost(&b->pinned, need));
-    b->pinned_cap = need;
-  }
-  char* hp = reinterpret_cast<char*>(b->pinned);
-  double* h_d1 = reinterpret_cast<double*>(hp);
-  double* h_d2 = h_d1 + nd1;
-  int32_t* h_a = reinterpret_cast<int32_t*>(h_d2 + nd2);
-  int32_t* h_e = h_a + na;
-  McBatchProblem* h_pr = reinterpret_cast<McBatchProblem*>(reinterpret_cast<char*>(h_e) + (((size_t)(2 * ne) * 4 + 15) & ~(size_t)15));
-  for (int p = 0; p < nprob; ++p) {
-    const McBatchProblem& q = probs[(size_t)p];
-    if (graph) {
+  CLP_CUDA(b, b->pinned.ensure(std::max(bytes_in, bytes_out) + 4096));
+  char* hp = b->pinned.as<char>();
+  int32_t* h_e = reinterpret_cast<int32_t*>(hp);
+  McBatchProblem* h_pr = reinterpret_cast<McBatchProblem*>(hp + (((size_t)(2 * ne) * 4 + 15) & ~(size_t)15));
+  if (graph)
+    for (int p = 0; p < nprob; ++p) {
+      const McBatchProblem& q = probs[(size_t)p];
       const int64_t* cp = in.colptr[p];
       int32_t* e = h_e + 2 * q.e_off;
       for (int c = 0; c < q.sp.m; ++c)
         for (int64_t k = cp[c]; k < cp[c + 1]; ++k) { *e++ = in.rowidx[p][k]; *e++ = c; }
-    } else {
-      std::memcpy(h_d1 + q.sp.d1_off, in.D1[p], (size_t)dd * q.sp.n1 * 8);
-      std::memcpy(h_d2 + q.sp.d2_off, in.D2[p], (size_t)dd * q.sp.n2 * 8);
-      if (q.sp.a_off >= 0) std::memcpy(h_a + q.sp.a_off, in.A[p], (size_t)2 * q.sp.m * 4);
     }
-  }
   std::memcpy(h_pr, probs.data(), (size_t)nprob * sizeof(McBatchProblem));
-  CLP_BCUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
-  CLP_BCUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
-  CLP_BCUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
-  CLP_BCUDA(b, b->mc_edges.ensure((size_t)ne * 8 + 16));
-  CLP_BCUDA(b, b->mc_probs.ensure((size_t)nprob * sizeof(McBatchProblem)));
-  CLP_BCUDA(b, b->mc_adj.ensure((size_t)nadj * 4 + 16));
-  CLP_BCUDA(b, b->mc_vint.ensure((size_t)nv * 4 + 16));
-  CLP_BCUDA(b, b->mc_tpre.ensure((size_t)nt * 8 + 16));
-  CLP_BCUDA(b, b->mc_out.ensure((size_t)nprob * sizeof(McBatchOut)));
-  if (nd1) CLP_BCUDA(b, cudaMemcpyAsync(b->in_d1.p, h_d1, (size_t)nd1 * 8, cudaMemcpyHostToDevice, b->stream));
-  if (nd2) CLP_BCUDA(b, cudaMemcpyAsync(b->in_d2.p, h_d2, (size_t)nd2 * 8, cudaMemcpyHostToDevice, b->stream));
-  if (na) CLP_BCUDA(b, cudaMemcpyAsync(b->in_a.p, h_a, (size_t)na * 4, cudaMemcpyHostToDevice, b->stream));
-  if (ne) CLP_BCUDA(b, cudaMemcpyAsync(b->mc_edges.p, h_e, (size_t)ne * 8, cudaMemcpyHostToDevice, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(b->mc_probs.p, h_pr, (size_t)nprob * sizeof(McBatchProblem), cudaMemcpyHostToDevice, b->stream));
-  if (graph) CLP_BCUDA(b, cudaMemsetAsync(b->mc_adj.p, 0, (size_t)nadj * 4, b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->mc_out.p, 0, (size_t)nprob * sizeof(McBatchOut), b->stream));
-  CLP_BCUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  CLP_CUDA(b, b->mc_edges.ensure((size_t)ne * 8 + 16));
+  CLP_CUDA(b, b->mc_probs.ensure((size_t)nprob * sizeof(McBatchProblem)));
+  CLP_CUDA(b, b->mc_adj.ensure((size_t)nadj * 4 + 16));
+  CLP_CUDA(b, b->mc_vint.ensure((size_t)nv * 4 + 16));
+  CLP_CUDA(b, b->mc_tpre.ensure((size_t)nt * 8 + 16));
+  CLP_CUDA(b, b->mc_out.ensure((size_t)nprob * sizeof(McBatchOut)));
+  if (ne) CLP_CUDA(b, cudaMemcpyAsync(b->mc_edges.p, h_e, (size_t)ne * 8, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->mc_probs.p, h_pr, (size_t)nprob * sizeof(McBatchProblem), cudaMemcpyHostToDevice, b->stream));
+  if (graph) CLP_CUDA(b, cudaMemsetAsync(b->mc_adj.p, 0, (size_t)nadj * 4, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->mc_out.p, 0, (size_t)nprob * sizeof(McBatchOut), b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
 
   // ---- phase A: one CTA per problem, as many CTAs as are co-resident and, for scored problems, fit their scratch
   const McbSmem sm = mcb_smem_plan(max_m);
-  if ((long long)sm.total > (long long)b->smem_optin) return bfail(b, CLP_ERR_UNSUPPORTED, "batched maximum clique: shared memory plan exceeds the device limit");
+  if ((long long)sm.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batched maximum clique: shared memory plan exceeds the device limit");
   const void* fn = mcb_prepare_fn(kind, dd);
-  CLP_BCUDA(b, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.total));
+  CLP_CUDA(b, cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sm.total));
   int occ = 0;
-  CLP_BCUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kBatchThreads, sm.total));
-  if (occ < 1) return bfail(b, CLP_ERR_CUDA, "batched maximum-clique kernel does not fit an SM");
-  long long grid = std::min<long long>(nprob, (long long)occ * b->sm_count);
-  size_t pstride = 0;
-  if (!graph) {
-    pstride = mcb_layout(max_m, dd).total;
-    size_t free_b = 0, total_b = 0;
-    CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
-    const long long by_mem = (long long)((double)(free_b + b->mc_pscratch.cap) * 0.8 / (double)pstride);
-    if (by_mem < 1) return bfail(b, CLP_ERR_ALLOC, "batched maximum clique: not enough device memory for one problem's scoring scratch");
-    grid = std::min(grid, by_mem);
-    CLP_BCUDA(b, b->mc_pscratch.ensure((size_t)grid * pstride));
-  }
+  CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kBatchThreads, sm.total));
+  if (occ < 1) return fail(b, CLP_ERR_CUDA, "batched maximum-clique kernel does not fit an SM");
+  const size_t pstride = graph ? 0 : mcb_layout(max_m, dd).total;
+  int grid = 0;
+  if (int rc = batch_grid(b, occ, nprob, pstride, b->mc_pscratch,
+                          "batched maximum clique: not enough device memory for one problem's scoring scratch", &grid))
+    return rc;
   McBatchArgs ba;
   std::memset(&ba, 0, sizeof(ba));
   ba.prob = b->mc_probs.as<McBatchProblem>(); ba.nprob = nprob; ba.run_heu = method != CLP_MC_KCORE ? 1 : 0; ba.build_tasks = search ? 1 : 0;
@@ -2292,20 +2296,20 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatch
   ba.error = &b->sync.as<SyncBlock>()->error;
   ba.scratch = b->mc_pscratch.as<unsigned char>(); ba.scratch_stride = pstride; ba.max_m = max_m;
   McEvents ev;
-  for (cudaEvent_t& x : ev.e) CLP_BCUDA(b, cudaEventCreate(&x));
-  CLP_BCUDA(b, cudaEventRecord(ev.e[0], b->stream));
+  for (cudaEvent_t& x : ev.e) CLP_CUDA(b, cudaEventCreate(&x));
+  CLP_CUDA(b, cudaEventRecord(ev.e[0], b->stream));
   {
     void* args[] = {&ba};
-    CLP_BCUDA(b, cudaLaunchKernel(fn, dim3((unsigned)grid), dim3(kBatchThreads), args, sm.total, b->stream));
+    CLP_CUDA(b, cudaLaunchKernel(fn, dim3((unsigned)grid), dim3(kBatchThreads), args, sm.total, b->stream));
   }
-  CLP_BCUDA(b, cudaEventRecord(ev.e[1], b->stream));
+  CLP_CUDA(b, cudaEventRecord(ev.e[1], b->stream));
   std::vector<McBatchOut> outs((size_t)nprob);
   SyncBlock h_sb;
-  CLP_BCUDA(b, cudaMemcpyAsync(outs.data(), b->mc_out.p, (size_t)nprob * sizeof(McBatchOut), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
-  if (h_sb.error == 2) return bfail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
-  b->last_ctas = (int)grid;
+  CLP_CUDA(b, cudaMemcpyAsync(outs.data(), b->mc_out.p, (size_t)nprob * sizeof(McBatchOut), cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaStreamSynchronize(b->stream));
+  if (h_sb.error == 2) return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
+  b->last_ctas = grid;
   b->last_scratch = (long long)grid * (long long)pstride;
 
   // ---- phases B and C: the search over the tasks of every problem, then the replays
@@ -2336,20 +2340,15 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatch
     if (total > 0) {
       int K = 1;
       for (int p : porder) K = std::max(K, outs[(size_t)p].K);
-      const int KW = (K + 31) / 32;
-      const unsigned arena_cap = (unsigned)std::min<long long>((long long)K * (K + 1) / 2 + 64, 1ll << 18);
-      const size_t stride = mc_scratch_bytes(K, KW, arena_cap);
       size_t free_b = 0, total_b = 0;
-      CLP_BCUDA(b, cudaMemGetInfo(&free_b, &total_b));
-      const long long want = (long long)b->sm_count * 2 * kMcSearchWarps;
-      long long nworkers = std::min<long long>(want, (long long)((free_b + b->mc_sscratch.cap) / 2 / stride));
-      nworkers = nworkers / kMcSearchWarps * kMcSearchWarps;
-      if (nworkers < kMcSearchWarps) return bfail(b, CLP_ERR_ALLOC, "batched maximum clique EXACT: not enough device memory for the search scratch");
-      CLP_BCUDA(b, b->mc_sscratch.ensure((size_t)nworkers * stride));
+      CLP_CUDA(b, cudaMemGetInfo(&free_b, &total_b));
+      const McSearchSetup ss = mc_search_setup(K, free_b + b->mc_sscratch.cap, b->sm_count, time_limit_s, t_begin);
+      if (ss.nworkers < kMcSearchWarps) return fail(b, CLP_ERR_ALLOC, "batched maximum clique EXACT: not enough device memory for the search scratch");
+      CLP_CUDA(b, b->mc_sscratch.ensure((size_t)ss.nworkers * ss.stride));
       const int nseg = (int)seg_width.size();
       // device state: best | branches | done [nprob] 8-byte, next, deadline, flags [2 nprob]; rounds: porder, segments
-      CLP_BCUDA(b, b->mc_state.ensure((size_t)nprob * 3 * 8 + 16 + (size_t)nprob * 8 + 16));
-      CLP_BCUDA(b, b->mc_rounds.ensure((size_t)(nprob + 1) * 4 + (size_t)(2 * nseg + 1) * 8 + (size_t)nseg * 4 + 64));
+      CLP_CUDA(b, b->mc_state.ensure((size_t)nprob * 3 * 8 + 16 + (size_t)nprob * 8 + 16));
+      CLP_CUDA(b, b->mc_rounds.ensure((size_t)(nprob + 1) * 4 + (size_t)(2 * nseg + 1) * 8 + (size_t)nseg * 4 + 64));
       unsigned long long* d_best = b->mc_state.as<unsigned long long>();
       unsigned long long* d_br = d_best + nprob;
       unsigned long long* d_done = d_br + nprob;
@@ -2362,40 +2361,37 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatch
       int* d_porder = d_seg_width + nseg;
       std::vector<unsigned long long> best0((size_t)nprob);
       for (int p = 0; p < nprob; ++p) best0[(size_t)p] = mc_key((unsigned)outs[(size_t)p].lb, 0u);
-      CLP_BCUDA(b, cudaMemcpyAsync(d_best, best0.data(), (size_t)nprob * 8, cudaMemcpyHostToDevice, b->stream));
-      CLP_BCUDA(b, cudaMemsetAsync(d_br, 0, (size_t)nprob * 2 * 8 + 16 + (size_t)nprob * 8, b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_start, seg_start.data(), seg_start.size() * 8, cudaMemcpyHostToDevice, b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_k0, seg_k0.data(), seg_k0.size() * 8, cudaMemcpyHostToDevice, b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(d_seg_width, seg_width.data(), seg_width.size() * 4, cudaMemcpyHostToDevice, b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(d_porder, porder.data(), porder.size() * 4, cudaMemcpyHostToDevice, b->stream));
-      const double left = time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
-      const double left_ns = std::max(0.0, left) * 1e9;
-      const unsigned long long limit_ns = left_ns >= 1.8e19 ? ~0ull : (unsigned long long)left_ns;
+      CLP_CUDA(b, cudaMemcpyAsync(d_best, best0.data(), (size_t)nprob * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_CUDA(b, cudaMemsetAsync(d_br, 0, (size_t)nprob * 2 * 8 + 16 + (size_t)nprob * 8, b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(d_seg_start, seg_start.data(), seg_start.size() * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(d_seg_k0, seg_k0.data(), seg_k0.size() * 8, cudaMemcpyHostToDevice, b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(d_seg_width, seg_width.data(), seg_width.size() * 4, cudaMemcpyHostToDevice, b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(d_porder, porder.data(), porder.size() * 4, cudaMemcpyHostToDevice, b->stream));
       McBatchSearchArgs sa;
       sa.prob = b->mc_probs.as<McBatchProblem>(); sa.out = b->mc_out.as<McBatchOut>();
       sa.adj = b->mc_adj.as<unsigned>(); sa.vint = b->mc_vint.as<int>(); sa.tpre = b->mc_tpre.as<long long>();
       sa.porder = d_porder; sa.seg_start = d_seg_start; sa.seg_k0 = d_seg_k0; sa.seg_width = d_seg_width; sa.nseg = nseg;
-      sa.total = total; sa.K = K; sa.KW = KW; sa.arena_cap = arena_cap;
-      sa.scratch = b->mc_sscratch.as<unsigned char>(); sa.stride = stride;
+      sa.total = total; sa.K = K; sa.KW = ss.KW; sa.arena_cap = ss.arena_cap;
+      sa.scratch = b->mc_sscratch.as<unsigned char>(); sa.stride = ss.stride;
       sa.best = d_best; sa.branches = d_br; sa.done = d_done; sa.flags = d_flags; sa.next = d_next; sa.deadline = d_deadline;
-      const size_t ssmem = (size_t)kMcSearchWarps * 2 * KW * sizeof(unsigned);
-      CLP_BCUDA(b, cudaFuncSetAttribute(mc_batch_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
-      CLP_BCUDA(b, cudaFuncSetAttribute(mc_batch_replay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
-      CLP_BCUDA(b, cudaEventRecord(ev.e[2], b->stream));
-      mc_deadline_kernel<<<1, 1, 0, b->stream>>>(d_deadline, limit_ns);
-      mc_batch_search_kernel<<<(unsigned)(nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, b->stream>>>(sa);
-      CLP_BCUDA(b, cudaGetLastError());
-      const long long rgrid = std::min<long long>(nworkers / kMcSearchWarps, (nprob + kMcSearchWarps - 1) / kMcSearchWarps);
+      const size_t ssmem = (size_t)kMcSearchWarps * 2 * ss.KW * sizeof(unsigned);
+      CLP_CUDA(b, cudaFuncSetAttribute(mc_batch_search_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+      CLP_CUDA(b, cudaFuncSetAttribute(mc_batch_replay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ssmem));
+      CLP_CUDA(b, cudaEventRecord(ev.e[2], b->stream));
+      mc_deadline_kernel<<<1, 1, 0, b->stream>>>(d_deadline, ss.limit_ns);
+      mc_batch_search_kernel<<<(unsigned)(ss.nworkers / kMcSearchWarps), kMcSearchWarps * 32, ssmem, b->stream>>>(sa);
+      CLP_CUDA(b, cudaGetLastError());
+      const long long rgrid = std::min<long long>(ss.nworkers / kMcSearchWarps, (nprob + kMcSearchWarps - 1) / kMcSearchWarps);
       mc_batch_replay_kernel<<<(unsigned)rgrid, kMcSearchWarps * 32, ssmem, b->stream>>>(sa, nprob);
-      CLP_BCUDA(b, cudaGetLastError());
-      CLP_BCUDA(b, cudaEventRecord(ev.e[3], b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(h_best, d_best, (size_t)nprob * 3 * 8, cudaMemcpyDeviceToHost, b->stream));
-      CLP_BCUDA(b, cudaMemcpyAsync(h_flags, d_flags, (size_t)nprob * 8, cudaMemcpyDeviceToHost, b->stream));
-      b->last_scratch += (long long)nworkers * (long long)stride;
+      CLP_CUDA(b, cudaGetLastError());
+      CLP_CUDA(b, cudaEventRecord(ev.e[3], b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(h_best, d_best, (size_t)nprob * 3 * 8, cudaMemcpyDeviceToHost, b->stream));
+      CLP_CUDA(b, cudaMemcpyAsync(h_flags, d_flags, (size_t)nprob * 8, cudaMemcpyDeviceToHost, b->stream));
+      b->last_scratch += (long long)ss.nworkers * (long long)ss.stride;
     }
   }
-  CLP_BCUDA(b, cudaMemcpyAsync(h_v, b->mc_vint.p, (size_t)nv * 4, cudaMemcpyDeviceToHost, b->stream));
-  CLP_BCUDA(b, cudaStreamSynchronize(b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(h_v, b->mc_vint.p, (size_t)nv * 4, cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaStreamSynchronize(b->stream));
   if (total > 0) search_ms = mc_elapsed(ev.e[2], ev.e[3]);
 
   // ---- results per problem
@@ -2429,13 +2425,13 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const McBatch
           timed_out = h_done[p] < (unsigned long long)o.ntasks ? 1 : 0;
           proven = (!timed_out && h_flags[2 * p + 1] == 0) ? 1 : 0;
           if (s > lb && (size < s || size > m))
-            return bfail(b, CLP_ERR_CUDA, "batched maximum clique: search replay did not reproduce its clique (problem " + std::to_string(p) + ")");
-          if (s <= lb && size != lb) return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+            return fail(b, CLP_ERR_CUDA, "batched maximum clique: search replay did not reproduce its clique (problem " + std::to_string(p) + ")");
+          if (s <= lb && size != lb) return fail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
         } else if (size != lb) {
-          return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+          return fail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
         }
       } else if (size != lb) {
-        return bfail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
+        return fail(b, CLP_ERR_CUDA, "batched maximum clique: heuristic replay disagrees with its winner");
       }
       nodes.assign(vnodes, vnodes + size);
       std::sort(nodes.begin(), nodes.end());
@@ -2466,22 +2462,17 @@ extern "C" {
 int clp_batch_create(int device, clp_batch* out) {
   if (!out) return CLP_ERR_INVALID;
   *out = nullptr;
-  int ndev = 0;
-  cudaError_t e = cudaGetDeviceCount(&ndev);
-  if (e != cudaSuccess || ndev == 0) return bfail(nullptr, CLP_ERR_CUDA, std::string("no usable CUDA device: ") + cudaGetErrorString(e));
-  if (device < 0 || device >= ndev) return bfail(nullptr, CLP_ERR_INVALID, "device ordinal out of range");
   cudaDeviceProp prop;
-  if ((e = cudaGetDeviceProperties(&prop, device)) != cudaSuccess) return bfail(nullptr, CLP_ERR_CUDA, cudaGetErrorString(e));
-  if (prop.major != 9 || prop.minor != 0) return bfail(nullptr, CLP_ERR_CUDA, "clipper_b200 is built for sm_90a only");
+  if (int rc = probe_device<clp_batch_s>(device, &prop)) return rc;
   clp_batch b = new (std::nothrow) clp_batch_s();
-  if (!b) return bfail(nullptr, CLP_ERR_ALLOC, "host allocation failed");
+  if (!b) return fail<clp_batch_s>(nullptr, CLP_ERR_ALLOC, "host allocation failed");
   b->device = device; b->sm_count = prop.multiProcessorCount;
   clp_default_params(&b->prm);
   auto bail = [&](const char* what, cudaError_t ce) {
-    g_batch_create_error = std::string(what) + ": " + cudaGetErrorString(ce);
     clp_batch_destroy(b);
-    return CLP_ERR_CUDA;
+    return fail<clp_batch_s>(nullptr, CLP_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(ce));
   };
+  cudaError_t e;
   if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
   if ((e = cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("cudaStreamCreate", e);
   if ((e = cudaEventCreate(&b->ev0)) != cudaSuccess) return bail("cudaEventCreate", e);
@@ -2500,7 +2491,8 @@ int clp_batch_destroy(clp_batch b) {
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
                     &b->mc_pscratch, &b->mc_sscratch})
     d->release();
-  if (b->pinned) cudaFreeHost(b->pinned);
+  b->pinned.release();
+  b->pinned_points.release();
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
   if (b->ev_up) cudaEventDestroy(b->ev_up);
@@ -2509,11 +2501,11 @@ int clp_batch_destroy(clp_batch b) {
   return CLP_OK;
 }
 
-const char* clp_batch_last_error(clp_batch b) { return b ? b->err.c_str() : g_batch_create_error.c_str(); }
+const char* clp_batch_last_error(clp_batch b) { return b ? b->err.c_str() : create_error<clp_batch_s>().c_str(); }
 
 int clp_batch_set_params(clp_batch b, const clp_params* p) {
   if (!b || !p) return CLP_ERR_INVALID;
-  if (p->rounding < 0 || p->rounding > 2) return bfail(b, CLP_ERR_INVALID, "unknown rounding mode");
+  if (p->rounding < 0 || p->rounding > 2) return fail(b, CLP_ERR_INVALID, "unknown rounding mode");
   b->prm = *p;
   return CLP_OK;
 }
@@ -2522,27 +2514,29 @@ int clp_batch_solve_euclidean(clp_batch b, int32_t nprob, int32_t d, const doubl
                               const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
                               const double* const* u0, double sigma, double epsilon, double mindist,
                               clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
-  try { return batch_solve(b, 0, d, nprob, D1, n1, D2, n2, A, m, u0, sigma, epsilon, mindist, 0.0, sols, u_out, nodes_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  BatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
+  in.p[0] = sigma; in.p[1] = epsilon; in.p[2] = mindist;
+  return guarded(b, [&] { return batch_solve(b, 0, d, nprob, in, u0, sols, u_out, nodes_out); });
 }
 
 int clp_batch_solve_pointnormal(clp_batch b, int32_t nprob, const double* const* D1, const int64_t* n1,
                                 const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
                                 const double* const* u0, double sigp, double epsp, double sign, double epsn,
                                 clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
-  try { return batch_solve(b, 1, 6, nprob, D1, n1, D2, n2, A, m, u0, sigp, epsp, sign, epsn, sols, u_out, nodes_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  BatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
+  in.p[0] = sigp; in.p[1] = epsp; in.p[2] = sign; in.p[3] = epsn;
+  return guarded(b, [&] { return batch_solve(b, 1, 6, nprob, in, u0, sols, u_out, nodes_out); });
 }
 
 int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
                              const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
                              const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
                              const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
-  try { return batch_solve_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, u0, sols, u_out, nodes_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  return guarded(b, [&] {
+    return batch_solve_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, u0, sols, u_out, nodes_out);
+  });
 }
 
 int clp_batch_info(clp_batch b, int32_t* n_ctas, int64_t* scratch_bytes, int64_t* nnz_upper_total) {
@@ -2557,34 +2551,28 @@ int clp_batch_max_clique_euclidean(clp_batch b, int32_t nprob, int32_t d, const 
                                    const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
                                    double sigma, double epsilon, double mindist, int method, double time_limit_s,
                                    clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
-  McBatchInput in;
+  BatchInput in;
   in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
   in.p[0] = sigma; in.p[1] = epsilon; in.p[2] = mindist;
-  try { return batch_max_clique(b, 0, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  return guarded(b, [&] { return batch_max_clique(b, 0, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
 }
 
 int clp_batch_max_clique_pointnormal(clp_batch b, int32_t nprob, const double* const* D1, const int64_t* n1,
                                      const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
                                      double sigp, double epsp, double sign, double epsn, int method, double time_limit_s,
                                      clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
-  McBatchInput in;
+  BatchInput in;
   in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m;
   in.p[0] = sigp; in.p[1] = epsp; in.p[2] = sign; in.p[3] = epsn;
-  try { return batch_max_clique(b, 1, 6, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  return guarded(b, [&] { return batch_max_clique(b, 1, 6, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
 }
 
 int clp_batch_max_clique_graphs(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* colptr,
                                 const int32_t* const* rowidx, int method, double time_limit_s, clp_mc_info* infos,
                                 int32_t* const* nodes_out, int32_t* const* core_out) {
-  McBatchInput in;
+  BatchInput in;
   in.m = m; in.colptr = colptr; in.rowidx = rowidx;
-  try { return batch_max_clique(b, kMcbKindGraph, 0, nprob, in, method, time_limit_s, infos, nodes_out, core_out); }
-  catch (const std::bad_alloc&) { return bfail(b, CLP_ERR_ALLOC, "host allocation failed"); }
-  catch (...) { return bfail(b, CLP_ERR_INVALID, "internal error"); }
+  return guarded(b, [&] { return batch_max_clique(b, kMcbKindGraph, 0, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
 }
 
 }  // extern "C"
