@@ -58,6 +58,13 @@ struct PinnedBuf {  // page-locked host staging: the asynchronous copies from an
   template <typename U> U* as() const { return reinterpret_cast<U*>(p); }
 };
 
+// layout of the compact copy (compact_shape): whole rows for the resident sweep (one segment W = ld wide, column
+// indices; padding entries point at column m of the staged vector), else the plan's column segments (byte offsets)
+struct CompactShape {
+  bool resident = false;
+  int nseg = 0, W = 0;
+};
+
 }  // namespace
 
 static int env_int(const char* name, int dflt) {
@@ -111,13 +118,8 @@ struct clp_handle_s {
   // resident-vector solver (clp_resident.cuh): the default whenever the whole trial vector fits shared memory
   int res_G = 0;                                    // CTAs of the resident kernels for the current matrix
   int res_NI = 0;
-  bool compact_resident = false;                    // layout of the current compact copy: full rows + column indices
   int smem_optin = 0;                               // cudaDevAttrMaxSharedMemoryPerBlockOptin
-  bool score_pending = false;                       // a scoring launch's error flag has not been read back yet
-  bool counts_fused = false;                        // sp_ptr4 already holds the counts of the current matrix
-  long long counts_m = 0; int counts_rows_pad = 0, counts_nseg = 0, counts_W = 0;  // ... which was this one
   int pack = env_int("CLP_PACK", 1);              // resident layout of plain fp32 matrices with 4-byte entries (0: always 6 bytes)
-  bool counts_win = false;                          // the fused counts came with the occupied-window bitmap (sp_win)
 
   // solver workspace
   DevBuf vecs;    // V_SLOTS x mpad doubles: U0 U1 MV0 MV1 CV0 CV1 (local only)
@@ -144,6 +146,7 @@ struct clp_handle_s {
   DevBuf sp_hist, sp_bsum;  // compact build: class histograms of the row tiles | block sums of the scans
   DevBuf sp_win, res_wcol;  // packed layout: occupied 16-column windows per row | members' columns where every warp starts
   unsigned long long sp_nnz = 0, sp_nnz_real = 0;
+  CompactShape sp_shape{};  // layout of the last compact copy built
   SparseView sp{};
   Plan2 plan2{};
   Dense2Buffers d2{};
@@ -186,6 +189,12 @@ int fail(H* h, int code, const std::string& msg) {
 
 inline long long round_up(long long x, long long q) { return (x + q - 1) / q * q; }
 int reset_sync(clp_handle h);
+
+// f(T{}) with T the handle's storage type (float or double)
+template <typename F>
+decltype(auto) with_storage(clp_handle h, F&& f) {
+  return h->storage == CLP_STORE_F64 ? f(double{}) : f(float{});
+}
 
 // nothing may propagate out of an extern "C" entry point (the library is loaded into Python and into C callers)
 template <typename H, typename F>
@@ -335,7 +344,7 @@ ResKernels res_kernels(clp_handle h) {
   return {(const void*)solver_resident_kernel<T, false>, (const void*)matvec_resident_kernel<T, S>, S::NT};
 }
 int res_warps(clp_handle h) {
-  return (h->storage == CLP_STORE_F64 ? res_kernels<double>(h) : res_kernels<float>(h)).NT / 32;
+  return with_storage(h, [&](auto t) { return res_kernels<decltype(t)>(h); }).NT / 32;
 }
 
 // On-chip tables behind the plan's minimum: the CTA's piece table and per-row solver state, sized for 1.5x the mean
@@ -362,11 +371,14 @@ unsigned int res_launch_smem(clp_handle h) {
   return res_smem_plan((int)h->m, res_warps(h), pc, sc).total_ext;
 }
 
-// can the resident solver take a problem of this size on this handle?
-bool resident_possible(clp_handle h, long long m) {
-  if (m > kResMaxM || m > 65535) return false;
-  if (!(h->dense_mode == 4 || h->dense_mode == 6)) return false;
-  return (long long)res_smem_plan((int)m, kResThreads / 32).total <= (long long)h->smem_optin;
+// The one decision of the compact layout for the current m, requested mode and plan: whole rows when the resident
+// solver can take the problem (mode 4 or 6, the vector fits shared memory), else the plan's column segments.  The
+// scoring kernel counts for this layout and the build cuts along it; the plan's NSEG and W depend on m only.
+CompactShape compact_shape(clp_handle h) {
+  const bool resident = h->m <= kResMaxM && h->m <= 65535 && (h->dense_mode == 4 || h->dense_mode == 6) &&
+                        (long long)res_smem_plan((int)h->m, kResThreads / 32).total <= (long long)h->smem_optin;
+  if (resident) return {true, 1, (int)h->ld};
+  return {false, h->plan.NSEG, h->plan.W};
 }
 
 template <typename T>
@@ -447,42 +459,38 @@ unsigned packed_fill_grid(clp_handle h, long long items) {
   return (unsigned)std::max<long long>(1, (warps + kDevFillWarps - 1) / kDevFillWarps);
 }
 
-// Called once the dense store holds the new matrix: pick the sweep (dense mode) and build what it needs.
+// What a scoring launch hands to the compact build of the same call; every other build passes {}.
+struct ScoreHandoff {
+  // the sync block still carries the scoring launch's error flag (read back with the build's totals: one host
+  // synchronisation per scoring call) and zeroed counters
+  bool after_score = false;
+  // the scoring kernel counted the kept entries for compact_shape(h) into sp_ptr4, and for the packed layout also
+  // the occupied windows (sp_win) and the exponent range: the build skips its counting pass
+  bool counted = false;
+};
+
+// Called once the dense store holds the new matrix: build the compact copy of layout s.
 template <typename T>
-int build_sparse(clp_handle h, bool force, bool resident) {
-  // layout of the compact copy: the column segments of the Plan (segmented sweep, byte offsets), or one segment =
-  // the whole row (resident sweep, column indices; padding entries point at column m of the staged vector)
-  Plan p = h->plan;
-  if (resident) { p.NSEG = 1; p.W = (int)h->ld; }
-  const int nseg = p.NSEG;
+int build_sparse(clp_handle h, bool force, const CompactShape& s, ScoreHandoff ho) {
+  const int nseg = s.nseg;
   const long long nptr = (long long)nseg * (h->rows_pad + 1);
-  // counts produced by the scoring kernel (scored matrices are "plain"): only trusted for the very matrix and
-  // segmentation they were counted for
-  const bool fused = h->counts_fused && h->counts_m == h->m && h->counts_rows_pad == h->rows_pad &&
-                     h->counts_nseg == nseg && h->counts_W == p.W;
-  const bool fused_win = fused && h->counts_win;
-  h->counts_fused = false; h->counts_win = false;
-  // right after a scoring launch the sync block still carries that launch's error flag (checked below, with the
-  // totals: one host synchronisation per scoring call) and zeroed counters; otherwise start from a clean block
-  const bool after_score = h->score_pending;
-  h->score_pending = false;
-  if (!after_score) { if (int rc = reset_sync(h)) return rc; }
+  if (!ho.after_score) { if (int rc = reset_sync(h)) return rc; }
   SyncBlock* sb = h->sync.as<SyncBlock>();
   const T* M = h->Mbuf.as<T>();
   const unsigned blocks = (unsigned)(((size_t)h->rows_pad * 32 + 255) / 256);
   // packed layout (whole rows, fp32): the counts also describe the occupied 16-column windows and the exponent range;
   // the sort and the item lengths then decide on the device whether the fillers count (PackCount::on), the host reads
   // the same decision back with the totals
-  const bool want_pack = resident && h->pack_candidate() && (!fused || fused_win);
+  const bool want_pack = s.resident && h->pack_candidate();
   const int wwords = h->wwords();
-  if (!fused) {
+  if (!ho.counted) {
     CLP_CUDA(h, h->sp_ptr4.ensure((size_t)nptr * sizeof(unsigned int)));
     CLP_CUDA(h, cudaMemsetAsync(h->sp_ptr4.p, 0, (size_t)nptr * sizeof(unsigned int), h->stream));
     if (want_pack) {
       CLP_CUDA(h, h->sp_win.ensure((size_t)h->rows_pad * wwords * sizeof(unsigned int)));
       CLP_CUDA(h, cudaMemsetAsync(h->sp_win.p, 0, (size_t)h->rows_pad * wwords * sizeof(unsigned int), h->stream));
     }
-    sparse_count_kernel<T><<<blocks, 256, 0, h->stream>>>(M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg,
+    sparse_count_kernel<T><<<blocks, 256, 0, h->stream>>>(M, h->ld, (int)h->m, h->rows, h->rows_pad, s.W, nseg,
                                                           h->sp_ptr4.as<unsigned int>(), &sb->counts[0],
                                                           want_pack ? h->sp_win.as<unsigned int>() : nullptr, wwords, &sb->expo[0]);
     CLP_CUDA(h, cudaGetLastError());
@@ -493,7 +501,7 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   const long long nitem = (long long)nseg * (NI + 1);
   CLP_CUDA(h, h->sp_rowid.ensure((size_t)nseg * h->rows_pad * sizeof(unsigned int)));
   CLP_CUDA(h, h->sp_item.ensure((size_t)nitem * sizeof(unsigned int)));
-  const int nb = p.W / 4 + 2;  // possible slice lengths in chunks
+  const int nb = s.W / 4 + 2;  // possible slice lengths in chunks
   const int ntile = (h->rows_pad + kSortTile - 1) / kSortTile;
   const long long nhist = (long long)nseg * nb * ntile;
   const long long nblk = (std::max(nhist, nitem) + kScanBlock - 1) / kScanBlock;
@@ -511,7 +519,7 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   };
   const dim3 tiles((unsigned)ntile, (unsigned)nseg);
   sell_hist_kernel<<<tiles, kSortTile, (size_t)nb * sizeof(unsigned int), h->stream>>>(
-      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, ntile, h->sp_hist.as<unsigned int>(), fused ? &sb->counts[0] : nullptr, pc);
+      h->sp_ptr4.as<unsigned int>(), h->rows_pad, nb, ntile, h->sp_hist.as<unsigned int>(), ho.counted ? &sb->counts[0] : nullptr, pc);
   CLP_CUDA(h, cudaGetLastError());
   if (int rc = scan(h->sp_hist.as<unsigned int>(), nhist, nullptr)) return rc;
   sell_place_kernel<<<tiles, kSortTile, (size_t)nb * sizeof(unsigned int), h->stream>>>(
@@ -525,7 +533,7 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   CLP_CUDA(h, cudaMemcpyAsync(&host[0], total4_d, sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   CLP_CUDA(h, cudaMemcpyAsync(&host[1], &sb->counts[0], 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->stream));
   if (want_pack) CLP_CUDA(h, cudaMemcpyAsync(hexpo, &sb->expo[0], sizeof(hexpo), cudaMemcpyDeviceToHost, h->stream));
-  if (after_score) CLP_CUDA(h, cudaMemcpyAsync(&host_err, &sb->error, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  if (ho.after_score) CLP_CUDA(h, cudaMemcpyAsync(&host_err, &sb->error, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CLP_CUDA(h, cudaStreamSynchronize(h->stream));
   if (host_err == 2) return fail(h, CLP_ERR_INVALID, "association index out of range of D1/D2");
   const unsigned long long n4 = host[0];
@@ -546,20 +554,20 @@ int build_sparse(clp_handle h, bool force, bool resident) {
   if (h->sp.packed) {  // whole rows (nseg = 1), fp32 only
     if constexpr (sizeof(T) == 4)
       sparse_fill_items_kernel<T, true><<<packed_fill_grid(h, NI), kDevFillWarps * 32, 0, h->stream>>>(
-          M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
+          M, h->ld, (int)h->m, h->rows, h->rows_pad, s.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
           h->sp_val.as<T>(), nullptr, 0, 0u, next_item, bias);
   } else {
     const long long nwarp = (long long)nseg * NI;  // one warp per item
     sparse_fill_items_kernel<T><<<(unsigned)((nwarp + kDevFillWarps - 1) / kDevFillWarps), kDevFillWarps * 32, 0, h->stream>>>(
-        M, h->ld, (int)h->m, h->rows, h->rows_pad, p.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
-        h->sp_val.as<T>(), h->sp_col.as<unsigned short>(), resident ? 0 : 3, resident ? (unsigned int)h->m : kZeroSlot, nullptr);
+        M, h->ld, (int)h->m, h->rows, h->rows_pad, s.W, nseg, h->sp_item.as<unsigned int>(), h->sp_rowid.as<unsigned int>(),
+        h->sp_val.as<T>(), h->sp_col.as<unsigned short>(), s.resident ? 0 : 3, s.resident ? (unsigned int)h->m : kZeroSlot, nullptr);
   }
   CLP_CUDA(h, cudaGetLastError());
   h->sp.val = h->sp_val.p; h->sp.off16 = h->sp.packed ? nullptr : h->sp_col.as<unsigned short>();
   h->sp.itemptr = h->sp_item.as<unsigned int>(); h->sp.rowid = h->sp_rowid.as<unsigned int>(); h->sp.rows_pad = h->rows_pad;
   // byte-balanced contiguous item range of every CTA (depends on the grid size: rebuilt with the plan)
-  int G = p.G;
-  if (resident) {
+  int G = h->plan.G;
+  if (s.resident) {
     // one fat CTA per SM; small problems use fewer CTAs -- every CTA should stream at least ~32 KB per sweep, since
     // with more CTAs the per-evaluation exchange costs more than the sweep saves; shards sharing a GPU honour the cap
     h->res_NI = NI;
@@ -584,7 +592,7 @@ int build_sparse(clp_handle h, bool force, bool resident) {
     res_warp_cols_kernel<<<(unsigned)((G * NW * 32 + 255) / 256), 256, 0, h->stream>>>(h->sp, G, NW, h->res_wcol.as<int>());
     CLP_CUDA(h, cudaGetLastError());
   }
-  h->compact_resident = resident;
+  h->sp_shape = s;
   return CLP_OK;
 }
 
@@ -604,15 +612,21 @@ int set_plan_for(clp_handle h, int mode) {
   return CLP_OK;
 }
 
-int finalize_matrix_impl(clp_handle h) {
+// the plan of the requested mode, before a matrix decides the effective one: auto (4) plans for the compact sweep
+int plan_requested(clp_handle h) { return set_plan_for(h, h->dense_mode == 3 || h->dense_mode == 4 ? 3 : h->dense_mode); }
+
+// modes 3, 4 and 6 try the compact copy first
+bool compact_requested(clp_handle h) { return h->dense_mode == 3 || h->dense_mode == 4 || h->dense_mode == 6; }
+
+int finalize_matrix_impl(clp_handle h, ScoreHandoff ho) {
   int eff = h->dense_mode;
-  if (eff == 3 || eff == 4 || eff == 6) {
+  if (compact_requested(h)) {
     h->sp.plain = 0; h->sp.packed = 0;
-    if (int rc = set_plan_for(h, 3)) return rc;  // column segmentation (NSEG, W) depends on m only
-    const bool resident = (eff != 3) && resident_possible(h, h->m);
+    if (int rc = set_plan_for(h, 3)) return rc;
+    const CompactShape s = compact_shape(h);
     const bool force = (eff == 3) || (eff == 6);
-    const int rc = (h->storage == CLP_STORE_F64) ? build_sparse<double>(h, force, resident) : build_sparse<float>(h, force, resident);
-    if (rc == CLP_OK) eff = resident ? 6 : 3;
+    const int rc = with_storage(h, [&](auto t) { return build_sparse<decltype(t)>(h, force, s, ho); });
+    if (rc == CLP_OK) eff = s.resident ? 6 : 3;
     else if (rc == kKeepDense) eff = (h->world > 1) ? 0 : 2;
     else return rc;
   }
@@ -623,7 +637,7 @@ int finalize_matrix_impl(clp_handle h) {
   return CLP_OK;
 }
 
-int finalize_matrix(clp_handle h) { return guarded(h, [&] { return finalize_matrix_impl(h); }); }
+int finalize_matrix(clp_handle h, ScoreHandoff ho = {}) { return guarded(h, [&] { return finalize_matrix_impl(h, ho); }); }
 
 // (re)allocate the matrix store for problem size m under the current shard config
 int ensure_matrix(clp_handle h, long long m) {
@@ -639,7 +653,6 @@ int ensure_matrix(clp_handle h, long long m) {
   h->ld = round_up(m, 128);
   h->mpad = round_up(m, 128);
   CLP_CUDA(h, h->Mbuf.ensure((size_t)h->rows_pad * (size_t)h->ld * h->esize()));
-  h->plan = make_plan(m, h->rows_pad, h->grid_for(h->ctas_for(h->dense_mode == 3 || h->dense_mode == 4 ? 3 : h->dense_mode)));
   // workspace
   CLP_CUDA(h, h->vecs.ensure((size_t)V_SLOTS * h->mpad * sizeof(double)));
   {
@@ -650,8 +663,7 @@ int ensure_matrix(clp_handle h, long long m) {
       h->shard_ready = false;
     }
   }
-  CLP_CUDA(h, h->parts.ensure((size_t)2 * h->plan.NSEG * h->rows_pad * sizeof(double)));
-  CLP_CUDA(h, h->small.ensure(((size_t)kMaxSeg + (size_t)2 * h->plan.G * kRedVals) * sizeof(double)));
+  if (int rc = plan_requested(h)) return rc;
   CLP_CUDA(h, h->result.ensure(256 + (size_t)h->mpad * sizeof(double)));
   CLP_CUDA(h, h->u0dev.ensure((size_t)h->mpad * sizeof(double)));
   CLP_CUDA(h, h->ybuf.ensure((size_t)4 * h->mpad * sizeof(double)));
@@ -727,18 +739,17 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   a.A0 = Ad; a.A1 = Ad + m;
   a.M = h->Mbuf.p; a.ld = h->ld; a.m = (int)m; a.row0 = h->row0; a.rows = h->rows; a.rows_pad = h->rows_pad;
   a.F1 = h->F12.as<float4>(); a.F2 = a.F1 + m; a.scale_bits = &sb->scale_bits;
-  const bool res_layout = resident_possible(h, m);  // the compact copy will use one segment = the whole row
-  const int cnt_nseg = res_layout ? 1 : h->plan.NSEG, cnt_W = res_layout ? (int)h->ld : h->plan.W;
-  a.cnt = nullptr; a.W = cnt_W; a.win = nullptr; a.wwords = 0; a.expo = nullptr;
-  h->counts_fused = false;
-  const bool compact_next = (h->dense_mode == 3 || h->dense_mode == 4 || h->dense_mode == 6);
-  if (compact_next && screened_scoring(h, kind, d)) {
+  const CompactShape s = compact_shape(h);  // the layout the build of this call cuts (finalize_matrix_impl)
+  const bool compact = compact_requested(h);
+  a.cnt = nullptr; a.W = s.W; a.win = nullptr; a.wwords = 0; a.expo = nullptr;
+  if (compact && screened_scoring(h, kind, d)) {
     // the screened scoring kernel also counts the kept entries per (segment, row): first pass of the compact build
-    const size_t nptr = (size_t)cnt_nseg * (h->rows_pad + 1);
+    const size_t nptr = (size_t)s.nseg * (h->rows_pad + 1);
     CLP_CUDA(h, h->sp_ptr4.ensure(nptr * sizeof(unsigned int)));
     CLP_CUDA(h, cudaMemsetAsync(h->sp_ptr4.p, 0, nptr * sizeof(unsigned int), h->stream));
     a.cnt = h->sp_ptr4.as<unsigned int>();
-    if (res_layout && h->pack_candidate()) {  // and what the packed layout needs (occupied windows, exponent range)
+    // and what the packed layout needs (occupied windows, exponent range), under the build's own condition (want_pack)
+    if (s.resident && h->pack_candidate()) {
       const size_t nw = (size_t)h->rows_pad * h->wwords();
       CLP_CUDA(h, h->sp_win.ensure(nw * sizeof(unsigned int)));
       CLP_CUDA(h, cudaMemsetAsync(h->sp_win.p, 0, nw * sizeof(unsigned int), h->stream));
@@ -746,23 +757,15 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
     }
   }
   a.d = d; a.p0 = p0; a.p1 = p1; a.p2 = p2; a.p3 = p3; a.affinityeps = h->prm.affinityeps;
-  int rc = (h->storage == CLP_STORE_F64) ? launch_score<double>(h, kind, d, a) : launch_score<float>(h, kind, d, a);
+  int rc = with_storage(h, [&](auto t) { return launch_score<decltype(t)>(h, kind, d, a); });
   if (rc) return rc;
-  if (!compact_next) {  // dense sweeps: nothing else synchronises with the scoring launch
+  if (!compact) {  // dense sweeps: nothing else synchronises with the scoring launch
     SyncBlock host;
     if ((rc = read_sync(h, &host))) return rc;
     if (host.error == 2) return fail(h, CLP_ERR_INVALID, "association index out of range of D1/D2");
-  } else {
-    h->score_pending = true;  // the compact build reads the flag back together with its totals
   }
   const auto tp1 = std::chrono::steady_clock::now();
-  if (a.cnt) {  // counts produced by this launch describe this matrix (a failed launch / bad index aborts the build)
-    h->counts_fused = true; h->counts_win = a.win != nullptr;
-    h->counts_m = m; h->counts_rows_pad = h->rows_pad; h->counts_nseg = cnt_nseg; h->counts_W = cnt_W;
-  }
-  rc = finalize_matrix(h);
-  h->score_pending = false;
-  if (rc) { h->counts_fused = false; return rc; }
+  if ((rc = finalize_matrix(h, ScoreHandoff{compact, a.cnt != nullptr}))) return rc;
   h->has_matrix = true;
   h->has_A = true;
   if (h->prof_host) {
@@ -773,10 +776,12 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   return CLP_OK;
 }
 
-int score_from_host(clp_handle h, int kind, const double* D1, int d, long long n1, const double* D2,
-                    long long n2, const int32_t* A, long long m, double p0, double p1, double p2, double p3) {
+// the scoring entry points: D1, D2 and A on the host (clp_score_*) or on the device (clp_score_*_dev)
+int score(clp_handle h, bool on_device, int kind, const double* D1, int d, long long n1, const double* D2,
+          long long n2, const int32_t* A, long long m, double p0, double p1, double p2, double p3) {
   if (!h) return CLP_ERR_INVALID;
-  if (!D1 || !D2 || d <= 0 || n1 <= 0 || n2 <= 0) return fail(h, CLP_ERR_INVALID, "bad data set arguments");
+  if (!D1 || !D2 || d <= 0 || n1 <= 0 || n2 <= 0 || (on_device && (m < 0 || (A && m == 0))))
+    return fail(h, CLP_ERR_INVALID, on_device ? "bad device arguments" : "bad data set arguments");
   CLP_CUDA(h, cudaSetDevice(h->device));
   const bool all_to_all = (A == nullptr || m == 0);  // all-to-all hypothesis (ref clipper.cpp:24, utils.h:61-71)
   if (all_to_all) {
@@ -784,41 +789,61 @@ int score_from_host(clp_handle h, int kind, const double* D1, int d, long long n
     if (m > (long long)kMaxSeg * kSegMax) return fail(h, CLP_ERR_INVALID, "all-to-all hypothesis too large");
   } else if (m < 0) return fail(h, CLP_ERR_INVALID, "negative m");
   CLP_CUDA(h, h->A_dev.ensure((size_t)2 * m * sizeof(int32_t)));
-  CLP_CUDA(h, h->D1dev.ensure((size_t)d * n1 * sizeof(double)));
-  CLP_CUDA(h, h->D2dev.ensure((size_t)d * n2 * sizeof(double)));
+  if (!on_device) {
+    CLP_CUDA(h, h->D1dev.ensure((size_t)d * n1 * sizeof(double)));
+    CLP_CUDA(h, h->D2dev.ensure((size_t)d * n2 * sizeof(double)));
+  }
   if (all_to_all) {  // generated on the device: A never crosses PCIe; the host copy is fetched only if asked for
     all_to_all_kernel<<<(unsigned)std::min<long long>((m + 255) / 256, 4096), 256, 0, h->stream>>>(n1, n2, h->A_dev.as<int32_t>());
     CLP_CUDA(h, cudaGetLastError());
-    h->A_host_valid = false;
+  } else if (on_device) {
+    CLP_CUDA(h, cudaMemcpyAsync(h->A_dev.p, A, (size_t)2 * m * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
   } else {
     h->A_host.assign(A, A + (size_t)2 * m);
-    h->A_host_valid = true;
     CLP_CUDA(h, cudaMemcpyAsync(h->A_dev.p, h->A_host.data(), (size_t)2 * m * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
   }
-  CLP_CUDA(h, cudaMemcpyAsync(h->D1dev.p, D1, (size_t)d * n1 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  CLP_CUDA(h, cudaMemcpyAsync(h->D2dev.p, D2, (size_t)d * n2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
-  return score_on_device(h, kind, h->D1dev.as<double>(), d, n1, h->D2dev.as<double>(), n2,
-                         h->A_dev.as<int32_t>(), m, p0, p1, p2, p3);
+  h->A_host_valid = !all_to_all && !on_device;
+  if (!on_device) {
+    CLP_CUDA(h, cudaMemcpyAsync(h->D1dev.p, D1, (size_t)d * n1 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    CLP_CUDA(h, cudaMemcpyAsync(h->D2dev.p, D2, (size_t)d * n2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+    D1 = h->D1dev.as<double>(); D2 = h->D2dev.as<double>();
+  }
+  return score_on_device(h, kind, D1, d, n1, D2, n2, h->A_dev.as<int32_t>(), m, p0, p1, p2, p3);
 }
 
-int score_from_device(clp_handle h, int kind, const double* D1d, int d, long long n1, const double* D2d,
-                      long long n2, const int32_t* Ad, long long m, double p0, double p1, double p2, double p3) {
-  if (!h) return CLP_ERR_INVALID;
-  if (!D1d || !D2d || d <= 0 || n1 <= 0 || n2 <= 0 || m < 0 || (Ad && m == 0))
-    return fail(h, CLP_ERR_INVALID, "bad device arguments");
+// opens a load of a caller-given matrix (clp_set_dense, clp_set_sparse_upper): the store for m, no associations, a
+// clean sync block for the flags the load raises, every entry neutral
+int begin_load(clp_handle h, long long m) {
+  if (int rc = ensure_matrix(h, m)) return rc;
+  h->has_A = false; h->A_host_valid = false;
+  if (int rc = reset_sync(h)) return rc;
+  const size_t total = (size_t)h->rows_pad * (size_t)h->ld;
+  with_storage(h, [&](auto t) {
+    using T = decltype(t);
+    fill_neutral_kernel<T><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<T>(), total);
+  });
+  CLP_CUDA(h, cudaGetLastError());
+  return CLP_OK;
+}
+
+struct LoadCheck { int flag, code; const char* msg; };  // a flag the load may raise, and the error it makes
+
+// closes it: the first raised flag in the order of checks fails the call, else the matrix is built for its sweep
+int end_load(clp_handle h, std::initializer_list<LoadCheck> checks) {
+  SyncBlock host;
+  if (int rc = read_sync(h, &host)) return rc;
+  for (const LoadCheck& c : checks)
+    if (host.flags & c.flag) return fail(h, c.code, c.msg);
+  if (int rc = finalize_matrix(h)) return rc;
+  h->has_matrix = true;
+  return CLP_OK;
+}
+
+// after a change of the grid knobs: rebuild the loaded matrix for the new grid, or only re-plan
+int apply_grid_knobs(clp_handle h) {
+  if (h->m == 0) return CLP_OK;
   CLP_CUDA(h, cudaSetDevice(h->device));
-  if (!Ad) {  // all-to-all hypothesis, generated on the device
-    m = n1 * n2;
-    if (m > (long long)kMaxSeg * kSegMax) return fail(h, CLP_ERR_INVALID, "all-to-all hypothesis too large");
-  }
-  CLP_CUDA(h, h->A_dev.ensure((size_t)2 * m * sizeof(int32_t)));
-  if (Ad) CLP_CUDA(h, cudaMemcpyAsync(h->A_dev.p, Ad, (size_t)2 * m * sizeof(int32_t), cudaMemcpyDeviceToDevice, h->stream));
-  else {
-    all_to_all_kernel<<<(unsigned)std::min<long long>((m + 255) / 256, 4096), 256, 0, h->stream>>>(n1, n2, h->A_dev.as<int32_t>());
-    CLP_CUDA(h, cudaGetLastError());
-  }
-  h->A_host_valid = false;
-  return score_on_device(h, kind, D1d, d, n1, D2d, n2, h->A_dev.as<int32_t>(), m, p0, p1, p2, p3);
+  return h->has_matrix ? finalize_matrix(h) : plan_requested(h);
 }
 
 template <typename T>
@@ -850,8 +875,7 @@ int matvec_enqueue(clp_handle h, const double* v_dev, double d, double* y_dev, d
   st.mode = STAGE_RAW; st.srcA = v_dev; st.llA = nullptr; st.llB = nullptr; st.tag = 0;
   st.error = &h->sync.as<SyncBlock>()->error; st.alpha = 0.0; st.z = 1.0; st.dst = nullptr;
   st.segsum = h->small.as<double>();
-  return (h->storage == CLP_STORE_F64) ? launch_matvec<double>(h, st, v_dev, d, y_dev, Mv_dev, Cv_dev)
-                                       : launch_matvec<float>(h, st, v_dev, d, y_dev, Mv_dev, Cv_dev);
+  return with_storage(h, [&](auto t) { return launch_matvec<decltype(t)>(h, st, v_dev, d, y_dev, Mv_dev, Cv_dev); });
 }
 
 template <typename T>
@@ -904,9 +928,9 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
     // the per-CTA partial sums travel as LL cells tagged with the launch-local round number: start from tag 0
     CLP_CUDA(h, cudaMemsetAsync(h->res_redll.p, 0, (size_t)2 * h->res_G * kRedVals * sizeof(uint4), h->stream));
     ResArgs ra = res_args(h);
-    le = (h->storage == CLP_STORE_F64) ? launch_resident_solver<double>(h, ra) : launch_resident_solver<float>(h, ra);
+    le = with_storage(h, [&](auto t) { return launch_resident_solver<decltype(t)>(h, ra); });
   } else {
-    le = (h->storage == CLP_STORE_F64) ? launch_solver<double>(h, a) : launch_solver<float>(h, a);
+    le = with_storage(h, [&](auto t) { return launch_solver<decltype(t)>(h, a); });
   }
   CLP_CUDA(h, le);
   CLP_CUDA(h, cudaEventRecord(h->ev1, h->stream));
@@ -967,8 +991,10 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
       int32_t* S_d = reinterpret_cast<int32_t*>(sub_d + (size_t)k * k);
       CLP_CUDA(h, cudaMemcpyAsync(S_d, S.data(), (size_t)k * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
       dim3 g((unsigned)((k + 127) / 128), (unsigned)k);
-      if (h->storage == CLP_STORE_F64) gather_subblock_kernel<double><<<g, 128, 0, h->stream>>>(h->Mbuf.as<double>(), h->ld, S_d, k, sub_d);
-      else gather_subblock_kernel<float><<<g, 128, 0, h->stream>>>(h->Mbuf.as<float>(), h->ld, S_d, k, sub_d);
+      with_storage(h, [&](auto t) {
+        using T = decltype(t);
+        gather_subblock_kernel<T><<<g, 128, 0, h->stream>>>(h->Mbuf.as<T>(), h->ld, S_d, k, sub_d);
+      });
       CLP_CUDA(h, cudaGetLastError());
       std::vector<double> sub((size_t)k * k);
       CLP_CUDA(h, cudaMemcpyAsync(sub.data(), sub_d, sub.size() * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
@@ -1083,10 +1109,10 @@ int mc_prepare(clp_handle h, McLayout* L, McPeeled* out, McEvents& ev) {
   const bool rebuild = !h->mc_adj_valid;
   if (rebuild) {
     CLP_CUDA(h, h->mc_adj.ensure((size_t)m * W * sizeof(unsigned)));
-    if (h->storage == CLP_STORE_F64)
-      mc_adjacency_kernel<double><<<(unsigned)m, kMcThreads, 0, h->stream>>>(h->Mbuf.as<double>(), h->ld, (int)m, W, h->mc_adj.as<unsigned>(), L->deg0);
-    else
-      mc_adjacency_kernel<float><<<(unsigned)m, kMcThreads, 0, h->stream>>>(h->Mbuf.as<float>(), h->ld, (int)m, W, h->mc_adj.as<unsigned>(), L->deg0);
+    with_storage(h, [&](auto t) {
+      using T = decltype(t);
+      mc_adjacency_kernel<T><<<(unsigned)m, kMcThreads, 0, h->stream>>>(h->Mbuf.as<T>(), h->ld, (int)m, W, h->mc_adj.as<unsigned>(), L->deg0);
+    });
     CLP_CUDA(h, cudaGetLastError());
   }
   CLP_CUDA(h, cudaEventRecord(ev.e[1], h->stream));
@@ -1377,33 +1403,26 @@ int clp_set_stream(clp_handle h, void* cuda_stream) {
 // ---- scoring ------------------------------------------------------------------------------
 int clp_score_euclidean(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2,
                         const int32_t* A, int64_t m, double sigma, double epsilon, double mindist) {
-  return guarded(h, [&] { return score_from_host(h, 0, D1, d, n1, D2, n2, A, m, sigma, epsilon, mindist, 0.0); });
+  return guarded(h, [&] { return score(h, false, 0, D1, d, n1, D2, n2, A, m, sigma, epsilon, mindist, 0.0); });
 }
 int clp_score_pointnormal(clp_handle h, const double* D1, int64_t n1, const double* D2, int64_t n2,
                           const int32_t* A, int64_t m, double sigp, double epsp, double sign, double epsn) {
-  return guarded(h, [&] { return score_from_host(h, 1, D1, 6, n1, D2, n2, A, m, sigp, epsp, sign, epsn); });
+  return guarded(h, [&] { return score(h, false, 1, D1, 6, n1, D2, n2, A, m, sigp, epsp, sign, epsn); });
 }
 int clp_score_euclidean_dev(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2,
                             const int32_t* A, int64_t m, double sigma, double epsilon, double mindist) {
-  return guarded(h, [&] { return score_from_device(h, 0, D1, d, n1, D2, n2, A, m, sigma, epsilon, mindist, 0.0); });
+  return guarded(h, [&] { return score(h, true, 0, D1, d, n1, D2, n2, A, m, sigma, epsilon, mindist, 0.0); });
 }
 int clp_score_pointnormal_dev(clp_handle h, const double* D1, int64_t n1, const double* D2, int64_t n2,
                               const int32_t* A, int64_t m, double sigp, double epsp, double sign, double epsn) {
-  return guarded(h, [&] { return score_from_device(h, 1, D1, 6, n1, D2, n2, A, m, sigp, epsp, sign, epsn); });
+  return guarded(h, [&] { return score(h, true, 1, D1, 6, n1, D2, n2, A, m, sigp, epsp, sign, epsn); });
 }
 
 // ---- get / set ----------------------------------------------------------------------------
 int clp_set_dense(clp_handle h, const double* M, const double* C, int64_t m) {
   if (!h || !M || !C) return CLP_ERR_INVALID;
-  h->counts_fused = false;
-  if (int rc = ensure_matrix(h, m)) return rc;
-  h->has_A = false; h->A_host_valid = false;
-  if (int rc = reset_sync(h)) return rc;
+  if (int rc = begin_load(h, m)) return rc;
   SyncBlock* sb = h->sync.as<SyncBlock>();
-  const size_t total = (size_t)h->rows_pad * (size_t)h->ld;
-  if (h->storage == CLP_STORE_F64) fill_neutral_kernel<double><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<double>(), total);
-  else fill_neutral_kernel<float><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<float>(), total);
-  CLP_CUDA(h, cudaGetLastError());
   // column panels of at most 32 MB per matrix
   const long long pc = std::max<long long>(1, std::min<long long>(m, (32ll << 20) / (8 * m)));
   CLP_CUDA(h, h->panel.ensure((size_t)2 * pc * m * sizeof(double)));
@@ -1414,34 +1433,22 @@ int clp_set_dense(clp_handle h, const double* M, const double* C, int64_t m) {
     CLP_CUDA(h, cudaMemcpyAsync(Mp, M + (size_t)j0 * m, (size_t)(j1 - j0) * m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CLP_CUDA(h, cudaMemcpyAsync(Cp, C + (size_t)j0 * m, (size_t)(j1 - j0) * m * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     dim3 grid((unsigned)((m + 255) / 256), (unsigned)(j1 - j0));
-    if (h->storage == CLP_STORE_F64)
-      encode_dense_panel_kernel<double><<<grid, 256, 0, h->stream>>>(Mp, Cp, (int)m, (int)j0, (int)j1, h->Mbuf.as<double>(), h->ld, h->row0, h->rows, &sb->flags);
-    else
-      encode_dense_panel_kernel<float><<<grid, 256, 0, h->stream>>>(Mp, Cp, (int)m, (int)j0, (int)j1, h->Mbuf.as<float>(), h->ld, h->row0, h->rows, &sb->flags);
+    with_storage(h, [&](auto t) {
+      using T = decltype(t);
+      encode_dense_panel_kernel<T><<<grid, 256, 0, h->stream>>>(Mp, Cp, (int)m, (int)j0, (int)j1, h->Mbuf.as<T>(), h->ld, h->row0, h->rows, &sb->flags);
+    });
     CLP_CUDA(h, cudaGetLastError());
     CLP_CUDA(h, cudaStreamSynchronize(h->stream));  // the panel buffer is reused
   }
-  SyncBlock host;
-  if (int rc = read_sync(h, &host)) return rc;
-  if (host.flags & 1) return fail(h, CLP_ERR_UNSUPPORTED, "affinity matrix has negative entries (contract: M in [0,1], ref clipper.h:166-171)");
-  if (host.flags & 2) return fail(h, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary (contract: ref clipper.h:176)");
-  if (int rc = finalize_matrix(h)) return rc;
-  h->has_matrix = true;
-  return CLP_OK;
+  return end_load(h, {{1, CLP_ERR_UNSUPPORTED, "affinity matrix has negative entries (contract: M in [0,1], ref clipper.h:166-171)"},
+                      {2, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary (contract: ref clipper.h:176)"}});
 }
 
 int clp_set_sparse_upper(clp_handle h, int64_t m, const int64_t* cpM, const int32_t* riM, const double* vM,
                          const int64_t* cpC, const int32_t* riC, const double* vC) {
   if (!h || !cpM || !cpC) return CLP_ERR_INVALID;
-  h->counts_fused = false;
-  if (int rc = ensure_matrix(h, m)) return rc;
-  h->has_A = false; h->A_host_valid = false;
-  if (int rc = reset_sync(h)) return rc;
+  if (int rc = begin_load(h, m)) return rc;
   SyncBlock* sb = h->sync.as<SyncBlock>();
-  const size_t total = (size_t)h->rows_pad * (size_t)h->ld;
-  if (h->storage == CLP_STORE_F64) fill_neutral_kernel<double><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<double>(), total);
-  else fill_neutral_kernel<float><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<float>(), total);
-  CLP_CUDA(h, cudaGetLastError());
   for (int which = 0; which < 2; ++which) {
     const int64_t* cp = which ? cpC : cpM; const int32_t* ri = which ? riC : riM; const double* vv = which ? vC : vM;
     const long long nnz = cp[m];
@@ -1458,24 +1465,17 @@ int clp_set_sparse_upper(clp_handle h, int64_t m, const int64_t* cpM, const int3
       CLP_CUDA(h, cudaMemcpyAsync(v_d, vv, (size_t)nnz * sizeof(double), cudaMemcpyHostToDevice, h->stream));
       CLP_CUDA(h, cudaMemcpyAsync(ri_d, ri, (size_t)nnz * sizeof(int32_t), cudaMemcpyHostToDevice, h->stream));
     }
-    if (h->storage == CLP_STORE_F64) {
-      if (which == 0) scatter_csc_M_kernel<double><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<double>(), h->ld, h->row0, h->rows, &sb->flags);
-      else scatter_csc_C_kernel<double><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<double>(), h->ld, h->row0, h->rows, &sb->flags);
-    } else {
-      if (which == 0) scatter_csc_M_kernel<float><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<float>(), h->ld, h->row0, h->rows, &sb->flags);
-      else scatter_csc_C_kernel<float><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<float>(), h->ld, h->row0, h->rows, &sb->flags);
-    }
+    with_storage(h, [&](auto t) {
+      using T = decltype(t);
+      if (which == 0) scatter_csc_M_kernel<T><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<T>(), h->ld, h->row0, h->rows, &sb->flags);
+      else scatter_csc_C_kernel<T><<<(unsigned)m, 128, 0, h->stream>>>(cp_d, ri_d, v_d, (int)m, h->Mbuf.as<T>(), h->ld, h->row0, h->rows, &sb->flags);
+    });
     CLP_CUDA(h, cudaGetLastError());
     CLP_CUDA(h, cudaStreamSynchronize(h->stream));
   }
-  SyncBlock host;
-  if (int rc = read_sync(h, &host)) return rc;
-  if (host.flags & 4) return fail(h, CLP_ERR_INVALID, "sparse input is not strictly upper triangular (ref clipper.h:137-138)");
-  if (host.flags & 1) return fail(h, CLP_ERR_UNSUPPORTED, "affinity matrix has negative entries");
-  if (host.flags & 2) return fail(h, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary");
-  if (int rc = finalize_matrix(h)) return rc;
-  h->has_matrix = true;
-  return CLP_OK;
+  return end_load(h, {{4, CLP_ERR_INVALID, "sparse input is not strictly upper triangular (ref clipper.h:137-138)"},
+                      {1, CLP_ERR_UNSUPPORTED, "affinity matrix has negative entries"},
+                      {2, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary"}});
 }
 
 int clp_get_dense(clp_handle h, int which, double* out) {
@@ -1490,8 +1490,10 @@ int clp_get_dense(clp_handle h, int which, double* out) {
   for (long long j0 = 0; j0 < m; j0 += pc) {
     const long long j1 = std::min<long long>(m, j0 + pc);
     dim3 grid((unsigned)((m + 255) / 256), (unsigned)(j1 - j0));
-    if (h->storage == CLP_STORE_F64) decode_dense_panel_kernel<double><<<grid, 256, 0, h->stream>>>(h->Mbuf.as<double>(), h->ld, (int)m, (int)j0, (int)j1, which, P);
-    else decode_dense_panel_kernel<float><<<grid, 256, 0, h->stream>>>(h->Mbuf.as<float>(), h->ld, (int)m, (int)j0, (int)j1, which, P);
+    with_storage(h, [&](auto t) {
+      using T = decltype(t);
+      decode_dense_panel_kernel<T><<<grid, 256, 0, h->stream>>>(h->Mbuf.as<T>(), h->ld, (int)m, (int)j0, (int)j1, which, P);
+    });
     CLP_CUDA(h, cudaGetLastError());
     CLP_CUDA(h, cudaMemcpyAsync(out + (size_t)j0 * m, P, (size_t)(j1 - j0) * m * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CLP_CUDA(h, cudaStreamSynchronize(h->stream));
@@ -1525,8 +1527,10 @@ int clp_count_nonzeros(clp_handle h, int64_t* nnzM, int64_t* nnzC) {
   CLP_CUDA(h, cudaSetDevice(h->device));
   if (int rc = reset_sync(h)) return rc;
   SyncBlock* sb = h->sync.as<SyncBlock>();
-  if (h->storage == CLP_STORE_F64) count_upper_kernel<double><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<double>(), h->ld, (int)h->m, h->row0, h->rows, sb->counts);
-  else count_upper_kernel<float><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<float>(), h->ld, (int)h->m, h->row0, h->rows, sb->counts);
+  with_storage(h, [&](auto t) {
+    using T = decltype(t);
+    count_upper_kernel<T><<<h->sm_count * 8, 256, 0, h->stream>>>(h->Mbuf.as<T>(), h->ld, (int)h->m, h->row0, h->rows, sb->counts);
+  });
   CLP_CUDA(h, cudaGetLastError());
   SyncBlock host;
   if (int rc = read_sync(h, &host)) return rc;
@@ -1728,23 +1732,13 @@ int clp_shard_import(clp_handle h, const void* blobs, int64_t blob_bytes_each, i
 int clp_set_grid_cap(clp_handle h, int n_ctas) {
   if (!h || n_ctas < 0) return fail(h, CLP_ERR_INVALID, "grid cap must be >= 0 (0 = whole GPU)");
   h->grid_cap = n_ctas;
-  if (h->m > 0) {
-    CLP_CUDA(h, cudaSetDevice(h->device));
-    if (h->has_matrix) { if (int rc = finalize_matrix(h)) return rc; }
-    else { if (int rc = set_plan_for(h, h->dense_mode == 3 || h->dense_mode == 4 ? 3 : h->dense_mode)) return rc; }
-  }
-  return CLP_OK;
+  return apply_grid_knobs(h);
 }
 
 int clp_set_ctas_per_sm(clp_handle h, int n) {
   if (!h || n < 1 || n > 3) return fail(h, CLP_ERR_INVALID, "ctas_per_sm must be 1, 2 or 3");
   h->ctas_cap = n;
-  if (h->m > 0) {
-    CLP_CUDA(h, cudaSetDevice(h->device));
-    if (h->has_matrix) { if (int rc = finalize_matrix(h)) return rc; }
-    else { if (int rc = set_plan_for(h, h->dense_mode == 3 || h->dense_mode == 4 ? 3 : h->dense_mode)) return rc; }
-  }
-  return CLP_OK;
+  return apply_grid_knobs(h);
 }
 
 int clp_sparse_info(clp_handle h, int64_t* nnz_kept, int64_t* bytes_per_pass) {
@@ -1752,7 +1746,7 @@ int clp_sparse_info(clp_handle h, int64_t* nnz_kept, int64_t* bytes_per_pass) {
   if (nnz_kept) *nnz_kept = (int64_t)h->sp_nnz_real;
   if (bytes_per_pass)
     *bytes_per_pass = (int64_t)(h->sp_nnz * h->entry_bytes() +
-                                (unsigned long long)(h->rows_pad / 4) * (h->compact_resident ? 1 : h->plan.NSEG) * 20);
+                                (unsigned long long)(h->rows_pad / 4) * (h->sp_shape.resident ? 1 : h->plan.NSEG) * 20);
   return CLP_OK;
 }
 

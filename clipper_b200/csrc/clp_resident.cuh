@@ -35,7 +35,7 @@
 
 namespace clp {
 
-constexpr int kResThreads = 768;                  // widest resident instance (24 warps): sizes the fit test of resident_possible
+constexpr int kResThreads = 768;                  // widest resident instance (24 warps): sizes the fit test of compact_shape
 constexpr int kResWarps = kResThreads / 32;
 constexpr int kResMaxM = 27648;                   // largest m whose fp64 trial vector (+ scratch) fits 227 KB
 constexpr int kPieceVals = 8;                     // a piece: 4 members x (|M| v, C v)
