@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "lib", "libclipper_b200.so")
 
 OK = 0
 STORE_F32, STORE_F64 = 0, 1
+IN_F32, IN_F64 = 0, 1
 ROUND_NONZERO, ROUND_DSD, ROUND_DSD_HEU = 0, 1, 2
 
 # every symbol include/clipper_b200.h declares (checked by tests/test_capi_symbols.py)
@@ -29,7 +30,7 @@ SYMBOLS = [
     "clp_batch_solve_euclidean", "clp_batch_solve_pointnormal", "clp_batch_info",
     "clp_max_clique", "clp_core_numbers",
     "clp_batch_max_clique_euclidean", "clp_batch_max_clique_pointnormal", "clp_batch_max_clique_graphs",
-    "clp_batch_solve_matrices",
+    "clp_batch_solve_matrices", "clp_set_dense_dev", "clp_batch_set_stream", "clp_batch_solve_dense_dev",
 ]
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 
@@ -103,6 +104,7 @@ def load():
     L.clp_score_euclidean_dev.argtypes = [vp, vp, i32, i64, vp, i64, vp, i64, dbl, dbl, dbl]
     L.clp_score_pointnormal_dev.argtypes = [vp, vp, i64, vp, i64, vp, i64, dbl, dbl, dbl, dbl]
     L.clp_set_dense.argtypes = [vp, dp, dp, i64]
+    L.clp_set_dense_dev.argtypes = [vp, vp, vp, i64, C.c_int, i64, i64]
     L.clp_set_sparse_upper.argtypes = [vp, i64, lp, ip, dp, lp, ip, dp]
     L.clp_get_dense.argtypes = [vp, C.c_int, dp]
     L.clp_num_associations.argtypes = [vp, lp]
@@ -139,6 +141,9 @@ def load():
     L.clp_batch_solve_pointnormal.argtypes = [vp, i32, pp, lp, pp, lp, pp, lp, pp, dbl, dbl, dbl, dbl,
                                               C.POINTER(ClpSolution), pp, pp]
     L.clp_batch_solve_matrices.argtypes = [vp, i32, lp, pp, pp, pp, pp, pp, pp, pp, C.POINTER(ClpSolution), pp, pp]
+    L.clp_batch_set_stream.argtypes = [vp, vp]
+    L.clp_batch_solve_dense_dev.argtypes = [vp, i32, lp, C.c_int, vp, vp, i64, i64, i64, vp, i64, C.POINTER(ClpSolution),
+                                            vp, i64, pp]
     L.clp_batch_info.argtypes = [vp, ip, lp, lp]
     L.clp_max_clique.argtypes = [vp, C.c_int, dbl, ip, C.POINTER(ClpMcInfo)]
     L.clp_core_numbers.argtypes = [vp, ip]

@@ -127,6 +127,34 @@ invariants = types.SimpleNamespace(
 # --------------------------------------------------------------------------------------------
 # utils / dsd
 # --------------------------------------------------------------------------------------------
+def _dev_matrix_dtype(device, mats, ndim):
+    """the C-ABI dtype (IN_F32 / IN_F64) of CUDA tensors of equal shape and strides with ndim dimensions on device;
+    TypeError / ValueError otherwise.  torch is imported here only: the rest of the package does not need it."""
+    import torch
+    for X in mats:
+        if not isinstance(X, torch.Tensor):
+            raise TypeError("expected a torch tensor, got %s" % type(X).__name__)
+        if not X.is_cuda:
+            raise ValueError("expected a CUDA tensor, got one on %s" % X.device)
+        if X.device.index != device:
+            raise ValueError("the tensor is on %s, the handle on cuda:%d" % (X.device, device))
+    if any(X.dtype != mats[0].dtype for X in mats) or mats[0].dtype not in (torch.float32, torch.float64):
+        raise TypeError("M and C must both be float32 or both float64, got %s" % ", ".join(str(X.dtype) for X in mats))
+    if any(X.dim() != ndim for X in mats) or any(X.shape != mats[0].shape or X.stride() != mats[0].stride() for X in mats):
+        raise ValueError("M and C must be %d-dimensional with equal shapes and strides" % ndim)
+    rs, cs = mats[0].stride()[-2:]
+    if not ((rs == 1 and cs >= 1) or (cs == 1 and rs >= 1)):
+        raise ValueError("M and C need a unit stride along rows or columns, got strides %s" % (mats[0].stride(),))
+    return _capi.IN_F32 if mats[0].dtype == torch.float32 else _capi.IN_F64
+
+
+def _wait_for_torch(stream, device):
+    """a handle on its own stream reads tensors torch may still be writing: synchronise torch's current stream"""
+    if not stream:
+        import torch
+        torch.cuda.current_stream(device).synchronize()
+
+
 def create_all_to_all(n1, n2):
     """reference utils.h:61-71 -> (n1*n2, 2) int32, column-major"""
     A = np.zeros((int(n1) * int(n2), 2), dtype=np.int32, order="F")
@@ -280,6 +308,8 @@ class CLIPPER:
         if rc != _capi.OK:
             msg = self._lib.clp_last_error(None)
             raise ClipperError(rc, msg.decode() if msg else "clp_create failed")
+        self._device = int(device)
+        self._stream = None   # a caller's stream set with set_stream, else the handle's own
         self._invariant = invariant
         self._params = params
         self._parallelize = True
@@ -305,6 +335,7 @@ class CLIPPER:
 
     def set_stream(self, cuda_stream):
         _capi.check(self._h, self._lib.clp_set_stream(self._h, C.c_void_p(cuda_stream)))
+        self._stream = cuda_stream or None
 
     def set_dense_mode(self, mode):
         """4 (default) auto; 6 compact rows + resident trial vector (m <= 27648); 3 compact rows, column segments;
@@ -504,6 +535,20 @@ class CLIPPER:
             raise ValueError("M and C must be square and of equal shape")
         self._A_custom = None
         _capi.check(self._h, self._lib.clp_set_dense(self._h, _dp(M), _dp(C_), M.shape[0]))
+
+    def set_matrix_data_dev(self, M, C_):
+        """set_matrix_data from CUDA tensors already on the handle's device (clp_set_dense_dev): M and C are (m, m), both
+        float32 or both float64, each with one unit stride (``.t()`` views and slices of larger tensors need no copy).
+        Only the strict upper triangle is read; a float32 x is stored as the float64 (double)x would be.  Runs on the
+        handle's stream (set_stream) and returns when the matrix is built.  Without a stream of the caller's, torch's
+        current stream is synchronised first: the handle's own stream does not wait for the work that made M and C."""
+        dtype = _dev_matrix_dtype(self._device, (M, C_), 2)
+        if M.shape[0] != M.shape[1]:
+            raise ValueError("M and C must be square, got %s" % (tuple(M.shape),))
+        _wait_for_torch(self._stream, M.device)
+        self._A_custom = None
+        _capi.check(self._h, self._lib.clp_set_dense_dev(self._h, M.data_ptr(), C_.data_ptr(), M.shape[0], dtype,
+                                                         M.stride(0), M.stride(1)))
 
     def set_sparse_matrix_data(self, M, C_):
         """reference clipper.cpp:162-166; M, C: scipy.sparse matrices, strictly upper triangular"""

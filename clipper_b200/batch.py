@@ -14,7 +14,8 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from .api import EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64
+from .api import (EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64, _dev_matrix_dtype,
+                  _wait_for_torch)
 
 
 class BatchCLIPPER:
@@ -212,6 +213,8 @@ class MatrixBatchCLIPPER:
     def __init__(self, params=None, device=0):
         self._lib = _capi.load()
         self._b = _new_batch(self._lib, device)
+        self._device = int(device)
+        self._stream = None   # a caller's stream set with set_stream, else the batch's own
         self._params = params if params is not None else Params()
 
     __del__ = BatchCLIPPER.__del__
@@ -248,6 +251,43 @@ class MatrixBatchCLIPPER:
         sols = (_capi.ClpSolution * n)()
         self._check(self._lib.clp_batch_solve_matrices(self._b, n, m, *ptrs, u0p, sols, up, np_))
         return _solutions(sols, n, u0s, us, nodes)
+
+    def set_stream(self, cuda_stream):
+        """run on an existing CUDA stream (an int handle, e.g. torch.cuda.current_stream().cuda_stream); None or 0: the
+        batch's own stream"""
+        self._check(self._lib.clp_batch_set_stream(self._b, C.c_void_p(cuda_stream or None)))
+        self._stream = cuda_stream or None
+
+    def solve_dense_dev(self, M, C_, u0, m=None):
+        """Problems given as CUDA tensors on the batch's device (clp_batch_solve_dense_dev): M and C (B, m_max, m_max),
+        both float32 or both float64, with a unit stride along rows or columns; problem p is the leading m[p] x m[p]
+        block, of which only the strict upper triangle is read.  u0: (B, m_max) float64.  m: B sizes (default m_max
+        each, at most 4096).  Returns one api.Solution per problem as solve_many fills it, except that .u and .u0 are
+        device tensor views of length m[p].  Runs on the batch's stream (set_stream); without a stream of the caller's,
+        torch's current stream is synchronised first."""
+        import torch
+        dtype = _dev_matrix_dtype(self._device, (M, C_), 3)
+        nb, mm = M.shape[0], M.shape[1]
+        if M.shape[2] != mm or nb == 0:
+            raise ValueError("M and C must be (B, m_max, m_max) with B >= 1, got %s" % (tuple(M.shape),))
+        if not isinstance(u0, torch.Tensor) or u0.dtype != torch.float64:
+            raise TypeError("u0 must be a float64 torch tensor")
+        if tuple(u0.shape) != (nb, mm) or not u0.is_cuda or u0.device.index != self._device or u0.stride(1) != 1:
+            raise ValueError("u0 must be a (B, m_max) float64 CUDA tensor on the batch's device with unit column stride")
+        ms = [mm] * nb if m is None else [int(x) for x in m]
+        if len(ms) != nb or any(x < 1 or x > mm for x in ms):
+            raise ValueError("m must hold B sizes in [1, m_max]")
+        self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
+        _wait_for_torch(self._stream, M.device)
+        marr = (C.c_int64 * nb)(*ms)
+        u = torch.empty((nb, mm), dtype=torch.float64, device=M.device)
+        nodes = [np.zeros(max(mk, 1), np.int32) for mk in ms]
+        np_ = (C.c_void_p * nb)(*[nk.ctypes.data for nk in nodes])
+        sols = (_capi.ClpSolution * nb)()
+        self._check(self._lib.clp_batch_solve_dense_dev(self._b, nb, marr, dtype, M.data_ptr(), C_.data_ptr(), M.stride(0),
+                                                         M.stride(1), M.stride(2), u0.data_ptr(), u0.stride(0), sols,
+                                                         u.data_ptr(), u.stride(0), np_))
+        return _solutions(sols, nb, [u0[k, :ms[k]] for k in range(nb)], [u[k, :ms[k]] for k in range(nb)], nodes)
 
 
 def _mc_outputs(ms, params):

@@ -188,6 +188,8 @@ int fail(H* h, int code, const std::string& msg) {
   } while (0)
 
 inline long long round_up(long long x, long long q) { return (x + q - 1) / q * q; }
+// element strides of a dense device matrix (clp_set_dense_dev, clp_batch_solve_dense_dev): one is 1, the other >= 1
+inline bool dense_strides_ok(long long rs, long long cs) { return (rs == 1 && cs >= 1) || (cs == 1 && rs >= 1); }
 int reset_sync(clp_handle h);
 
 // f(T{}) with T the handle's storage type (float or double)
@@ -1444,6 +1446,30 @@ int clp_set_dense(clp_handle h, const double* M, const double* C, int64_t m) {
                       {2, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary (contract: ref clipper.h:176)"}});
 }
 
+int clp_set_dense_dev(clp_handle h, const void* M, const void* C, int64_t m, int dtype, int64_t row_stride, int64_t col_stride) {
+  if (!h || !M || !C) return CLP_ERR_INVALID;
+  if (dtype != CLP_IN_F32 && dtype != CLP_IN_F64) return fail(h, CLP_ERR_INVALID, "unknown input dtype (CLP_IN_F32 or CLP_IN_F64)");
+  if (!dense_strides_ok(row_stride, col_stride)) return fail(h, CLP_ERR_INVALID, "one of row_stride, col_stride must be 1 and the other >= 1");
+  if (h->world > 1) return fail(h, CLP_ERR_UNSUPPORTED, "clp_set_dense_dev on a sharded handle (a rank would need the whole matrix)");
+  return guarded(h, [&] {
+    if (int rc = begin_load(h, m)) return rc;
+    SyncBlock* sb = h->sync.as<SyncBlock>();
+    const unsigned nt = (unsigned)((m + 31) / 32);
+    with_storage(h, [&](auto t) {
+      using T = decltype(t);
+      if (dtype == CLP_IN_F32)
+        load_dense_dev_kernel<T, float><<<dim3(nt, nt), 256, 0, h->stream>>>(static_cast<const float*>(M), static_cast<const float*>(C), (int)m,
+                                                                          row_stride, col_stride, h->Mbuf.as<T>(), h->ld, &sb->flags);
+      else
+        load_dense_dev_kernel<T, double><<<dim3(nt, nt), 256, 0, h->stream>>>(static_cast<const double*>(M), static_cast<const double*>(C), (int)m,
+                                                                           row_stride, col_stride, h->Mbuf.as<T>(), h->ld, &sb->flags);
+    });
+    CLP_CUDA(h, cudaGetLastError());
+    return end_load(h, {{1, CLP_ERR_UNSUPPORTED, "affinity matrix has negative entries (contract: M in [0,1], ref clipper.h:166-171)"},
+                        {2, CLP_ERR_UNSUPPORTED, "constraint matrix is not binary (contract: ref clipper.h:176)"}});
+  });
+}
+
 int clp_set_sparse_upper(clp_handle h, int64_t m, const int64_t* cpM, const int32_t* riM, const double* vM,
                          const int64_t* cpC, const int32_t* riC, const double* vC) {
   if (!h || !cpM || !cpC) return CLP_ERR_INVALID;
@@ -1775,6 +1801,7 @@ int clp_set_dense_mode(clp_handle h, int mode) {
 struct clp_batch_s {
   int device = 0;
   cudaStream_t stream = nullptr;
+  bool own_stream = true;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_up = nullptr;
   clp_params prm;
   std::string err;
@@ -1911,6 +1938,7 @@ int batch_grid(clp_batch b, int occ, int32_t nprob, size_t stride, DevBuf& scrat
 // problem and the sync block into the staging buffer with one synchronisation, prints the CLP_PROF_BATCH line, maps the
 // device's error words (batch_matrix_solve_kernel sets flags, batch_solve_kernel error 2, both time out with error 1),
 // and fills the results.  `label` names the call and `first` its first in-kernel phase in the profile line.
+// batch_dense_solve_kernel leaves its first bad problem in counts[1] (BatchDenseArgs::bad); it is reported first.
 template <typename Prob>
 int batch_finish(clp_batch b, const char* label, const char* first, const std::vector<Prob>& probs, long long nu, int max_m,
                  int grid, size_t stride, size_t bytes_in, std::chrono::steady_clock::time_point t_begin, clp_solution* sols,
@@ -1937,6 +1965,12 @@ int batch_finish(clp_batch b, const char* label, const char* first, const std::v
     std::fprintf(stderr, "[clp %s prof] %d problems (max m %d), %d CTAs, upload %zu bytes %.3f ms, kernel %.3f ms; "
                  "mean per problem: %s %.3f  build %.3f  solve %.3f  total %.3f ms\n",
                  label, nprob, max_m, grid, bytes_in, up_ms, ms, first, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
+  }
+  if (h_sb.counts[1] != 0) {
+    const bool neg = (h_sb.counts[1] >> 32) == 2;
+    const unsigned int p = 0xffffffffu - (unsigned int)(h_sb.counts[1] & 0xffffffffu);
+    return fail(b, CLP_ERR_UNSUPPORTED, "problem " + std::to_string(p) +
+                                            (neg ? ", M: affinity matrix has negative entries" : ", C: constraint matrix is not binary"));
   }
   if (h_sb.flags != 0) return fail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
   if (h_sb.error == 2) return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
@@ -2178,6 +2212,86 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   if (int rc = batch_launch_matrices(b, ba, grid, bs.total)) return rc;
   return batch_finish(b, "batch matrices", "scatter", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+}
+
+// ---- batched solve of dense device tensors (batch_dense_solve_kernel) ---------------------------------------------
+// The values are checked on the device (batch_finish maps what the kernel found); only the sizes, pointers, strides and
+// dtype are checked here.  Only the problem table is uploaded.
+template <typename In>
+int batch_launch_dense(clp_batch b, BatchDenseArgs& ba, size_t smem, int nprob, size_t stride, int* grid) {
+  int occ = 0;
+  CLP_CUDA(b, cudaFuncSetAttribute(batch_dense_solve_kernel<In>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, batch_dense_solve_kernel<In>, kBatchThreads, smem));
+  if (occ < 1) return fail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
+  if (int rc = batch_grid(b, occ, nprob, stride, b->scratch, nullptr, grid)) return rc;
+  ba.scratch = b->scratch.as<unsigned char>();
+  CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
+  batch_dense_solve_kernel<In><<<*grid, kBatchThreads, smem, b->stream>>>(ba);
+  CLP_CUDA(b, cudaGetLastError());
+  return CLP_OK;
+}
+
+int batch_solve_dense_dev(clp_batch b, int32_t nprob, const int64_t* m, int dtype, const void* M, const void* Cm, int64_t bstride,
+                          int64_t rs, int64_t cs, const double* u0, int64_t u0_stride, clp_solution* sols, double* u_out_dev,
+                          int64_t u_out_stride, int32_t* const* nodes_out) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !m || !M || !Cm || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (!u0) return fail(b, CLP_ERR_INVALID, "null u0");
+  int max_m = 1;
+  for (int p = 0; p < nprob; ++p) {
+    if (m[p] < 1 || m[p] > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "problem " + std::to_string(p) + ": batched problems need 1 <= m <= 4096");
+    max_m = std::max(max_m, (int)m[p]);
+  }
+  if (!dense_strides_ok(rs, cs) || bstride < 1 || u0_stride < 1 || (u_out_dev && u_out_stride < max_m))
+    return fail(b, CLP_ERR_INVALID, "bad strides (one of row_stride, col_stride must be 1 and the other >= 1; batch_stride, "
+                                    "u0_stride >= 1; u_out_stride >= the largest m)");
+  if (dtype != CLP_IN_F32 && dtype != CLP_IN_F64) return fail(b, CLP_ERR_INVALID, "unknown input dtype (CLP_IN_F32 or CLP_IN_F64)");
+  const clp_params& P = b->prm;
+  if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
+  if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
+  const auto t_begin = std::chrono::steady_clock::now();
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  // every problem's u0 / u slot starts on a 128-byte line of its own: the CTAs stage u0 and read u back themselves
+  const long long ustride = round_up(max_m, 16);
+  const long long nu = (long long)nprob * ustride;
+  std::vector<BatchMatProblem> probs((size_t)nprob);
+  for (int p = 0; p < nprob; ++p) { probs[(size_t)p].m = (int)m[p]; probs[(size_t)p].u_off = p * ustride; }
+  const size_t bytes_in = (size_t)nprob * sizeof(BatchMatProblem);
+  const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
+  CLP_CUDA(b, b->pinned.ensure(std::max(bytes_in, bytes_out) + 4096));
+  std::memcpy(b->pinned.p, probs.data(), bytes_in);
+  CLP_CUDA(b, b->probs.ensure(bytes_in));
+  CLP_CUDA(b, b->in_u0.ensure((size_t)nu * 8 + 16));
+  CLP_CUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
+  CLP_CUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
+  CLP_CUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
+  CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->probs.p, b->pinned.p, bytes_in, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  const BatchSmem bs = batch_smem_plan(max_m);
+  if ((long long)bs.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
+  const BatchLayout L = batch_layout(max_m, 0, /*points*/ false);
+  SyncBlock* sb = b->sync.as<SyncBlock>();
+  BatchDenseArgs ba;
+  std::memset(&ba, 0, sizeof(ba));
+  ba.prob = b->probs.as<BatchMatProblem>(); ba.nprob = nprob;
+  ba.M = M; ba.C = Cm; ba.bstride = bstride; ba.rs = rs; ba.cs = cs;
+  ba.u0_in = u0; ba.u0_stride = u0_stride; ba.u0 = b->in_u0.as<double>();
+  ba.u_out = b->out_u.as<double>(); ba.u_out_dev = u_out_dev; ba.u_out_stride = u_out_stride;
+  ba.out = b->outs.as<SolverOut>(); ba.nnz_out = b->nnz.as<unsigned int>();
+  ba.next = reinterpret_cast<int*>(&sb->counts[0]); ba.bad = &sb->counts[1];
+  ba.scratch_stride = L.total;
+  ba.max_m = max_m;
+  ba.prm = solver_params(P);
+  ba.sb = sb; ba.spin_limit = 4LL * 1900000000LL;
+  if (b->prof_on) { CLP_CUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  int grid = 0;
+  const int rc = dtype == CLP_IN_F32 ? batch_launch_dense<float>(b, ba, bs.total, nprob, L.total, &grid)
+                                     : batch_launch_dense<double>(b, ba, bs.total, nprob, L.total, &grid);
+  if (rc) return rc;
+  return batch_finish(b, "batch dense", "load", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, nullptr, nodes_out);
 }
 
 // ---- batched maximum clique (clp_batch_clique.cuh) ----------------------------------------------------------------
@@ -2490,7 +2604,7 @@ int clp_batch_destroy(clp_batch b) {
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
   if (b->ev_up) cudaEventDestroy(b->ev_up);
-  if (b->stream) cudaStreamDestroy(b->stream);
+  if (b->stream && b->own_stream) cudaStreamDestroy(b->stream);
   delete b;
   return CLP_OK;
 }
@@ -2530,6 +2644,25 @@ int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
                              const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
   return guarded(b, [&] {
     return batch_solve_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, u0, sols, u_out, nodes_out);
+  });
+}
+
+int clp_batch_set_stream(clp_batch b, void* cuda_stream) {
+  if (!b) return CLP_ERR_INVALID;
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  if (b->stream && b->own_stream) { cudaStreamSynchronize(b->stream); cudaStreamDestroy(b->stream); }
+  if (cuda_stream) { b->stream = reinterpret_cast<cudaStream_t>(cuda_stream); b->own_stream = false; }
+  else { CLP_CUDA(b, cudaStreamCreateWithFlags(&b->stream, cudaStreamNonBlocking)); b->own_stream = true; }
+  return CLP_OK;
+}
+
+int clp_batch_solve_dense_dev(clp_batch b, int32_t nprob, const int64_t* m, int dtype, const void* M_dev, const void* C_dev,
+                              int64_t batch_stride, int64_t row_stride, int64_t col_stride, const double* u0_dev,
+                              int64_t u0_stride, clp_solution* sols, double* u_out_dev, int64_t u_out_stride,
+                              int32_t* const* nodes_out) {
+  return guarded(b, [&] {
+    return batch_solve_dense_dev(b, nprob, m, dtype, M_dev, C_dev, batch_stride, row_stride, col_stride, u0_dev, u0_stride,
+                                 sols, u_out_dev, u_out_stride, nodes_out);
   });
 }
 

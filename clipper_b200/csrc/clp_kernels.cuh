@@ -1344,6 +1344,18 @@ __global__ void fill_neutral_kernel(T* M, size_t n) {
   for (; i < n; i += stride) M[i] = encode<T>(0.0, false);
 }
 
+// The storage rule of a dense entry (i, j), i < j, of caller-given M and C (fp64 or fp32 input; an fp32 x is stored as
+// the fp64 (double)x would be): the element stored at (i, j) and (j, i).  bad |= 1 for a negative affinity, 2 for a
+// constraint value outside {0, 1} (NaN included).  Every dense load stores through it: the host panels
+// (encode_dense_panel_kernel), device tensors (load_dense_dev_kernel) and the batch (batch_dense_solve_kernel).
+template <typename T, typename In>
+__device__ __forceinline__ T dense_entry(In mv, In cv, unsigned int& bad) {
+  const double mval = (double)mv, cval = (double)cv;
+  if (mval < 0.0) bad |= 1u;
+  if (cval != 0.0 && cval != 1.0) bad |= 2u;
+  return encode<T>(mval, cval != 0.0);
+}
+
 // Panel of columns [j0, j1) of the column-major inputs (panel-local pointers). Only the strict
 // upper triangle (i<j) is read (clipper.cpp:149-158); both (i,j) and (j,i) are written.
 // flags: bit0 = negative affinity seen, bit1 = constraint value outside {0,1}
@@ -1353,13 +1365,59 @@ __global__ void encode_dense_panel_kernel(const double* Mp, const double* Cp, in
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   const int j = j0 + blockIdx.y;
   if (j >= j1 || i >= j) return;
-  const double mval = Mp[(size_t)(j - j0) * m + i];
-  const double cval = Cp[(size_t)(j - j0) * m + i];
-  if (mval < 0.0) atomicOr(flags, 1);
-  if (cval != 0.0 && cval != 1.0) atomicOr(flags, 2);
-  const T e = encode<T>(mval, cval != 0.0);
+  unsigned int bad = 0;
+  const T e = dense_entry<T>(Mp[(size_t)(j - j0) * m + i], Cp[(size_t)(j - j0) * m + i], bad);
+  if (bad) atomicOr(flags, (int)bad);
   if (i >= row0 && i < row0 + rows) M[(size_t)(i - row0) * ld + j] = e;
   if (j >= row0 && j < row0 + rows) M[(size_t)(j - row0) * ld + i] = e;
+}
+
+// 32 x 32 tile [i0, i0 + 32) x [j0, j0 + 32) of caller-given M and C (entry (i, j) at base[i * rs + j * cs], one of
+// rs, cs is 1) into sh[i - i0][j - j0] through dense_entry, by 256 threads.  Entries outside i < j < m are neutral and
+// are not read.  The reads are coalesced along the unit-stride dimension.
+template <typename T, typename In>
+__device__ __forceinline__ void dense_tile_load(const In* Mg, const In* Cg, long long rs, long long cs, int m, int i0, int j0,
+                                                T (*sh)[33], unsigned int& bad) {
+  const int lane = threadIdx.x & 31, k0 = threadIdx.x >> 5;
+  const bool rowmajor = cs == 1;
+  In mv[4], cv[4];
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int k = k0 + 8 * q;
+    const int i = i0 + (rowmajor ? k : lane), j = j0 + (rowmajor ? lane : k);
+    const bool in = i < j && j < m;
+    const long long o = in ? (long long)i * rs + (long long)j * cs : 0;
+    mv[q] = in ? Mg[o] : In(0);
+    cv[q] = in ? Cg[o] : In(0);
+  }
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int k = k0 + 8 * q;
+    const int r = rowmajor ? k : lane, c = rowmajor ? lane : k;
+    sh[r][c] = (i0 + r < j0 + c && j0 + c < m) ? dense_entry<T>(mv[q], cv[q], bad) : encode<T>(0.0, false);
+  }
+}
+
+// clp_set_dense_dev: one CTA of 256 threads per tile pair (blockIdx.y <= blockIdx.x) of the strict upper triangle of
+// device-resident M and C; the tile and its mirror are stored row by row (coalesced along the store's rows).  The store
+// was filled with the neutral element before (begin_load), so only the entries i < j < m are written.
+template <typename T, typename In>
+__global__ void __launch_bounds__(256) load_dense_dev_kernel(const In* Mg, const In* Cg, int m, long long rs, long long cs,
+                                                             T* M, long long ld, int* flags) {
+  __shared__ T sh[32][33];
+  if (blockIdx.y > blockIdx.x) return;
+  const int i0 = blockIdx.y * 32, j0 = blockIdx.x * 32;
+  unsigned int bad = 0;
+  dense_tile_load<T, In>(Mg, Cg, rs, cs, m, i0, j0, sh, bad);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, k0 = threadIdx.x >> 5;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const int k = k0 + 8 * q;
+    if (i0 + k < j0 + lane && j0 + lane < m) M[(size_t)(i0 + k) * ld + j0 + lane] = sh[k][lane];  // (i, j)
+    if (i0 + lane < j0 + k && j0 + k < m) M[(size_t)(j0 + k) * ld + i0 + lane] = sh[lane][k];  // (j, i)
+  }
+  if (bad) atomicOr(flags, (int)bad);
 }
 
 // strictly-upper CSC -> HBM layout.  pass 0: M values (sign cleared => C=1 provisional is wrong),

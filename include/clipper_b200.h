@@ -118,6 +118,17 @@ int clp_score_pointnormal_dev(clp_handle h, const double* D1_dev, int64_t n1, co
 /* setMatrixData: strict upper triangle of the column-major m x m inputs is used, diagonal and
  * lower triangle ignored (clipper.cpp:149-158). Contract: M >= 0, C in {0,1} (clipper.h:166-176). */
 int clp_set_dense(clp_handle h, const double* M, const double* C, int64_t m);
+/* setMatrixData from matrices already on the handle's device (e.g. torch tensors): entry (i, j) of M and C is
+ * base[i * row_stride + j * col_stride] (element units; a torch tensor passes its own .stride(), a column-major caller
+ * (1, ld)), of element type CLP_IN_F32 (float) or CLP_IN_F64 (double).  Only entries i < j are read.  An fp32 input x
+ * is stored exactly as the fp64 value (double)x would be.  One stride must be 1 and the other >= 1; a bad stride, a NULL
+ * pointer or an unknown dtype is CLP_ERR_INVALID.  Otherwise the call behaves as clp_set_dense: same checks, error codes
+ * and messages, same compact layout, same state after a failure.  Runs on the handle's stream (clp_set_stream) and
+ * returns when the load and the build are done.  A sharded handle returns CLP_ERR_UNSUPPORTED. */
+#define CLP_IN_F32 0
+#define CLP_IN_F64 1
+int clp_set_dense_dev(clp_handle h, const void* M_dev, const void* C_dev, int64_t m, int dtype, int64_t row_stride,
+                      int64_t col_stride);
 /* setSparseMatrixData: strictly-upper CSC (column-major compressed) of M and of C (clipper.h:137). */
 int clp_set_sparse_upper(clp_handle h, int64_t m, const int64_t* colptrM, const int32_t* rowidxM,
                          const double* valM, const int64_t* colptrC, const int32_t* rowidxC,
@@ -275,6 +286,25 @@ int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
                              const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
                              const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
                              const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out);
+/* Run the batch's work on an existing cudaStream_t (e.g. torch's current stream); NULL -> handle-owned stream. */
+int clp_batch_set_stream(clp_batch b, void* cuda_stream);
+/* Problems given as dense matrices already on the batch's device (e.g. a torch tensor [nprob, m_max, m_max]): problem
+ * p is the leading m[p] x m[p] block (m host array, 1 <= m[p] <= 4096), entry (i, j) at
+ * base[p * batch_stride + i * row_stride + j * col_stride] of M_dev and C_dev (element units, type dtype: CLP_IN_F32 or
+ * CLP_IN_F64).  Only the strict upper triangle of each block is read: not the padding, the diagonal or the lower
+ * triangle.  u0 of problem p: m[p] doubles at u0_dev + p * u0_stride (device).  Problem p gets exactly what
+ * clp_batch_solve_matrices gives for the same values (u, score, d_final, ifinal, n_evals, n_inner, nodes and the
+ * kept-entry count of clp_batch_info).  u_out_dev (device, nullable) receives u of problem p at p * u_out_stride
+ * (u_out_stride >= the largest m[p]); nodes_out as for clp_batch_solve_*.  Errors, in this order: CLP_ERR_INVALID for
+ * bad sizes, pointers, strides (one of row_stride, col_stride is 1 and the other >= 1; batch_stride, u0_stride >= 1) or
+ * dtype; CLP_ERR_UNSUPPORTED for Rounding::DSD; then, found on the device, CLP_ERR_UNSUPPORTED naming the lowest problem
+ * with a negative M value, else the lowest with a C value other than 0 and 1 (NaN included).  A problem with bad values
+ * is not solved, the other outputs of a failed call are unspecified, and the handle stays usable.  Runs on the batch's
+ * stream (clp_batch_set_stream) and returns when the results are host-visible. */
+int clp_batch_solve_dense_dev(clp_batch b, int32_t nprob, const int64_t* m, int dtype, const void* M_dev, const void* C_dev,
+                              int64_t batch_stride, int64_t row_stride, int64_t col_stride, const double* u0_dev,
+                              int64_t u0_stride, clp_solution* sols, double* u_out_dev, int64_t u_out_stride,
+                              int32_t* const* nodes_out);
 /* diagnostics of the last batch: CTAs of the launch, HBM scratch bytes, and the kept entries i<j over all problems
  * (entries whose stored affinity is non-zero or whose C bit is set; for scored problems: the stored affinities) */
 int clp_batch_info(clp_batch b, int32_t* n_ctas, int64_t* scratch_bytes, int64_t* nnz_upper_total);
