@@ -5,7 +5,7 @@
 // an H100: as a stand-alone launch it pays a device-wide synchronisation per objective evaluation and leaves most of
 // the 132 SMs idle.  Here ONE CTA owns one problem from the raw inputs to the final iterate:
 //     gather the association endpoints -> score all pairs (fp32 screening, exact fp64 for the survivors: the arithmetic
-//     of score_tile_kernel) into a per-CTA fp32 scratch matrix -> build the full-row sliced-ELL copy (counting sort of
+//     of score_tile_kernel_runs) into a per-CTA fp32 scratch matrix -> build the full-row sliced-ELL copy (counting sort of
 //     the rows by length, item lengths, scan, item-wise fill: the steps of clp_sparse.cuh as device functions) ->
 //     run findDenseClique with the resident-vector solver body (clp_resident.cuh, SOLO: every "device-wide" exchange is
 //     a __syncthreads-level block reduction)
@@ -164,7 +164,7 @@ __device__ __forceinline__ void batch_score_pairs(const BatchProblem& P, const d
     __syncthreads();
   }
 
-  // ---- 2. scoring: warp per row, 128 columns per step; screening + survivor queue as in score_tile_kernel.
+  // ---- 2. scoring: warp per row, 128 columns per step; screening + survivor queue as in score_tile_kernel_runs.
   //      A row's warp evaluates its diagonal block of 128 columns and the blocks to the right of it; an entry kept in
   //      a block right of the diagonal block is also stored transposed (the pair functions are symmetric bit for bit:
   //      squared differences and commutative products), so every pair outside the diagonal blocks is evaluated once

@@ -698,19 +698,44 @@ bool screened_scoring(clp_handle h, int kind, int d) {
   return h->storage == CLP_STORE_F32 && (kind == 1 || d == 2 || d == 3);
 }
 
+// The persistent screened kernel runs one wave: as many CTAs as fit on the device at once.  The shared-memory opt-in
+// (more than 48 KB) is a property of the current device's context and is set on every launch; the occupancy is asked
+// once per device ordinal (ordinals past the table are asked every time).
+template <int KIND, int D, bool MIRROR>
+int launch_score_runs(clp_handle h, const ScoreArgs& a) {
+  const auto kernel = score_tile_kernel_runs<KIND, D, MIRROR>;
+  constexpr int smem = (int)sizeof(ScoreRunSmem<KIND == 1 ? 6 : D>);
+  CLP_CUDA(h, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+  constexpr int kCachedDevices = 64;
+  static std::atomic<int> occ_of[kCachedDevices];  // 0: not asked yet
+  const bool cached = h->device >= 0 && h->device < kCachedDevices;
+  int occ = cached ? occ_of[h->device].load(std::memory_order_relaxed) : 0;
+  if (occ == 0) {
+    CLP_CUDA(h, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, smem));
+    if (occ < 1) return fail(h, CLP_ERR_CUDA, "the screened scoring kernel does not fit on an SM");
+    if (cached) occ_of[h->device].store(occ, std::memory_order_relaxed);
+  }
+  const int nruns = (int)((h->ld / 128 + kRunTiles - 1) / kRunTiles), nrb = h->rows_pad / kRowTile;
+  const long long units = score_units_before<MIRROR>(nrb, nruns);
+  const unsigned grid = (unsigned)std::min<long long>(units, (long long)occ * h->sm_count);
+  kernel<<<grid, kThreads, smem, h->stream>>>(a);
+  CLP_CUDA(h, cudaGetLastError());
+  return CLP_OK;
+}
+
 template <typename T, bool MIRROR>
 int launch_score_m(clp_handle h, int kind, int d, const ScoreArgs& a) {
   dim3 grid((unsigned)(h->ld / 128), (unsigned)(h->rows_pad / kRowTile));
   if constexpr (sizeof(T) == 4) {
-    if (!screened_scoring(h, kind, d)) score_tile_kernel<T, 0, 0, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
-    else if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
-    else if (d == 3) score_tile_kernel<T, 0, 3, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
-    else score_tile_kernel<T, 0, 2, MIRROR, true><<<grid, kThreads, 0, h->stream>>>(a);
+    if (!screened_scoring(h, kind, d)) score_tile_kernel<T, 0, 0, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
+    else if (kind == 1) return launch_score_runs<1, 6, MIRROR>(h, a);
+    else if (d == 3) return launch_score_runs<0, 3, MIRROR>(h, a);
+    else return launch_score_runs<0, 2, MIRROR>(h, a);
   } else {
-    if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
-    else if (d == 3) score_tile_kernel<T, 0, 3, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
-    else if (d == 2) score_tile_kernel<T, 0, 2, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
-    else score_tile_kernel<T, 0, 0, MIRROR, false><<<grid, kThreads, 0, h->stream>>>(a);
+    if (kind == 1) score_tile_kernel<T, 1, 6, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
+    else if (d == 3) score_tile_kernel<T, 0, 3, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
+    else if (d == 2) score_tile_kernel<T, 0, 2, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
+    else score_tile_kernel<T, 0, 0, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
   }
   CLP_CUDA(h, cudaGetLastError());
   return CLP_OK;
@@ -743,7 +768,7 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   a.F1 = h->F12.as<float4>(); a.F2 = a.F1 + m; a.scale_bits = &sb->scale_bits;
   const CompactShape s = compact_shape(h);  // the layout the build of this call cuts (finalize_matrix_impl)
   const bool compact = compact_requested(h);
-  a.cnt = nullptr; a.W = s.W; a.win = nullptr; a.wwords = 0; a.expo = nullptr;
+  a.cnt = nullptr; a.W = s.W; a.win = nullptr; a.wwords = 0; a.expo = nullptr; a.next_unit = &sb->score_next;
   if (compact && screened_scoring(h, kind, d)) {
     // the screened scoring kernel also counts the kept entries per (segment, row): first pass of the compact build
     const size_t nptr = (size_t)s.nseg * (h->rows_pad + 1);

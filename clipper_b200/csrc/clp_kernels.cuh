@@ -102,7 +102,7 @@ struct SyncBlock {  // zeroed by the host before every launch
   unsigned long long counts[2];
   unsigned int scale_bits;         // scoring: float bits of max |position coordinate| (gather_endpoints_kernel)
   unsigned int expo[2];            // compact build: largest kept fp32 exponent, 255 - smallest (atomicMax, see pack_window)
-  unsigned int pad_;
+  unsigned int score_next;         // scoring: next work unit of score_tile_kernel_runs (ScoreArgs::next_unit)
 };
 
 struct TreeBar {
@@ -202,11 +202,11 @@ struct ScoreArgs {
   int d;             // runtime dimension (generic path)
   double p0, p1, p2, p3;  // sigma,epsilon,mindist | sigp,epsp,sign,epsn
   double affinityeps;
-  // fp32 screening (FILTER instances): positions of both endpoints as float4 and the largest |coordinate|
+  // fp32 screening (score_tile_kernel_runs): positions of both endpoints as float4 and the largest |coordinate|
   const float4* F1;  // [m] (x, y, z, 0) of E1
   const float4* F2;  // [m]
   const unsigned int* scale_bits;  // float bits of max |position coordinate| over E1 and E2 (written by the gather kernel)
-  // optional by-product (FILTER instances): kept entries per (column segment, local row), the first pass of the
+  // optional by-product (score_tile_kernel_runs): kept entries per (column segment, local row), the first pass of the
   // compact-copy build (clp_sparse.cuh); zeroed by the host, += by the kernel
   unsigned int* cnt;  // [NSEG][rows_pad + 1] or null
   int W;              // segment width (multiple of 128)
@@ -215,6 +215,7 @@ struct ScoreArgs {
   unsigned int* win;
   int wwords;
   unsigned int* expo;
+  unsigned int* next_unit;  // screened kernel: work-unit counter, zeroed by the host (SyncBlock::score_next)
 };
 
 __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.SQRT, relative error <= 2^-22
@@ -270,7 +271,7 @@ __device__ __forceinline__ bool keep_score(double scr, double affinityeps) {
   return scr > affinityeps && scr != 0.0;
 }
 
-// Threshold of the fp32 screen (FILTER instances, batch scoring): a pair is dropped iff |l1_32 - l2_32| >= thr.
+// Threshold of the fp32 screen (score_tile_kernel_runs, batch scoring): a pair is dropped iff |l1_32 - l2_32| >= thr.
 // R = largest |position coordinate| after conversion to fp32, u = 2^-24.  Converting the inputs (u R per coordinate),
 // the subtraction (2 u R more), the three-term sum of squares (3 u relative) and sqrt.approx (2^-22 relative) put the
 // fp32 length within 7 u R + 10 u l <= 42 u R of the exact one (d <= 3, l <= 2 sqrt(3) R) as long as no square
@@ -307,13 +308,9 @@ template <> struct Quad<double> {
 // MIRROR (unsharded handles): the score is symmetric in (i,j) bit for bit, so only tiles that touch the
 // upper triangle are computed; every value s(i,j), i<j, is stored at [i][j] (row-wise float4) and mirrored
 // to [j][i] (the lane's 4 rows of one column are 16 contiguous bytes of row j).  Halves the fp64 work.
-// FILTER (compile-time dimension only): the kernel is bound by fp64 arithmetic (two square roots and an exp
-// per pair), yet only ~15 % of the pairs pass the consistency test |l1 - l2| < epsilon.  Every pair is first
-// screened in fp32 against epsilon + a rigorous error margin (a pair is dropped only when the exact test must
-// fail too, so every stored value is still produced by the exact fp64 path below, bit for bit); the survivors
-// of a warp's 4 x 128 block are compacted into a shared-memory queue and scored 32 at a time with all lanes
-// busy, the results pass through a shared-memory copy of the block so that the stores stay row-wise float4.
-template <typename T, int KIND, int D, bool MIRROR, bool FILTER>
+// This is the unscreened kernel (fp64 storage, or a dimension without an fp32 screen); fp32 storage with
+// d = 2, 3 or PointNormal runs score_tile_kernel_runs below.
+template <typename T, int KIND, int D, bool MIRROR>
 __global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
   constexpr int DD = (KIND == 1) ? 6 : D;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -323,146 +320,12 @@ __global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
   T* Mbase = reinterpret_cast<T*>(a.M);
   const int dd = (DD > 0) ? DD : a.d;
 
-  // FILTER: survivor queue of every warp and the CTA's 32 x 128 block (row stride 132: the transposed reads of
-  // the mirror stores hit 8 banks instead of 1)
-  constexpr bool kF = FILTER && DD > 0;
-  __shared__ unsigned short queue[kF ? kWarps : 1][kF ? kRowsPerWarp * 128 : 1];
-  __shared__ __align__(16) T tile[kF ? kRowTile : 1][kF ? 132 : 4];
-  // fp64 endpoints of the block's 128 columns and 32 rows (E1 then E2; odd row stride against bank conflicts):
-  // the survivors' scattered 8-byte reads would otherwise keep the L1 data path 86 % busy
-  constexpr int kES = 2 * (DD > 0 ? DD : 1) + 1;
-  __shared__ double colE[kF ? 128 : 1][kES];
-  __shared__ double rowE[kF ? kRowTile : 1][kES];
-  __shared__ unsigned int s_expo[2];  // the block's kept exponent range (ScoreArgs::expo)
-
   T out[kRowsPerWarp][4];
 #pragma unroll
   for (int q = 0; q < kRowsPerWarp; ++q)
 #pragma unroll
     for (int e = 0; e < 4; ++e) out[q][e] = encode<T>(0.0, false);
 
-  if constexpr (kF) {
-    for (int idx = threadIdx.x; idx < 128 * DD; idx += kThreads) {
-      const int c = idx / DD, t = idx - c * DD, j = blockIdx.x * 128 + c;
-      colE[c][t] = (j < a.m) ? __ldg(a.E1 + (size_t)j * DD + t) : 0.0;
-      colE[c][DD + t] = (j < a.m) ? __ldg(a.E2 + (size_t)j * DD + t) : 0.0;
-    }
-    for (int idx = threadIdx.x; idx < kRowTile * DD; idx += kThreads) {
-      const int r = idx / DD, t = idx - r * DD, li = blockIdx.y * kRowTile + r;
-      rowE[r][t] = (li < a.rows) ? __ldg(a.E1 + (size_t)(a.row0 + li) * DD + t) : 0.0;
-      rowE[r][DD + t] = (li < a.rows) ? __ldg(a.E2 + (size_t)(a.row0 + li) * DD + t) : 0.0;
-    }
-    if (threadIdx.x < 2) s_expo[threadIdx.x] = 0u;
-    __syncthreads();
-#pragma unroll
-    for (int q = 0; q < kRowsPerWarp; ++q) Quad<T>::store(&tile[warp * kRowsPerWarp + q][lane * 4], out[q]);
-    // Screening threshold (screen_threshold: the error analysis and the scales where the screen is off).  A NaN
-    // length or threshold makes the comparison below false, i.e. the pair goes to the exact path.
-    const float R = __uint_as_float(*a.scale_bits);
-    const float thr = screen_threshold(a.p1, R);  // epsilon (Euclidean) / epsp (PointNormal)
-    unsigned int cnt = 0;
-    // the warp's four rows: association pair and fp32 positions, fetched once (warp-uniform broadcasts)
-    int ai0[kRowsPerWarp], ai1[kRowsPerWarp];
-    float4 f1i[kRowsPerWarp], f2i[kRowsPerWarp];
-#pragma unroll
-    for (int q = 0; q < kRowsPerWarp; ++q) {
-      const int li = lr0 + q;
-      ai0[q] = ai1[q] = -1; f1i[q] = f2i[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (li < a.rows) {
-        const int i = a.row0 + li;
-        ai0[q] = __ldg(a.A0 + i); ai1[q] = __ldg(a.A1 + i); f1i[q] = __ldg(a.F1 + i); f2i[q] = __ldg(a.F2 + i);
-      }
-    }
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int j = c0 + e;
-      const bool jok = (j < a.m) && !(MIRROR && j <= a.row0 + lr0);
-      int aj0 = -2, aj1 = -2;
-      float4 f1j = make_float4(0.f, 0.f, 0.f, 0.f), f2j = f1j;
-      if (jok) { aj0 = __ldg(a.A0 + j); aj1 = __ldg(a.A1 + j); f1j = __ldg(a.F1 + j); f2j = __ldg(a.F2 + j); }
-#pragma unroll
-      for (int q = 0; q < kRowsPerWarp; ++q) {
-        const int li = lr0 + q;
-        const int i = a.row0 + li;
-        const float x1 = f1i[q].x - f1j.x, y1 = f1i[q].y - f1j.y, z1 = f1i[q].z - f1j.z;
-        const float x2 = f2i[q].x - f2j.x, y2 = f2i[q].y - f2j.y, z2 = f2i[q].z - f2j.z;
-        const float l1 = sqrt_approx(fmaf(z1, z1, fmaf(y1, y1, x1 * x1)));
-        const float l2 = sqrt_approx(fmaf(z2, z2, fmaf(y2, y2, x2 * x2)));
-        // distinctness (ref clipper.cpp:35-38); "certainly inconsistent" last: a NaN keeps the pair
-        const bool cand = jok && li < a.rows && i != j && !(MIRROR && j < i) && ai0[q] != aj0 && ai1[q] != aj1 &&
-                          !(fabsf(l1 - l2) >= thr);
-        const unsigned int vote = __ballot_sync(0xffffffffu, cand);
-        if (cand) queue[warp][cnt + __popc(vote & ((1u << lane) - 1u))] = (unsigned short)((q << 7) | (e << 5) | lane);
-        cnt += __popc(vote);
-      }
-    }
-    __syncwarp();
-    for (unsigned int k = lane; k < cnt; k += 32) {
-      const unsigned int code = queue[warp][k];
-      const int q = code >> 7, e = (code >> 5) & 3, l = code & 31;
-      const int r = warp * kRowsPerWarp + q, c = l * 4 + e;
-      double e1i[DD], e2i[DD], e1j[DD], e2j[DD];
-#pragma unroll
-      for (int t = 0; t < DD; ++t) {
-        e1i[t] = rowE[r][t]; e2i[t] = rowE[r][DD + t];
-        e1j[t] = colE[c][t]; e2j[t] = colE[c][DD + t];
-      }
-      double scr;
-      if (KIND == 0) {
-        const double l1 = point_dist<DD>(e1i, e1j, 0), l2 = point_dist<DD>(e2i, e2j, 0);
-        scr = euclid_score(l1, l2, a.p0, a.p1, a.p2);
-      } else {
-        const double l1 = point_dist<3>(e1i, e1j, 0), l2 = point_dist<3>(e2i, e2j, 0);
-        const double dot1 = __dadd_rn(__dadd_rn(__dmul_rn(e1i[3], e1j[3]), __dmul_rn(e1i[4], e1j[4])), __dmul_rn(e1i[5], e1j[5]));
-        const double dot2 = __dadd_rn(__dadd_rn(__dmul_rn(e2i[3], e2j[3]), __dmul_rn(e2i[4], e2j[4])), __dmul_rn(e2i[5], e2j[5]));
-        scr = pointnormal_score(l1, l2, dot1, dot2, a.p0, a.p1, a.p2, a.p3);
-      }
-      if (keep_score(scr, a.affinityeps)) tile[warp * kRowsPerWarp + q][l * 4 + e] = encode<T>(scr, true);
-    }
-    __syncwarp();
-#pragma unroll
-    for (int q = 0; q < kRowsPerWarp; ++q)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) out[q][e] = tile[warp * kRowsPerWarp + q][lane * 4 + e];
-    if (a.cnt) {  // kept entries of the warp's four rows in this 128-column block (one column segment)
-      unsigned int packed = 0;  // four 8-bit fields, <= 128 each after the warp sum
-#pragma unroll
-      for (int q = 0; q < kRowsPerWarp; ++q)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) packed += (is_neutral<T>(out[q][e]) ? 0u : 1u) << (8 * q);
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) packed += __shfl_xor_sync(0xffffffffu, packed, o);
-      if (lane < kRowsPerWarp) {
-        const unsigned int c = (packed >> (8 * lane)) & 0xffu;
-        if (c) atomicAdd(a.cnt + (size_t)((blockIdx.x * 128) / a.W) * (a.rows_pad + 1) + lr0 + lane, c);
-      }
-      if constexpr (sizeof(T) == 4) {
-        if (a.win) {  // packed layout: occupied 16-column windows (lanes 4w..4w+3 = window w of the block), exponent range
-          unsigned int ehi = 0u, elo = 0u;
-#pragma unroll
-          for (int q = 0; q < kRowsPerWarp; ++q) {
-            bool any = false;
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              if (is_neutral<T>(out[q][e])) continue;
-              any = true;
-              const unsigned int x = (__float_as_uint(out[q][e]) >> 23) & 0xffu;
-              ehi = max(ehi, x); elo = max(elo, 255u - x);
-            }
-            const unsigned int v = __ballot_sync(0xffffffffu, any);
-            unsigned int wm = 0u;
-#pragma unroll
-            for (int w = 0; w < 8; ++w) wm |= ((v >> (4 * w)) & 0xfu) ? (1u << w) : 0u;
-            if (lane == q && wm) atomicOr(a.win + (size_t)(lr0 + q) * a.wwords + (blockIdx.x >> 2), wm << (8 * (blockIdx.x & 3)));
-          }
-          ehi = __reduce_max_sync(0xffffffffu, ehi); elo = __reduce_max_sync(0xffffffffu, elo);
-          if (lane == 0 && (ehi | elo)) { atomicMax(&s_expo[0], ehi); atomicMax(&s_expo[1], elo); }
-          __syncthreads();
-          if (threadIdx.x == 0 && (s_expo[0] | s_expo[1])) { atomicMax(a.expo, s_expo[0]); atomicMax(a.expo + 1, s_expo[1]); }
-        }
-      }
-    }
-  } else {
   // row endpoints are warp-uniform: fetched through the read-only path as broadcasts
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
@@ -505,7 +368,6 @@ __global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
       if (keep_score(scr, a.affinityeps)) out[q][e] = encode<T>(scr, true);
     }
   }
-  }  // !FILTER
   if (!MIRROR) {
 #pragma unroll
     for (int q = 0; q < kRowsPerWarp; ++q) {
@@ -527,39 +389,332 @@ __global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
         if (c0 + e >= i) Mbase[(size_t)i * a.ld + c0 + e] = out[q][e];
     }
   }
-  if constexpr (kF) {
-    // ... and the mirror image through the shared-memory block: column cc of the block is 32 consecutive
-    // elements (one 128-byte line) of row j = column index, stored by one warp instruction
-    __syncthreads();
-    const int i = blockIdx.y * kRowTile + lane;
-    for (int cc = warp; cc < 128; cc += kWarps) {
-      const int j = blockIdx.x * 128 + cc;
-      const bool st = j < a.rows_pad && i < j && i < a.ld;
-      const T v = tile[lane][cc];
-      if (st) Mbase[(size_t)j * a.ld + i] = v;
-      if (a.cnt) {  // the same 32 entries are a piece of row j inside the segment of this block's rows
-        const unsigned int vote = __ballot_sync(0xffffffffu, st && !is_neutral<T>(v));
-        if (lane == 0 && vote) atomicAdd(a.cnt + (size_t)((blockIdx.y * kRowTile) / a.W) * (a.rows_pad + 1) + j, (unsigned int)__popc(vote));
-        if (a.win && lane == 0) {  // the two 16-column windows of row j covered by this block's rows
-          const unsigned int wm = ((vote & 0xffffu) ? 1u : 0u) | ((vote >> 16) ? 2u : 0u);
-          if (wm) atomicOr(a.win + (size_t)j * a.wwords + (blockIdx.y * kRowTile) / 512, wm << (((blockIdx.y * kRowTile) / 16) & 31u));
-        }
-      }
+  // ... and the mirror image: column j of this thread's 4 rows is 4 consecutive elements of row j
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int j = c0 + e;
+    if (j >= a.rows_pad) continue;
+    T col[4] = {out[0][e], out[1][e], out[2][e], out[3][e]};
+    if (r0 + 3 < j && r0 + 3 < a.ld) Quad<T>::store(Mbase + (size_t)j * a.ld + r0, col);
+    else {
+#pragma unroll
+      for (int q = 0; q < kRowsPerWarp; ++q)
+        if (r0 + q < j && r0 + q < a.ld) Mbase[(size_t)j * a.ld + r0 + q] = col[q];
     }
-  } else {
-    // ... and the mirror image: column j of this thread's 4 rows is 4 consecutive elements of row j
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// K1, screened: fp32 storage and Euclidean d = 2, 3 or PointNormal.  The kernel is bound by fp64 arithmetic
+// (two square roots and an exp per pair), yet only ~15 % of the pairs pass the consistency test |l1 - l2| < epsilon.
+// Every pair is first screened in fp32 against epsilon + a rigorous error margin (a pair is dropped only when the
+// exact test must fail too, so every stored value is still produced by the exact fp64 path, bit for bit); the
+// survivors of a warp's 4 x 128 block are compacted into a shared-memory queue and scored 32 at a time with all lanes
+// busy, the results pass through a shared-memory copy of the block so that the stores stay row-wise float4.
+//
+// Persistent: one wave of CTAs draws work units from a device-wide counter.  A unit is a run of up to kRunTiles
+// consecutive 32 x 128 tiles of one row block, aligned to kRunTiles tiles (MIRROR: only tiles touching the upper
+// triangle).  A count-segment width W is only a multiple of 128 (mode 3 cuts round_up(ceil(m / NSEG), 128)), so a
+// run may cross a segment boundary: the row counts are flushed whenever the next tile lies in another segment.  Units are numbered row block by row block, left to right: the CTAs
+// of a wave work on neighbouring row blocks, and the last units handed out are the short rows at the bottom.
+//   * the row side (fp64 endpoints, association pair, fp32 positions of 32 rows) is loaded once per unit;
+//   * per-row kept counts are added up along the run and flushed once per (row block, column segment), the 16-column
+//     window bits once per 32-bit word, the exponent range once per CTA;
+//   * the column side of the next tile (fp64 endpoints, fp32 positions, association pairs) is copied into the other
+//     half of a double buffer with cp.async while the current tile is screened, scored and stored; columns at or past
+//     m are zero-filled by the copy itself.
+// The stores, the elements written and every stored bit are those of one tile of the unscreened kernel.
+// ------------------------------------------------------------------------------------------
+template <int DD>
+struct ScoreRunSmem {
+  static constexpr int kES = 2 * DD + 1;  // E1 then E2 of one endpoint; odd stride against bank conflicts
+  double colE[2][128][kES];               // double-buffered column endpoints
+  double rowE[kRowTile][kES];
+  float4 rowF[2][kRowTile];               // fp32 positions and association pair of the rows: read as broadcasts
+  int2 rowA[kRowTile];
+  float4 colF[2][2][128];                // [buffer][F1, F2][slot]: column c at slot (c & 3) * 32 + (c >> 2)
+  int colA[2][2][128];                    // [buffer][A0, A1][slot], same slots
+  float tile[kRowTile][132];              // row stride 132: the transposed reads of the mirror stores hit 8 banks, not 1
+  unsigned short queue[kWarps][kRowsPerWarp * 128];
+  unsigned int expo[2];
+  unsigned int unit[2];                   // the CTA's current and next work unit, alternating slots
+};
+
+template <int N>
+__device__ __forceinline__ void cp_async_zfill(void* dst, const void* src, bool ok) {  // N bytes, or N zero bytes
+  asm volatile("cp.async.ca.shared.global [%0], [%1], %2, %3;"
+               ::"r"((unsigned int)__cvta_generic_to_shared(dst)), "l"(src), "n"(N), "r"(ok ? N : 0) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
+
+constexpr int kRunTiles = 8;  // tiles per work unit of score_tile_kernel_runs (a power of two <= kSegMax / 128)
+
+// work units of row blocks 0 .. rb-1 (nruns = runs of a full row; MIRROR: row block rb starts at tile rb / 4, i.e. in
+// run rb / (4 kRunTiles))
+template <bool MIRROR>
+__host__ __device__ __forceinline__ long long score_units_before(int rb, int nruns) {
+  if (!MIRROR) return (long long)rb * nruns;
+  constexpr long long P = 4 * kRunTiles;
+  const long long q = rb / P, s = rb % P;
+  return (long long)rb * nruns - (P * q * (q - 1) / 2 + s * q);  // minus sum over r < rb of r / P
+}
+
+// unit u -> row block rb and its tiles [tb, tend)
+template <bool MIRROR>
+__device__ __forceinline__ void score_unit(unsigned int u, int nrb, int nt, int& rb, int& tb, int& tend) {
+  const int nruns = (nt + kRunTiles - 1) / kRunTiles;
+  int lo = 0;
+  for (int hi = nrb; hi - lo > 1;) {
+    const int mid = (lo + hi) >> 1;
+    if (score_units_before<MIRROR>(mid, nruns) <= (long long)u) lo = mid; else hi = mid;
+  }
+  rb = lo;
+  const int tb0 = MIRROR ? (rb >> 2) : 0;
+  const int run = tb0 / kRunTiles + (int)((long long)u - score_units_before<MIRROR>(rb, nruns));
+  tb = max(run * kRunTiles, tb0);
+  tend = min(run * kRunTiles + kRunTiles, nt);
+}
+
+template <int DD>
+__device__ __forceinline__ void score_fetch_columns(const ScoreArgs& a, ScoreRunSmem<DD>& s, int buf, int tb) {
+  const int j0 = tb * 128;
+  for (int idx = threadIdx.x; idx < 128 * DD; idx += kThreads) {
+    const int c = idx / DD, t = idx - c * DD, j = j0 + c;
+    const bool ok = j < a.m;
+    const size_t g = ok ? (size_t)j * DD + t : 0;
+    cp_async_zfill<8>(&s.colE[buf][c][t], a.E1 + g, ok);
+    cp_async_zfill<8>(&s.colE[buf][c][DD + t], a.E2 + g, ok);
+  }
+  const int c = threadIdx.x & 127, side = threadIdx.x >> 7, j = j0 + c, slot = (c & 3) * 32 + (c >> 2);
+  const bool ok = j < a.m;
+  cp_async_zfill<16>(&s.colF[buf][side][slot], (side ? a.F2 : a.F1) + (ok ? j : 0), ok);
+  cp_async_zfill<4>(&s.colA[buf][side][slot], (side ? a.A1 : a.A0) + (ok ? j : 0), ok);
+}
+
+template <int KIND, int D, bool MIRROR>
+__global__ void __launch_bounds__(kThreads, 4) score_tile_kernel_runs(ScoreArgs a) {
+  constexpr int DD = (KIND == 1) ? 6 : D;
+  static_assert(DD > 0, "the screened kernel needs a compile-time dimension");
+  extern __shared__ __align__(16) unsigned char score_smem[];
+  ScoreRunSmem<DD>& s = *reinterpret_cast<ScoreRunSmem<DD>*>(score_smem);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nt = (int)(a.ld / 128), nrb = a.rows_pad / kRowTile;
+  const long long total = score_units_before<MIRROR>(nrb, (nt + kRunTiles - 1) / kRunTiles);
+  float* Mbase = reinterpret_cast<float*>(a.M);
+
+  if (threadIdx.x == 0) s.unit[0] = atomicAdd(a.next_unit, 1u);
+  if (threadIdx.x < 2) s.expo[threadIdx.x] = 0u;
+  __syncthreads();
+  if ((long long)s.unit[0] >= total) return;
+  int rb, tb, tend;
+  score_unit<MIRROR>(s.unit[0], nrb, nt, rb, tb, tend);
+  score_fetch_columns<DD>(a, s, 0, tb);
+  cp_async_commit();
+
+  // Screening threshold (screen_threshold: the error analysis and the scales where the screen is off).  A NaN
+  // length or threshold makes the comparison below false, i.e. the pair goes to the exact path.
+  const float thr = screen_threshold(a.p1, __uint_as_float(*a.scale_bits));  // epsilon (Euclidean) / epsp (PointNormal)
+  unsigned int rowc = 0u, roww = 0u, ehi = 0u, elo = 0u;  // run accumulators (rowc, roww: lane q < 4 for row q)
+  int rb_loaded = -1;
+  unsigned int seq = 0, unext = 0;  // units taken so far; the unit after the current one
+  bool unit_start = true;
+
+  for (int n = 0;; ++n) {
+    const int buf = n & 1;
+    // the next unit is drawn while the current one starts; slot (seq + 1) & 1 was last read before the previous
+    // unit's first barrier, which thread 0 has passed
+    if (unit_start && threadIdx.x == 0) s.unit[(seq + 1) & 1] = atomicAdd(a.next_unit, 1u);
+
+    const int lr0 = rb * kRowTile + warp * kRowsPerWarp;  // local row of the warp's first row
+    if (rb != rb_loaded) {  // the row side of a new row block
+      __syncthreads();      // every warp is done with the previous block's rowE
+      for (int idx = threadIdx.x; idx < kRowTile * DD; idx += kThreads) {
+        const int r = idx / DD, t = idx - r * DD, li = rb * kRowTile + r;
+        s.rowE[r][t] = (li < a.rows) ? __ldg(a.E1 + (size_t)(a.row0 + li) * DD + t) : 0.0;
+        s.rowE[r][DD + t] = (li < a.rows) ? __ldg(a.E2 + (size_t)(a.row0 + li) * DD + t) : 0.0;
+      }
+      if (threadIdx.x < kRowTile) {
+        const int li = rb * kRowTile + threadIdx.x;
+        int2 ai = make_int2(-1, -1);
+        float4 f1 = make_float4(0.f, 0.f, 0.f, 0.f), f2 = f1;
+        if (li < a.rows) {
+          const int i = a.row0 + li;
+          ai = make_int2(__ldg(a.A0 + i), __ldg(a.A1 + i)); f1 = __ldg(a.F1 + i); f2 = __ldg(a.F2 + i);
+        }
+        s.rowA[threadIdx.x] = ai; s.rowF[0][threadIdx.x] = f1; s.rowF[1][threadIdx.x] = f2;
+      }
+      rb_loaded = rb;
+    }
+    cp_async_wait_all();
+    // this tile's columns and the row side are visible; every warp is done with the previous tile, so its column
+    // buffer and the shared block may be refilled
+    __syncthreads();
+    if (unit_start) unext = s.unit[(seq + 1) & 1];
+    int nrb_ = rb, ntb = tb + 1, ntend = tend;  // the next tile
+    const bool more = ntb < tend || (long long)unext < total;
+    if (ntb >= tend && more) score_unit<MIRROR>(unext, nrb, nt, nrb_, ntb, ntend);
+    if (more) {
+      score_fetch_columns<DD>(a, s, buf ^ 1, ntb);
+      cp_async_commit();
+    }
+
+    const int c0 = tb * 128 + lane * 4;
+    float out[kRowsPerWarp][4];
+#pragma unroll
+    for (int q = 0; q < kRowsPerWarp; ++q) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) out[q][e] = -0.0f;
+      Quad<float>::store(&s.tile[warp * kRowsPerWarp + q][lane * 4], out[q]);
+    }
+    unsigned int cnt = 0;
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int j = c0 + e;
-      if (j >= a.rows_pad) continue;
-      T col[4] = {out[0][e], out[1][e], out[2][e], out[3][e]};
-      if (r0 + 3 < j && r0 + 3 < a.ld) Quad<T>::store(Mbase + (size_t)j * a.ld + r0, col);
-      else {
+      const bool jok = (j < a.m) && !(MIRROR && j <= a.row0 + lr0);
+      const int slot = e * 32 + lane;
+      const int aj0 = s.colA[buf][0][slot], aj1 = s.colA[buf][1][slot];
+      const float4 f1j = s.colF[buf][0][slot], f2j = s.colF[buf][1][slot];
 #pragma unroll
-        for (int q = 0; q < kRowsPerWarp; ++q)
-          if (r0 + q < j && r0 + q < a.ld) Mbase[(size_t)j * a.ld + r0 + q] = col[q];
+      for (int q = 0; q < kRowsPerWarp; ++q) {
+        const int li = lr0 + q;
+        const int i = a.row0 + li;
+        const float4 f1i = s.rowF[0][warp * kRowsPerWarp + q], f2i = s.rowF[1][warp * kRowsPerWarp + q];
+        const int2 ai = s.rowA[warp * kRowsPerWarp + q];
+        const float x1 = f1i.x - f1j.x, y1 = f1i.y - f1j.y, z1 = f1i.z - f1j.z;
+        const float x2 = f2i.x - f2j.x, y2 = f2i.y - f2j.y, z2 = f2i.z - f2j.z;
+        const float l1 = sqrt_approx(fmaf(z1, z1, fmaf(y1, y1, x1 * x1)));
+        const float l2 = sqrt_approx(fmaf(z2, z2, fmaf(y2, y2, x2 * x2)));
+        // distinctness (ref clipper.cpp:35-38); "certainly inconsistent" last: a NaN keeps the pair
+        const bool cand = jok && li < a.rows && i != j && !(MIRROR && j < i) && ai.x != aj0 && ai.y != aj1 &&
+                          !(fabsf(l1 - l2) >= thr);
+        const unsigned int vote = __ballot_sync(0xffffffffu, cand);
+        if (cand) s.queue[warp][cnt + __popc(vote & ((1u << lane) - 1u))] = (unsigned short)((q << 7) | (e << 5) | lane);
+        cnt += __popc(vote);
       }
     }
+    __syncwarp();
+    for (unsigned int k = lane; k < cnt; k += 32) {
+      const unsigned int code = s.queue[warp][k];
+      const int q = code >> 7, e = (code >> 5) & 3, l = code & 31;
+      const int r = warp * kRowsPerWarp + q, c = l * 4 + e;
+      double e1i[DD], e2i[DD], e1j[DD], e2j[DD];
+#pragma unroll
+      for (int t = 0; t < DD; ++t) {
+        e1i[t] = s.rowE[r][t]; e2i[t] = s.rowE[r][DD + t];
+        e1j[t] = s.colE[buf][c][t]; e2j[t] = s.colE[buf][c][DD + t];
+      }
+      double scr;
+      if (KIND == 0) {
+        const double l1 = point_dist<DD>(e1i, e1j, 0), l2 = point_dist<DD>(e2i, e2j, 0);
+        scr = euclid_score(l1, l2, a.p0, a.p1, a.p2);
+      } else {
+        const double l1 = point_dist<3>(e1i, e1j, 0), l2 = point_dist<3>(e2i, e2j, 0);
+        const double dot1 = __dadd_rn(__dadd_rn(__dmul_rn(e1i[3], e1j[3]), __dmul_rn(e1i[4], e1j[4])), __dmul_rn(e1i[5], e1j[5]));
+        const double dot2 = __dadd_rn(__dadd_rn(__dmul_rn(e2i[3], e2j[3]), __dmul_rn(e2i[4], e2j[4])), __dmul_rn(e2i[5], e2j[5]));
+        scr = pointnormal_score(l1, l2, dot1, dot2, a.p0, a.p1, a.p2, a.p3);
+      }
+      if (keep_score(scr, a.affinityeps)) s.tile[r][c] = encode<float>(scr, true);
+    }
+    __syncwarp();
+#pragma unroll
+    for (int q = 0; q < kRowsPerWarp; ++q)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) out[q][e] = s.tile[warp * kRowsPerWarp + q][lane * 4 + e];
+
+    if (a.cnt) {  // kept entries of the warp's four rows in this tile, added to the run's counts
+      const int seg = (tb * 128) / a.W;
+      const bool flush = !more || nrb_ != rb || (ntb * 128) / a.W != seg;
+      unsigned int packed = 0;  // four 8-bit fields, <= 128 each after the warp sum
+#pragma unroll
+      for (int q = 0; q < kRowsPerWarp; ++q)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) packed += (is_neutral<float>(out[q][e]) ? 0u : 1u) << (8 * q);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) packed += __shfl_xor_sync(0xffffffffu, packed, o);
+      if (lane < kRowsPerWarp) rowc += (packed >> (8 * lane)) & 0xffu;
+      if (flush) {
+        if (lane < kRowsPerWarp && rowc) atomicAdd(a.cnt + (size_t)seg * (a.rows_pad + 1) + lr0 + lane, rowc);
+        rowc = 0u;
+      }
+      if (a.win) {  // packed layout: occupied 16-column windows (lanes 4w..4w+3 = window w of the tile), exponent range
+#pragma unroll
+        for (int q = 0; q < kRowsPerWarp; ++q) {
+          bool any = false;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            if (is_neutral<float>(out[q][e])) continue;
+            any = true;
+            const unsigned int x = (__float_as_uint(out[q][e]) >> 23) & 0xffu;
+            ehi = max(ehi, x); elo = max(elo, 255u - x);
+          }
+          const unsigned int v = __ballot_sync(0xffffffffu, any);
+          unsigned int wm = 0u;
+#pragma unroll
+          for (int w = 0; w < 8; ++w) wm |= ((v >> (4 * w)) & 0xfu) ? (1u << w) : 0u;
+          if (lane == q) roww |= wm << (8 * (tb & 3));
+        }
+        // one word holds the windows of 4 tiles
+        if (flush || (ntb >> 2) != (tb >> 2)) {
+          if (lane < kRowsPerWarp && roww) atomicOr(a.win + (size_t)(lr0 + lane) * a.wwords + (tb >> 2), roww);
+          roww = 0u;
+        }
+      }
+    }
+
+    if (!MIRROR) {
+#pragma unroll
+      for (int q = 0; q < kRowsPerWarp; ++q) {
+        const int li = lr0 + q;
+        if (li < a.rows_pad && c0 < a.ld) Quad<float>::store(Mbase + (size_t)li * a.ld + c0, out[q]);
+      }
+    } else {
+      // MIRROR: row0 == 0 and rows == m.  Row-wise stores of the part right of the diagonal (and the diagonal itself) ...
+#pragma unroll
+      for (int q = 0; q < kRowsPerWarp; ++q) {
+        const int i = lr0 + q;
+        if (i >= a.rows_pad || c0 >= a.ld) continue;
+        if (c0 > i) Quad<float>::store(Mbase + (size_t)i * a.ld + c0, out[q]);
+        else {
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            if (c0 + e >= i) Mbase[(size_t)i * a.ld + c0 + e] = out[q][e];
+        }
+      }
+      // ... and the mirror image through the shared-memory block: column cc of the block is 32 consecutive
+      // elements (one 128-byte line) of row j = column index, stored by one warp instruction.  The counts of the 16
+      // columns of a warp are kept one per lane and added with one warp-wide atomic each.
+      __syncthreads();
+      const int i = rb * kRowTile + lane;
+      unsigned int myvote = 0u;
+#pragma unroll 4
+      for (int k = 0; k < 128 / kWarps; ++k) {
+        const int cc = warp + k * kWarps, j = tb * 128 + cc;
+        const bool st = j < a.rows_pad && i < j && i < a.ld;
+        const float v = s.tile[lane][cc];
+        if (st) Mbase[(size_t)j * a.ld + i] = v;
+        const unsigned int vote = __ballot_sync(0xffffffffu, st && !is_neutral<float>(v));
+        if (lane == k) myvote = vote;
+      }
+      if (a.cnt && lane < 128 / kWarps && myvote) {  // the column's entries are a piece of row j in the segment of rb
+        const int j = tb * 128 + warp + lane * kWarps;
+        atomicAdd(a.cnt + (size_t)((rb * kRowTile) / a.W) * (a.rows_pad + 1) + j, (unsigned int)__popc(myvote));
+        if (a.win) {  // the two 16-column windows of row j covered by this block's rows
+          const unsigned int wm = ((myvote & 0xffffu) ? 1u : 0u) | ((myvote >> 16) ? 2u : 0u);
+          atomicOr(a.win + (size_t)j * a.wwords + (rb * kRowTile) / 512, wm << (((rb * kRowTile) / 16) & 31u));
+        }
+      }
+    }
+    if (!more) break;
+    unit_start = tb + 1 >= tend;
+    if (unit_start) ++seq;
+    rb = nrb_; tb = ntb; tend = ntend;
+  }
+  if (a.win) {  // the exponent range of every tile this CTA scored
+    ehi = __reduce_max_sync(0xffffffffu, ehi); elo = __reduce_max_sync(0xffffffffu, elo);
+    if (lane == 0 && (ehi | elo)) { atomicMax(&s.expo[0], ehi); atomicMax(&s.expo[1], elo); }
+    __syncthreads();
+    if (threadIdx.x == 0 && (s.expo[0] | s.expo[1])) { atomicMax(a.expo, s.expo[0]); atomicMax(a.expo + 1, s.expo[1]); }
   }
 }
 
