@@ -31,7 +31,9 @@ SYMBOLS = [
     "clp_max_clique", "clp_core_numbers",
     "clp_batch_max_clique_euclidean", "clp_batch_max_clique_pointnormal", "clp_batch_max_clique_graphs",
     "clp_batch_solve_matrices", "clp_set_dense_dev", "clp_batch_set_stream", "clp_batch_solve_dense_dev",
+    "clp_score_custom", "clp_score_custom_dev", "clp_invariant_check", "clp_jit_stats",
 ]
+INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 
 
@@ -103,6 +105,10 @@ def load():
     L.clp_score_pointnormal.argtypes = [vp, dp, i64, dp, i64, ip, i64, dbl, dbl, dbl, dbl]
     L.clp_score_euclidean_dev.argtypes = [vp, vp, i32, i64, vp, i64, vp, i64, dbl, dbl, dbl]
     L.clp_score_pointnormal_dev.argtypes = [vp, vp, i64, vp, i64, vp, i64, dbl, dbl, dbl, dbl]
+    L.clp_score_custom.argtypes = [vp, C.c_char_p, dp, i32, dp, i32, i64, dp, i64, ip, i64]
+    L.clp_score_custom_dev.argtypes = [vp, C.c_char_p, dp, i32, vp, i32, i64, vp, i64, vp, i64]
+    L.clp_invariant_check.argtypes = [C.c_char_p, i32, C.c_char_p, i64]
+    L.clp_jit_stats.argtypes = [lp, dp]
     L.clp_set_dense.argtypes = [vp, dp, dp, i64]
     L.clp_set_dense_dev.argtypes = [vp, vp, vp, i64, C.c_int, i64, i64]
     L.clp_set_sparse_upper.argtypes = [vp, i64, lp, ip, dp, lp, ip, dp]

@@ -118,10 +118,51 @@ class PointNormalDistance(PairwiseInvariant):
                            "there is no host implementation in this package")
 
 
+class CudaInvariant(PairwiseInvariant):
+    """A custom pairwise invariant written in CUDA C++ and scored on the GPU (clp_score_custom).  ``source`` defines
+
+        __device__ double clp_invariant(const double* ai, const double* aj, const double* bi, const double* bj,
+                                        int d, const double* prm);
+
+    ai, aj, bi, bj are the d coordinates of D1.col(A(i,0)), D1.col(A(j,0)), D2.col(A(i,1)), D2.col(A(j,1)); it is
+    called with i < j, and ``prm`` holds ``params`` (at most 16 floats).  The source is compiled at run time (NVRTC)
+    once per process and setting; a source that does not compile raises ClipperError with the compiler's log."""
+
+    def __init__(self, source, params=()):
+        self._source = str(source)
+        self._params = tuple(float(x) for x in params)
+
+    def source(self):
+        return self._source
+
+    def params(self):
+        return self._params
+
+    def __call__(self, ai, aj, bi, bj):
+        raise RuntimeError("CudaInvariant is evaluated on the GPU only")
+
+
+def check_cuda_invariant(source, d):
+    """compile ``source`` for dimension d as CudaInvariant scoring would (no GPU needed): None, or ClipperError
+    carrying the compiler's log"""
+    log = C.create_string_buffer(1 << 16)
+    rc = _capi.load().clp_invariant_check(str(source).encode(), int(d), log, len(log))
+    if rc != _capi.OK:
+        raise ClipperError(rc, log.value.decode(errors="replace"))
+
+
+def jit_stats():
+    """(run-time compilations of invariant sources in this process, their total milliseconds)"""
+    n, ms = C.c_int64(), C.c_double()
+    _capi.check(None, _capi.load().clp_jit_stats(C.byref(n), C.byref(ms)))
+    return int(n.value), float(ms.value)
+
+
 invariants = types.SimpleNamespace(
     Invariant=Invariant, PairwiseInvariant=PairwiseInvariant,
     EuclideanDistanceParams=EuclideanDistanceParams, EuclideanDistance=EuclideanDistance,
-    PointNormalDistanceParams=PointNormalDistanceParams, PointNormalDistance=PointNormalDistance)
+    PointNormalDistanceParams=PointNormalDistanceParams, PointNormalDistance=PointNormalDistance,
+    CudaInvariant=CudaInvariant, check_cuda_invariant=check_cuda_invariant)
 
 
 # --------------------------------------------------------------------------------------------
@@ -391,6 +432,10 @@ class CLIPPER:
             p = inv.params()
             rc = self._lib.clp_score_pointnormal(self._h, _dp(D1), n1, _dp(D2), n2, Ap, m,
                                                  float(p.sigp), float(p.epsp), float(p.sign), float(p.epsn))
+        elif isinstance(inv, CudaInvariant):  # before the generic branch: a CudaInvariant is a PairwiseInvariant too
+            prm = np.asarray(inv.params(), dtype=np.float64)
+            rc = self._lib.clp_score_custom(self._h, inv.source().encode(), _dp(prm) if prm.size else None, prm.size,
+                                            _dp(D1), d, n1, _dp(D2), n2, Ap, m)
         elif isinstance(inv, PairwiseInvariant):
             return self._score_custom(D1, D2, A if Ap is not None else None)
         else:

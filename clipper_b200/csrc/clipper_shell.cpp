@@ -3,9 +3,10 @@
 // This is the "reference-side binding": every method of clipper::CLIPPER marshals its Eigen-typed
 // arguments into plain pointers and calls include/clipper_b200.h (which launches the sm_90a
 // kernels).  Nothing numerical of the hot path happens in this file; what does happen here is
-//   * the custom-invariant host path (SURVEY D9): a user-defined PairwiseInvariant cannot run in a
-//     CUDA kernel, so it is evaluated pair by pair on the host (like reference clipper.cpp:31-56)
-//     and the resulting dense matrices are uploaded with clp_set_dense;
+//   * the custom-invariant host path (SURVEY D9): a user-defined PairwiseInvariant other than a
+//     CudaInvariant (which is compiled into the scoring kernel, clp_score_custom) is evaluated pair by
+//     pair on the host (like reference clipper.cpp:31-56) and the resulting dense matrices are
+//     uploaded with clp_set_dense;
 //   * single-pair operator() of the two built-in invariants (API completeness; the reference
 //     exposes them, e.g. py_clipper.cpp:43), never used for scoring association sets.
 #include "clipper/clipper.h"
@@ -116,6 +117,14 @@ void CLIPPER::scorePairwiseConsistency(const invariants::Data& D1, const invaria
     const auto& ip = pn->params();
     check(h, clp_score_pointnormal(h, D1.data(), (int64_t)D1.cols(), D2.data(), (int64_t)D2.cols(), Ap, m,
                                    ip.sigp, ip.epsp, ip.sign, ip.epsn), "clp_score_pointnormal");
+    return;
+  }
+  if (auto* cu = dynamic_cast<invariants::CudaInvariant*>(invariant_.get())) {
+    if (D1.rows() != D2.rows()) throw std::runtime_error("CudaInvariant expects D1 and D2 of equal dimension");
+    const auto& prm = cu->params();
+    check(h, clp_score_custom(h, cu->source().c_str(), prm.empty() ? nullptr : prm.data(), (int32_t)prm.size(),
+                              D1.data(), (int32_t)D1.rows(), (int64_t)D1.cols(), D2.data(), (int64_t)D2.cols(), Ap, m),
+          "clp_score_custom");
     return;
   }
 

@@ -8,6 +8,7 @@
 #include "clp_batch_clique.cuh"
 #include "clp_batch_matrix.cuh"
 #include "clp_host_utils.h"
+#include "clp_jit.h"
 #include "../../include/clipper_b200.h"
 
 #include <algorithm>
@@ -111,6 +112,7 @@ struct clp_handle_s {
   std::vector<int32_t> A_host;  // column-major m x 2
   DevBuf A_dev;                 // int32 [2m]
   DevBuf E1, E2, D1dev, D2dev, F12;  // F12: fp32 positions of both endpoints (screening pass of the scoring kernel)
+  DevBuf inv_prm;                    // parameters of a CUDA-source invariant (CLP_INV_MAX_PARAMS doubles)
   int prof_ctas = env_int("CLP_PROF_CTAS", 0);      // print the per-CTA phase times of every resident solve (stderr)
   int prof_host = env_int("CLP_PROF_HOST", 0);      // print wall-clock marks of the scoring / solve calls (stderr)
   int prof_laps = env_int("CLP_PROF_LAPS", 1);      // in-kernel phase timers (the split reported in clp_solution.prof_*)
@@ -695,7 +697,7 @@ int read_sync(clp_handle h, SyncBlock* sb) {
 // and also counts the kept entries (first pass of the compact build); every other case runs the plain kernel.  The
 // screened kernel's shared-memory block is sized for fp32 storage.
 bool screened_scoring(clp_handle h, int kind, int d) {
-  return h->storage == CLP_STORE_F32 && (kind == 1 || d == 2 || d == 3);
+  return h->storage == CLP_STORE_F32 && kind != 2 && (kind == 1 || d == 2 || d == 3);
 }
 
 // The persistent screened kernel runs one wave: as many CTAs as fit on the device at once.  The shared-memory opt-in
@@ -724,9 +726,12 @@ int launch_score_runs(clp_handle h, const ScoreArgs& a) {
 }
 
 template <typename T, bool MIRROR>
-int launch_score_m(clp_handle h, int kind, int d, const ScoreArgs& a) {
+int launch_score_m(clp_handle h, int kind, int d, const ScoreArgs& a, const void* custom) {
   dim3 grid((unsigned)(h->ld / 128), (unsigned)(h->rows_pad / kRowTile));
-  if constexpr (sizeof(T) == 4) {
+  if (kind == 2) {  // score_tile_kernel<T, 2, D, MIRROR> compiled for the caller's invariant (clp_jit.cpp)
+    void* args[] = {const_cast<ScoreArgs*>(&a)};
+    CLP_CUDA(h, cudaLaunchKernel(custom, grid, dim3(kThreads), args, 0, h->stream));
+  } else if constexpr (sizeof(T) == 4) {
     if (!screened_scoring(h, kind, d)) score_tile_kernel<T, 0, 0, MIRROR><<<grid, kThreads, 0, h->stream>>>(a);
     else if (kind == 1) return launch_score_runs<1, 6, MIRROR>(h, a);
     else if (d == 3) return launch_score_runs<0, 3, MIRROR>(h, a);
@@ -741,14 +746,16 @@ int launch_score_m(clp_handle h, int kind, int d, const ScoreArgs& a) {
   return CLP_OK;
 }
 template <typename T>
-int launch_score(clp_handle h, int kind, int d, const ScoreArgs& a) {
+int launch_score(clp_handle h, int kind, int d, const ScoreArgs& a, const void* custom) {
   // an unsharded handle holds the whole symmetric matrix: compute the upper triangle, mirror the rest
-  return (h->world == 1) ? launch_score_m<T, true>(h, kind, d, a) : launch_score_m<T, false>(h, kind, d, a);
+  return (h->world == 1) ? launch_score_m<T, true>(h, kind, d, a, custom) : launch_score_m<T, false>(h, kind, d, a, custom);
 }
 
-// common tail of the four scoring entry points: D1/D2/A already on the device
+// common tail of the scoring entry points: D1/D2/A already on the device.  kind 0 Euclidean, 1 PointNormal, 2 a
+// CUDA-source invariant: `custom` is its compiled kernel, its parameters are in h->inv_prm.
 int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long n1, const double* D2d,
-                    long long n2, const int32_t* Ad, long long m, double p0, double p1, double p2, double p3) {
+                    long long n2, const int32_t* Ad, long long m, double p0, double p1, double p2, double p3,
+                    const void* custom) {
   const auto tp0 = std::chrono::steady_clock::now();
   if (int rc = ensure_matrix(h, m)) return rc;
   CLP_CUDA(h, h->E1.ensure((size_t)m * d * sizeof(double)));
@@ -784,7 +791,8 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
     }
   }
   a.d = d; a.p0 = p0; a.p1 = p1; a.p2 = p2; a.p3 = p3; a.affinityeps = h->prm.affinityeps;
-  int rc = with_storage(h, [&](auto t) { return launch_score<decltype(t)>(h, kind, d, a); });
+  a.prm = (kind == 2) ? h->inv_prm.as<double>() : nullptr;
+  int rc = with_storage(h, [&](auto t) { return launch_score<decltype(t)>(h, kind, d, a, custom); });
   if (rc) return rc;
   if (!compact) {  // dense sweeps: nothing else synchronises with the scoring launch
     SyncBlock host;
@@ -803,9 +811,17 @@ int score_on_device(clp_handle h, int kind, const double* D1d, int d, long long 
   return CLP_OK;
 }
 
+// a CUDA-source invariant (kind 2): its source and parameters
+struct CustomInvariant {
+  const char* source;
+  const double* prm;  // host, nprm doubles
+  int nprm;
+};
+
 // the scoring entry points: D1, D2 and A on the host (clp_score_*) or on the device (clp_score_*_dev)
 int score(clp_handle h, bool on_device, int kind, const double* D1, int d, long long n1, const double* D2,
-          long long n2, const int32_t* A, long long m, double p0, double p1, double p2, double p3) {
+          long long n2, const int32_t* A, long long m, double p0, double p1, double p2, double p3,
+          const CustomInvariant* inv = nullptr) {
   if (!h) return CLP_ERR_INVALID;
   if (!D1 || !D2 || d <= 0 || n1 <= 0 || n2 <= 0 || (on_device && (m < 0 || (A && m == 0))))
     return fail(h, CLP_ERR_INVALID, on_device ? "bad device arguments" : "bad data set arguments");
@@ -815,6 +831,15 @@ int score(clp_handle h, bool on_device, int kind, const double* D1, int d, long 
     m = n1 * n2;
     if (m > (long long)kMaxSeg * kSegMax) return fail(h, CLP_ERR_INVALID, "all-to-all hypothesis too large");
   } else if (m < 0) return fail(h, CLP_ERR_INVALID, "negative m");
+  const void* custom = nullptr;
+  if (kind == 2) {  // compiled and loaded before anything of the handle changes: a failure leaves its matrix as it was
+    std::string err;
+    if (int rc = jit_score_kernel(inv->source, d, h->storage == CLP_STORE_F64, h->world == 1, h->device, &custom, &err))
+      return fail(h, rc, err);
+    CLP_CUDA(h, h->inv_prm.ensure(CLP_INV_MAX_PARAMS * sizeof(double)));
+    if (inv->nprm > 0)
+      CLP_CUDA(h, cudaMemcpyAsync(h->inv_prm.p, inv->prm, (size_t)inv->nprm * sizeof(double), cudaMemcpyHostToDevice, h->stream));
+  }
   CLP_CUDA(h, h->A_dev.ensure((size_t)2 * m * sizeof(int32_t)));
   if (!on_device) {
     CLP_CUDA(h, h->D1dev.ensure((size_t)d * n1 * sizeof(double)));
@@ -835,7 +860,18 @@ int score(clp_handle h, bool on_device, int kind, const double* D1, int d, long 
     CLP_CUDA(h, cudaMemcpyAsync(h->D2dev.p, D2, (size_t)d * n2 * sizeof(double), cudaMemcpyHostToDevice, h->stream));
     D1 = h->D1dev.as<double>(); D2 = h->D2dev.as<double>();
   }
-  return score_on_device(h, kind, D1, d, n1, D2, n2, h->A_dev.as<int32_t>(), m, p0, p1, p2, p3);
+  return score_on_device(h, kind, D1, d, n1, D2, n2, h->A_dev.as<int32_t>(), m, p0, p1, p2, p3, custom);
+}
+
+// clp_score_custom(_dev): the built-ins' argument checks, plus the source and the parameter count
+int score_custom(clp_handle h, bool on_device, const char* source, const double* prm, int32_t nprm, const double* D1,
+                 int32_t d, int64_t n1, const double* D2, int64_t n2, const int32_t* A, int64_t m) {
+  if (!h) return CLP_ERR_INVALID;
+  if (!source || !*source) return fail(h, CLP_ERR_INVALID, "empty invariant source");
+  if (nprm < 0 || nprm > CLP_INV_MAX_PARAMS || (nprm > 0 && !prm))
+    return fail(h, CLP_ERR_INVALID, "invariant parameters: 0 to " + std::to_string(CLP_INV_MAX_PARAMS) + " doubles");
+  const CustomInvariant inv{source, prm, nprm};
+  return score(h, on_device, 2, D1, d, n1, D2, n2, A, m, 0.0, 0.0, 0.0, 0.0, &inv);
 }
 
 // opens a load of a caller-given matrix (clp_set_dense, clp_set_sparse_upper): the store for m, no associations, a
@@ -1392,7 +1428,7 @@ int clp_destroy(clp_handle h) {
   for (int r = 0; r < kMaxPeers; ++r)
     if (h->peer_opened[r]) { cudaIpcCloseMemHandle(h->peer_open_ptr[r][0]); cudaIpcCloseMemHandle(h->peer_open_ptr[r][1]); }
   h->comm.release();
-  for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
+  for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->inv_prm, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
                     &h->mc_adj, &h->mc_work, &h->mc_scratch})
     b->release();
@@ -1443,6 +1479,40 @@ int clp_score_euclidean_dev(clp_handle h, const double* D1, int32_t d, int64_t n
 int clp_score_pointnormal_dev(clp_handle h, const double* D1, int64_t n1, const double* D2, int64_t n2,
                               const int32_t* A, int64_t m, double sigp, double epsp, double sign, double epsn) {
   return guarded(h, [&] { return score(h, true, 1, D1, 6, n1, D2, n2, A, m, sigp, epsp, sign, epsn); });
+}
+
+
+int clp_score_custom(clp_handle h, const char* source, const double* prm, int32_t nprm, const double* D1, int32_t d,
+                     int64_t n1, const double* D2, int64_t n2, const int32_t* A, int64_t m) {
+  return guarded(h, [&] { return score_custom(h, false, source, prm, nprm, D1, d, n1, D2, n2, A, m); });
+}
+int clp_score_custom_dev(clp_handle h, const char* source, const double* prm, int32_t nprm, const double* D1_dev,
+                         int32_t d, int64_t n1, const double* D2_dev, int64_t n2, const int32_t* A_dev, int64_t m) {
+  return guarded(h, [&] { return score_custom(h, true, source, prm, nprm, D1_dev, d, n1, D2_dev, n2, A_dev, m); });
+}
+
+int clp_invariant_check(const char* source, int32_t d, char* log, int64_t log_bytes) {
+  std::string msg;
+  int rc = CLP_ERR_INVALID;
+  if (!source || !*source) msg = "empty invariant source";
+  else if (d <= 0) msg = "dimension must be positive";
+  else {
+    try { rc = jit_check(source, d, &msg); }
+    catch (const std::exception& e) { msg = std::string("internal error: ") + e.what(); rc = CLP_ERR_INVALID; }
+  }
+  if (log && log_bytes > 0) {
+    const size_t n = std::min<size_t>(msg.size(), (size_t)log_bytes - 1);
+    std::memcpy(log, msg.data(), n);
+    log[n] = '\0';
+  }
+  return rc;
+}
+
+int clp_jit_stats(int64_t* compiles, double* compile_ms) {
+  long long c = 0;
+  jit_stats(&c, compile_ms);
+  if (compiles) *compiles = c;
+  return CLP_OK;
 }
 
 // ---- get / set ----------------------------------------------------------------------------

@@ -28,12 +28,10 @@
 #include <stdint.h>
 #include <type_traits>
 
+#include "clp_score_tile.cuh"
+
 namespace clp {
 
-constexpr int kThreads = 256;          // threads per CTA everywhere
-constexpr int kWarps = kThreads / 32;  // 8
-constexpr int kRowsPerWarp = 4;        // register blocking of the mat-vec (rows per warp)
-constexpr int kRowTile = kWarps * kRowsPerWarp;  // 32 rows per CTA item
 constexpr int kSegMax = 4096;          // max columns of v staged in shared memory per pass
 constexpr int kMaxSeg = 64;            // max number of column segments (m <= 262144)
 constexpr int kRedVals = 8;            // doubles per CTA in the partial-reduction table
@@ -59,30 +57,6 @@ __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
-}
-
-// element -> (|s| as double, C bit)
-__device__ __forceinline__ void decode(float s, double& a, bool& c) {
-  a = (double)fabsf(s);
-  c = __float_as_int(s) >= 0;
-}
-__device__ __forceinline__ void decode(double s, double& a, bool& c) {
-  a = fabs(s);
-  c = __double2hiint(s) >= 0;
-}
-template <typename T> __device__ __forceinline__ T encode(double mval, bool cbit);
-template <> __device__ __forceinline__ float encode<float>(double mval, bool cbit) {
-  const float a = fabsf((float)mval);
-  return cbit ? a : -a;
-}
-template <> __device__ __forceinline__ double encode<double>(double mval, bool cbit) {
-  const double a = fabs(mval);
-  return cbit ? a : -a;
-}
-template <typename T> __device__ __forceinline__ bool is_neutral(T s);
-template <> __device__ __forceinline__ bool is_neutral<float>(float s) { return __float_as_uint(s) == 0x80000000u; }
-template <> __device__ __forceinline__ bool is_neutral<double>(double s) {
-  return (unsigned long long)__double_as_longlong(s) == 0x8000000000000000ULL;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -188,87 +162,10 @@ __device__ __forceinline__ double ll_load(const uint4* p, unsigned tag, int* err
 // ------------------------------------------------------------------------------------------
 // K1: scoring
 // ------------------------------------------------------------------------------------------
-struct ScoreArgs {
-  const double* E1;  // [m][d] endpoint in data set 1 of association i  (D1.col(A(i,0)))
-  const double* E2;  // [m][d] endpoint in data set 2                   (D2.col(A(i,1)))
-  const int* A0;     // A(:,0)
-  const int* A1;     // A(:,1)
-  void* M;           // T [rows_pad][ld]
-  long long ld;
-  int m;
-  int row0;          // first global row stored here (row-block sharding)
-  int rows;          // number of real local rows
-  int rows_pad;
-  int d;             // runtime dimension (generic path)
-  double p0, p1, p2, p3;  // sigma,epsilon,mindist | sigp,epsp,sign,epsn
-  double affinityeps;
-  // fp32 screening (score_tile_kernel_runs): positions of both endpoints as float4 and the largest |coordinate|
-  const float4* F1;  // [m] (x, y, z, 0) of E1
-  const float4* F2;  // [m]
-  const unsigned int* scale_bits;  // float bits of max |position coordinate| over E1 and E2 (written by the gather kernel)
-  // optional by-product (score_tile_kernel_runs): kept entries per (column segment, local row), the first pass of the
-  // compact-copy build (clp_sparse.cuh); zeroed by the host, += by the kernel
-  unsigned int* cnt;  // [NSEG][rows_pad + 1] or null
-  int W;              // segment width (multiple of 128)
-  // optional with cnt (whole-row layout, packed candidate): per local row a bitmap of the aligned 16-column windows that
-  // hold a kept entry ([rows_pad][wwords], zeroed by the host, |= by the kernel) and the kept exponent range (SyncBlock::expo)
-  unsigned int* win;
-  int wwords;
-  unsigned int* expo;
-  unsigned int* next_unit;  // screened kernel: work-unit counter, zeroed by the host (SyncBlock::score_next)
-};
-
 __device__ __forceinline__ float sqrt_approx(float x) {  // MUFU.SQRT, relative error <= 2^-22
   float r;
   asm("sqrt.approx.f32 %0, %1;" : "=f"(r) : "f"(x));
   return r;
-}
-
-template <int D>
-__device__ __forceinline__ double point_dist(const double* a, const double* b, int d_rt) {
-  double s = 0.0;
-  if (D > 0) {
-#pragma unroll
-    for (int q = 0; q < D; ++q) { const double t = __dsub_rn(a[q], b[q]); s = __dadd_rn(s, __dmul_rn(t, t)); }
-  } else {
-    for (int q = 0; q < d_rt; ++q) { const double t = __dsub_rn(a[q], b[q]); s = __dadd_rn(s, __dmul_rn(t, t)); }
-  }
-  return __dsqrt_rn(s);
-}
-
-// EuclideanDistance::operator()  (ref euclidean_distance.cpp:13-31), same operation order as
-// the oracle, no FMA contraction in the distance / exponent argument.
-__device__ __forceinline__ double euclid_score(double l1, double l2, double sigma, double epsilon,
-                                               double mindist) {
-  if (mindist > 0 && (l1 < mindist || l2 < mindist)) return 0.0;
-  const double c = fabs(__dsub_rn(l1, l2));
-  if (!(c < epsilon)) return 0.0;
-  const double arg = __ddiv_rn(__dmul_rn(__dmul_rn(-0.5, c), c), __dmul_rn(sigma, sigma));
-  return exp(arg);
-}
-
-// PointNormalDistance::operator()  (ref pointnormal_distance.cpp:13-35). acos is NOT clamped:
-// |dot|>1 gives NaN, both comparisons are false, the score is 0.
-__device__ __forceinline__ double pointnormal_score(double l1, double l2, double dot1, double dot2,
-                                                    double sigp, double epsp, double sign, double epsn) {
-  const double alpha1 = acos(dot1);
-  const double alpha2 = acos(dot2);
-  const double dp = fabs(__dsub_rn(l1, l2));
-  const double dn = fabs(__dsub_rn(alpha1, alpha2));
-  if (dp < epsp && dn < epsn) {
-    const double sp = exp(__ddiv_rn(__dmul_rn(__dmul_rn(-0.5, dp), dp), __dmul_rn(sigp, sigp)));
-    const double sn = exp(__ddiv_rn(__dmul_rn(__dmul_rn(-0.5, dn), dn), __dmul_rn(sign, sign)));
-    return __dmul_rn(sp, sn);
-  }
-  return 0.0;
-}
-
-// A pair enters M and C iff its score exceeds affinityeps and is not 0: the reference writes scr > affinityeps into a
-// dense M and takes M.sparseView() (exact zeros dropped) as M and its pattern as C (ref clipper.cpp:53-64), so a pair
-// that scores exactly 0 is never in C, whatever the sign of affinityeps.  A positive score that fp32 storage rounds to
-// +0.0 stays in C (M = 0, C = 1), as in the reference's fp64 M.
-__device__ __forceinline__ bool keep_score(double scr, double affinityeps) {
-  return scr > affinityeps && scr != 0.0;
 }
 
 // Threshold of the fp32 screen (score_tile_kernel_runs, batch scoring): a pair is dropped iff |l1_32 - l2_32| >= thr.
@@ -289,120 +186,6 @@ __device__ __forceinline__ float screen_threshold(double eps, float R) {
   return __double2float_ru((eps + 1024.0 * 5.9604644775390625e-08 * (double)R) * (1.0 + 9.5367431640625e-07));
 }
 
-template <typename T> struct Quad;
-template <> struct Quad<float> {
-  static __device__ __forceinline__ void store(float* p, const float* v) {
-    *reinterpret_cast<float4*>(p) = make_float4(v[0], v[1], v[2], v[3]);
-  }
-};
-template <> struct Quad<double> {
-  static __device__ __forceinline__ void store(double* p, const double* v) {
-    reinterpret_cast<double2*>(p)[0] = make_double2(v[0], v[1]);
-    reinterpret_cast<double2*>(p)[1] = make_double2(v[2], v[3]);
-  }
-};
-
-// One CTA = a 32-row x 128-column tile of the padded dense matrix; warp w owns 4 rows, lane l
-// owns 4 consecutive columns -> every row is written as 512 B (float) of consecutive float4.
-// KIND 0: EuclideanDistance with compile-time dimension D (D==0: runtime d). KIND 1: PointNormal.
-// MIRROR (unsharded handles): the score is symmetric in (i,j) bit for bit, so only tiles that touch the
-// upper triangle are computed; every value s(i,j), i<j, is stored at [i][j] (row-wise float4) and mirrored
-// to [j][i] (the lane's 4 rows of one column are 16 contiguous bytes of row j).  Halves the fp64 work.
-// This is the unscreened kernel (fp64 storage, or a dimension without an fp32 screen); fp32 storage with
-// d = 2, 3 or PointNormal runs score_tile_kernel_runs below.
-template <typename T, int KIND, int D, bool MIRROR>
-__global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
-  constexpr int DD = (KIND == 1) ? 6 : D;
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int c0 = blockIdx.x * 128 + lane * 4;
-  const int lr0 = blockIdx.y * kRowTile + warp * kRowsPerWarp;  // local row
-  if (MIRROR && (int)(blockIdx.x * 128 + 127) < (int)(blockIdx.y * kRowTile)) return;  // tile entirely below the diagonal
-  T* Mbase = reinterpret_cast<T*>(a.M);
-  const int dd = (DD > 0) ? DD : a.d;
-
-  T out[kRowsPerWarp][4];
-#pragma unroll
-  for (int q = 0; q < kRowsPerWarp; ++q)
-#pragma unroll
-    for (int e = 0; e < 4; ++e) out[q][e] = encode<T>(0.0, false);
-
-  // row endpoints are warp-uniform: fetched through the read-only path as broadcasts
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const int j = c0 + e;
-    if (j >= a.m) continue;
-    if (MIRROR && j <= a.row0 + lr0) continue;  // column not right of any of this thread's rows
-    const int aj0 = __ldg(a.A0 + j), aj1 = __ldg(a.A1 + j);
-    double e1j[DD > 0 ? DD : 1], e2j[DD > 0 ? DD : 1];
-    if (DD > 0) {
-#pragma unroll
-      for (int q = 0; q < DD; ++q) { e1j[q] = __ldg(a.E1 + (size_t)j * DD + q); e2j[q] = __ldg(a.E2 + (size_t)j * DD + q); }
-    }
-#pragma unroll
-    for (int q = 0; q < kRowsPerWarp; ++q) {
-      const int li = lr0 + q;
-      const int i = a.row0 + li;
-      if (li >= a.rows || i == j) continue;
-      if (MIRROR && j < i) continue;  // lower triangle: written as the mirror of (j,i)
-      const int ai0 = __ldg(a.A0 + i), ai1 = __ldg(a.A1 + i);
-      if (ai0 == aj0 || ai1 == aj1) continue;  // distinctness (ref clipper.cpp:35-38)
-      double scr;
-      if (DD > 0) {
-        double e1i[DD > 0 ? DD : 1], e2i[DD > 0 ? DD : 1];
-#pragma unroll
-        for (int t = 0; t < DD; ++t) { e1i[t] = __ldg(a.E1 + (size_t)i * DD + t); e2i[t] = __ldg(a.E2 + (size_t)i * DD + t); }
-        if (KIND == 0) {
-          const double l1 = point_dist<DD>(e1i, e1j, 0), l2 = point_dist<DD>(e2i, e2j, 0);
-          scr = euclid_score(l1, l2, a.p0, a.p1, a.p2);
-        } else {
-          const double l1 = point_dist<3>(e1i, e1j, 0), l2 = point_dist<3>(e2i, e2j, 0);
-          const double dot1 = __dadd_rn(__dadd_rn(__dmul_rn(e1i[3], e1j[3]), __dmul_rn(e1i[4], e1j[4])), __dmul_rn(e1i[5], e1j[5]));
-          const double dot2 = __dadd_rn(__dadd_rn(__dmul_rn(e2i[3], e2j[3]), __dmul_rn(e2i[4], e2j[4])), __dmul_rn(e2i[5], e2j[5]));
-          scr = pointnormal_score(l1, l2, dot1, dot2, a.p0, a.p1, a.p2, a.p3);
-        }
-      } else {
-        const double l1 = point_dist<0>(a.E1 + (size_t)i * dd, a.E1 + (size_t)j * dd, dd);
-        const double l2 = point_dist<0>(a.E2 + (size_t)i * dd, a.E2 + (size_t)j * dd, dd);
-        scr = euclid_score(l1, l2, a.p0, a.p1, a.p2);
-      }
-      if (keep_score(scr, a.affinityeps)) out[q][e] = encode<T>(scr, true);
-    }
-  }
-  if (!MIRROR) {
-#pragma unroll
-    for (int q = 0; q < kRowsPerWarp; ++q) {
-      const int li = lr0 + q;
-      if (li < a.rows_pad && c0 < a.ld) Quad<T>::store(Mbase + (size_t)li * a.ld + c0, out[q]);
-    }
-    return;
-  }
-  // MIRROR: row0 == 0 and rows == m.  Row-wise stores of the part right of the diagonal (and the diagonal itself) ...
-  const int r0 = lr0;
-#pragma unroll
-  for (int q = 0; q < kRowsPerWarp; ++q) {
-    const int i = r0 + q;
-    if (i >= a.rows_pad || c0 >= a.ld) continue;
-    if (c0 > i) Quad<T>::store(Mbase + (size_t)i * a.ld + c0, out[q]);
-    else {
-#pragma unroll
-      for (int e = 0; e < 4; ++e)
-        if (c0 + e >= i) Mbase[(size_t)i * a.ld + c0 + e] = out[q][e];
-    }
-  }
-  // ... and the mirror image: column j of this thread's 4 rows is 4 consecutive elements of row j
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const int j = c0 + e;
-    if (j >= a.rows_pad) continue;
-    T col[4] = {out[0][e], out[1][e], out[2][e], out[3][e]};
-    if (r0 + 3 < j && r0 + 3 < a.ld) Quad<T>::store(Mbase + (size_t)j * a.ld + r0, col);
-    else {
-#pragma unroll
-      for (int q = 0; q < kRowsPerWarp; ++q)
-        if (r0 + q < j && r0 + q < a.ld) Mbase[(size_t)j * a.ld + r0 + q] = col[q];
-    }
-  }
-}
 
 // ------------------------------------------------------------------------------------------
 // K1, screened: fp32 storage and Euclidean d = 2, 3 or PointNormal.  The kernel is bound by fp64 arithmetic

@@ -137,6 +137,12 @@ void pybind_invariants(py::module& m)
     .def_readwrite("epsn", &PointNormalDistance::Params::epsn);
   py::class_<PointNormalDistance, PairwiseInvariant, std::shared_ptr<PointNormalDistance>>(m, "PointNormalDistance")
     .def(py::init<const PointNormalDistance::Params&>());
+
+  // additive: a custom invariant written in CUDA C++, scored on the GPU (not a Python subclass: parallelize stays on)
+  py::class_<CudaInvariant, PairwiseInvariant, std::shared_ptr<CudaInvariant>>(m, "CudaInvariant")
+    .def(py::init<std::string, std::vector<double>>(), "source"_a, "params"_a = std::vector<double>{})
+    .def("source", &CudaInvariant::source)
+    .def("params", &CudaInvariant::params);
 }
 
 void pybind_utils(py::module& m)

@@ -23,7 +23,8 @@ namespace invariants {
   using InvariantPtr = std::shared_ptr<Invariant>;
 
   /// Real-valued pairwise scoring function f : A x A x A x A -> R (reference abstract.h:56-72).
-  /// EuclideanDistance and PointNormalDistance are evaluated inside the CUDA scoring kernel;
+  /// EuclideanDistance and PointNormalDistance are evaluated inside the CUDA scoring kernel, and so is
+  /// CudaInvariant (cuda_invariant.h), a custom invariant written in CUDA C++ and compiled at run time;
   /// any other subclass is evaluated on the host, pair by pair, like the reference does.
   class PairwiseInvariant : public Invariant
   {

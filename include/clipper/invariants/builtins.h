@@ -2,3 +2,4 @@
 #pragma once
 #include "clipper/invariants/euclidean_distance.h"
 #include "clipper/invariants/pointnormal_distance.h"
+#include "clipper/invariants/cuda_invariant.h"

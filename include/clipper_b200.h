@@ -114,6 +114,33 @@ int clp_score_pointnormal_dev(clp_handle h, const double* D1_dev, int64_t n1, co
                               int64_t n2, const int32_t* A_dev, int64_t m, double sigp, double epsp,
                               double sign, double epsn);
 
+/* A custom PairwiseInvariant (invariants/abstract.h:56-72) written in CUDA C++.  `source` defines
+ *   __device__ double clp_invariant(const double* ai, const double* aj, const double* bi, const double* bj,
+ *                                   int d, const double* prm);
+ * with ai = D1.col(A(i,0)), aj = D1.col(A(j,0)), bi = D2.col(A(i,1)), bj = D2.col(A(j,1)) (d doubles each) and prm
+ * the nprm parameters (0 <= nprm <= CLP_INV_MAX_PARAMS; given on the host, read by the function from device memory).
+ * The library calls it once per distinct pair with i < j, on every handle (sharded ones too), and stores the result
+ * exactly as for the built-ins: pairs sharing an endpoint are skipped, a score is kept iff it is > affinityeps and
+ * != 0 (NaN is dropped), M and C are symmetric.  Every pair takes the fp64 path (there is no fp32 screen).  The
+ * function must terminate and stay in bounds; the library does not guard it (a fault is CLP_ERR_CUDA).  Kept scores
+ * must be >= 0, the contract of M everywhere (clp_set_dense rejects a negative M); a kept negative score is not
+ * detected, and its magnitude is stored.
+ * The source is compiled at run time with NVRTC (sm_90a, -std=c++17, default precision flags) together with the
+ * library's scoring kernel, once per (source, d, storage, sharded or not, device) in a process; later calls reuse the
+ * kernel.  A source that does not compile returns CLP_ERR_INVALID with the compiler's log in clp_last_error, before
+ * anything of the handle changes: the matrix it held stays as it was.  Other arguments as clp_score_euclidean(_dev). */
+#define CLP_INV_MAX_PARAMS 16
+int clp_score_custom(clp_handle h, const char* source, const double* prm, int32_t nprm, const double* D1, int32_t d,
+                     int64_t n1, const double* D2, int64_t n2, const int32_t* A, int64_t m);
+int clp_score_custom_dev(clp_handle h, const char* source, const double* prm, int32_t nprm, const double* D1_dev,
+                         int32_t d, int64_t n1, const double* D2_dev, int64_t n2, const int32_t* A_dev, int64_t m);
+/* Compiles `source` for dimension d as clp_score_custom would (no device needed, nothing loaded).  CLP_OK or
+ * CLP_ERR_INVALID; the compiler's log (NUL-terminated, cut to log_bytes) goes to log, which may be NULL. */
+int clp_invariant_check(const char* source, int32_t d, char* log, int64_t log_bytes);
+/* run-time compilations of invariant sources in this process (clp_score_custom*, clp_invariant_check) and their total
+ * wall-clock time in milliseconds; either pointer may be NULL */
+int clp_jit_stats(int64_t* compiles, double* compile_ms);
+
 /* ---- K7: matrix get/set (clipper.cpp:131-166) -------------------------------------------- */
 /* setMatrixData: strict upper triangle of the column-major m x m inputs is used, diagonal and
  * lower triangle ignored (clipper.cpp:149-158). Contract: M >= 0, C in {0,1} (clipper.h:166-176). */
