@@ -32,6 +32,7 @@ SYMBOLS = [
     "clp_batch_max_clique_euclidean", "clp_batch_max_clique_pointnormal", "clp_batch_max_clique_graphs",
     "clp_batch_solve_matrices", "clp_set_dense_dev", "clp_batch_set_stream", "clp_batch_solve_dense_dev",
     "clp_score_custom", "clp_score_custom_dev", "clp_invariant_check", "clp_jit_stats",
+    "clp_batch_solve_custom", "clp_batch_max_clique_custom",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
@@ -159,6 +160,10 @@ def load():
     L.clp_batch_max_clique_pointnormal.argtypes = [vp, i32, pp, lp, pp, lp, pp, lp, dbl, dbl, dbl, dbl, C.c_int, dbl,
                                                    mip, pp, pp]
     L.clp_batch_max_clique_graphs.argtypes = [vp, i32, lp, pp, pp, C.c_int, dbl, mip, pp, pp]
+    L.clp_batch_solve_custom.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, pp, lp, pp, lp, pp, lp, pp,
+                                         C.POINTER(ClpSolution), pp, pp]
+    L.clp_batch_max_clique_custom.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, pp, lp, pp, lp, pp, lp, C.c_int, dbl,
+                                              mip, pp, pp]
     _lib = L
     return L
 

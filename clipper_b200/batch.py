@@ -5,7 +5,9 @@ one after the other, each with a fresh clipper::CLIPPER (reference benchmarks/ma
 takes the whole list: one CTA per problem scores the pairs, builds the compact copy and runs the solver, no device-wide
 synchronisation anywhere; results per problem are those of ``CLIPPER.score_pairwise_consistency`` + ``solve``.
 ``BatchCLIPPER.max_clique_many`` and ``maxclique_many`` solve each problem of such a list as a maximum clique
-(clp_batch_max_clique_*): per problem the answer of ``CLIPPER.solve_as_maximum_clique`` on an fp32 handle.
+(clp_batch_max_clique_*): per problem the answer of ``CLIPPER.solve_as_maximum_clique`` on an fp32 handle.  A
+``BatchCLIPPER`` built with a ``CudaInvariant`` scores with the caller's CUDA source (clp_batch_*_custom): per problem
+what an fp32 ``CLIPPER`` with the same invariant gives.
 ``MatrixBatchCLIPPER`` solves problems whose (M, C) the caller gives (clp_batch_solve_matrices): per problem the
 result of ``CLIPPER.set_sparse_matrix_data`` / ``set_matrix_data`` + ``solve`` on an fp32 handle.
 """
@@ -14,16 +16,18 @@ import ctypes as C
 import numpy as np
 
 from . import _capi
-from .api import (EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64, _dev_matrix_dtype,
-                  _wait_for_torch)
+from .api import (CudaInvariant, EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64,
+                  _dev_matrix_dtype, _wait_for_torch)
 
 
 class BatchCLIPPER:
-    """invariant: EuclideanDistance (data 2 x n or 3 x n) or PointNormalDistance (6 x n); params: Params (rounding NONZERO or DSD_HEU)"""
+    """invariant: EuclideanDistance (data 2 x n or 3 x n), PointNormalDistance (6 x n) or CudaInvariant (d x n, one d
+    per call; compiled at run time once per source and d); params: Params (rounding NONZERO or DSD_HEU)"""
 
     def __init__(self, invariant, params=None, device=0):
-        if not isinstance(invariant, (EuclideanDistance, PointNormalDistance)):
-            raise TypeError("a batch scores with the built-in invariants (EuclideanDistance, PointNormalDistance)")
+        if not isinstance(invariant, (EuclideanDistance, PointNormalDistance, CudaInvariant)):
+            raise TypeError("a batch scores with the built-in invariants (EuclideanDistance, PointNormalDistance) or a "
+                            "CudaInvariant")
         self._lib = _capi.load()
         self._b = _new_batch(self._lib, device)
         self._invariant = invariant
@@ -62,7 +66,10 @@ class BatchCLIPPER:
         d, pts, ms, keep = _point_problems(problems)  # keep: the arrays pts points into, alive during the call
         inv = self._invariant
         out, args = _mc_outputs(ms, params)
-        if isinstance(inv, EuclideanDistance):
+        if isinstance(inv, CudaInvariant):
+            src, prm, nprm = _custom_args(inv)
+            rc = self._lib.clp_batch_max_clique_custom(self._b, src, prm, nprm, n, int(d), *pts, *args)
+        elif isinstance(inv, EuclideanDistance):
             q = inv.params()
             rc = self._lib.clp_batch_max_clique_euclidean(self._b, n, int(d), *pts, float(q.sigma), float(q.epsilon),
                                                           float(q.mindist), *args)
@@ -97,7 +104,10 @@ class BatchCLIPPER:
             u0p[k], up[k], np_[k] = u0.ctypes.data, uk.ctypes.data, nk.ctypes.data
         sols = (_capi.ClpSolution * n)()
         inv = self._invariant
-        if isinstance(inv, EuclideanDistance):
+        if isinstance(inv, CudaInvariant):
+            src, prm, nprm = _custom_args(inv)
+            rc = self._lib.clp_batch_solve_custom(self._b, src, prm, nprm, n, int(d), *pts, u0p, sols, up, np_)
+        elif isinstance(inv, EuclideanDistance):
             q = inv.params()
             rc = self._lib.clp_batch_solve_euclidean(self._b, n, int(d), *pts, u0p, float(q.sigma), float(q.epsilon),
                                                      float(q.mindist), sols, up, np_)
@@ -109,6 +119,12 @@ class BatchCLIPPER:
                                                        float(q.epsn), sols, up, np_)
         self._check(rc)
         return _solutions(sols, n, u0s, us, nodes)
+
+
+def _custom_args(inv):
+    """(source, parameter pointer, parameter count) of a CudaInvariant as clp_batch_*_custom take them"""
+    prm = (C.c_double * max(len(inv.params()), 1))(*inv.params())
+    return inv.source().encode(), (prm if inv.params() else None), len(inv.params())
 
 
 def _solutions(sols, n, u0s, us, nodes):

@@ -21,12 +21,8 @@ constexpr int kBatchWarps = kBatchThreads / 32;
 constexpr int kBatchMaxM = 4096;      // largest problem a batch may hold (shared-memory tables of the in-CTA build)
 constexpr int kBatchU = 2, kBatchD = 3;
 
-struct BatchProblem {       // device array, one per problem; offsets into the concatenated input / output arrays
-  long long d1_off, d2_off; // in doubles
-  long long a_off;          // in int32 (column-major m x 2), -1: all-to-all hypothesis (utils.h:61-71)
-  long long u_off;          // in doubles: u0 in, final iterate out
-  int n1, n2, m, pad_;
-};
+// BatchProblem, the problem table entry of every scored batch, is defined in clp_score_tile.cuh: the run-time compiled
+// scoring kernel of clp_batch_*_custom reads it too.
 
 // per-CTA scratch in HBM, sized for the largest problem of the batch.  points = false (matrices given by the caller,
 // clp_batch_matrix.cuh): the endpoint, fp32 position and association regions are empty
@@ -417,6 +413,73 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_solve_kernel(BatchArgs
                       ctafirst, val, idx, sc, L, smem, bs, cnt, ba.nnz_out, ba.prm, ba.u0, ba.u_out, ba.out, ba.sb,
                       ba.spin_limit, ba.prof, t_begin, t_scored, sa);
   }
+}
+
+// ---- batches scored with a caller's invariant (clp_batch_solve_custom, clp_batch_max_clique_custom) ---------------------
+// Two launches per round of problems (BatchScoreArgs, clp_score_tile.cuh): the run-time compiled batch_score_custom_kernel
+// over the whole grid, then an nvcc-built kernel with one CTA per problem that reads the stored matrix.  Before them,
+// batch_gather_kernel lays out slot k (grid y) for problem first + k: E1[i][d], E2[i][d] and A[i], A[m + i], as
+// gather_endpoints_kernel does for a handle.  An association index out of range (the host has checked them) sets
+// *error = 2 and gathers point 0.
+__global__ void __launch_bounds__(kBatchThreads) batch_gather_kernel(BatchScoreArgs b) {
+  const BatchProblem P = b.prob[b.first + blockIdx.y];
+  unsigned char* sc = b.scratch + (size_t)blockIdx.y * b.stride;
+  double* E1 = reinterpret_cast<double*>(sc + b.e1);
+  double* E2 = reinterpret_cast<double*>(sc + b.e2);
+  int* Ag = reinterpret_cast<int*>(sc + b.a);
+  const int d = b.d;
+  for (int i = blockIdx.x * kBatchThreads + threadIdx.x; i < P.m; i += gridDim.x * kBatchThreads) {
+    int a0, a1;
+    if (P.a_off >= 0) { a0 = b.A[P.a_off + i]; a1 = b.A[P.a_off + P.m + i]; }
+    else { a0 = i / P.n2; a1 = i % P.n2; }
+    if (a0 < 0 || a0 >= P.n1 || a1 < 0 || a1 >= P.n2) { atomicExch(b.error, 2); a0 = 0; a1 = 0; }
+    Ag[i] = a0; Ag[P.m + i] = a1;
+    for (int q = 0; q < d; ++q) {
+      E1[(size_t)i * d + q] = b.D1[P.d1_off + (size_t)a0 * d + q];
+      E2[(size_t)i * d + q] = b.D2[P.d2_off + (size_t)a1 * d + q];
+    }
+  }
+}
+
+// steps 3-4 for problems whose fp32 matrix the round's scoring launch left in their slots: CTA k solves problem
+// first + k from slot k (layout batch_layout(max_m, dd)).  The kept (non-neutral) entries of every row are counted from
+// the matrix, then batch_build_solve runs as batch_solve_kernel runs it, plain included (every stored score is kept
+// with C = 1).  prof's first phase is the count.
+__global__ void __launch_bounds__(kBatchThreads, 3) batch_stored_solve_kernel(BatchArgs ba, int first) {
+  extern __shared__ __align__(128) unsigned char clp_batch_smem[];
+  unsigned char* smem = clp_batch_smem;
+  __shared__ ResArgs sa;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int p = first + (int)blockIdx.x;
+  if (p >= ba.nprob) return;
+  const BatchLayout L = batch_layout(ba.max_m, ba.dd);
+  unsigned char* sc = ba.scratch + (size_t)blockIdx.x * ba.scratch_stride;
+  const float* M = reinterpret_cast<const float*>(sc + L.M);
+  const BatchProblem P = ba.prob[p];
+  const unsigned long long t_begin = global_ns();
+  const int m = P.m;
+  const int ld = (m + 127) / 128 * 128;
+  const int rows_pad = (m + 3) / 4 * 4;
+  const BatchSmem bs = batch_smem_plan(ba.max_m);
+  unsigned int* cnt = reinterpret_cast<unsigned int*>(smem + bs.cnt);  // [rows_pad]
+  for (int i = warp; i < rows_pad; i += kBatchWarps) {
+    unsigned int kept = 0;
+    for (int j = lane * 4; j < ld; j += 128) {
+      const float4 v = *reinterpret_cast<const float4*>(M + (size_t)i * ld + j);
+      kept += (is_neutral<float>(v.x) ? 0u : 1u) + (is_neutral<float>(v.y) ? 0u : 1u) +
+              (is_neutral<float>(v.z) ? 0u : 1u) + (is_neutral<float>(v.w) ? 0u : 1u);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) kept += __shfl_xor_sync(0xffffffffu, kept, o);
+    if (lane == 0) cnt[i] = kept;
+  }
+  __syncthreads();
+  const unsigned long long t_scored = global_ns();
+  batch_build_solve(p, m, ld, rows_pad, rows_pad / 4, P.u_off, /*plain*/ 1, M,
+                    reinterpret_cast<unsigned int*>(sc + L.rowid), reinterpret_cast<unsigned int*>(sc + L.itemptr),
+                    reinterpret_cast<unsigned int*>(sc + L.ctafirst), reinterpret_cast<float*>(sc + L.val),
+                    reinterpret_cast<unsigned short*>(sc + L.idx), sc, L, smem, bs, cnt, ba.nnz_out, ba.prm, ba.u0,
+                    ba.u_out, ba.out, ba.sb, ba.spin_limit, ba.prof, t_begin, t_scored, sa);
 }
 
 }  // namespace clp

@@ -17,7 +17,11 @@
 
 namespace clp {
 
-constexpr int kMcbKindGraph = 2;  // mc_batch_prepare_kernel<KIND, DD>: 0 Euclidean, 1 PointNormal, 2 graph given as pairs
+// mc_batch_prepare_kernel<KIND, DD>: 0 Euclidean, 1 PointNormal, 2 graph given as pairs, 3 fp32 matrix already stored
+// (clp_batch_max_clique_custom: the round's batch_score_custom_kernel left problem p's matrix in slot p, and `scratch`
+// points at the matrix region of slot 0)
+constexpr int kMcbKindGraph = 2;
+constexpr int kMcbKindStored = 3;
 
 struct McBatchProblem {   // device array, one per problem
   BatchProblem sp;        // scored problems: offsets of the inputs (sp.m is the problem's m)
@@ -142,16 +146,22 @@ __global__ void __launch_bounds__(kBatchThreads) mc_batch_prepare_kernel(McBatch
         if (lane == 0) deg[i] = c;
       }
     } else {
-      const McbLayout L = mcb_layout(ba.max_m, DD);
-      unsigned char* sc = ba.scratch + (size_t)blockIdx.x * ba.scratch_stride;
-      float* M = reinterpret_cast<float*>(sc + L.M);
-      batch_score_pairs<KIND, DD>(Q.sp, ba.D1 + Q.sp.d1_off, ba.D2 + Q.sp.d2_off, ba.A, ba.p0, ba.p1, ba.p2, ba.p3,
-                                  ba.affinityeps, ba.error, reinterpret_cast<double*>(sc + L.E1),
-                                  reinterpret_cast<double*>(sc + L.E2), reinterpret_cast<float4*>(sc + L.F1),
-                                  reinterpret_cast<float4*>(sc + L.F2), reinterpret_cast<int*>(sc + L.A), M,
-                                  reinterpret_cast<unsigned*>(mcb_smem + sp.cnt),
-                                  reinterpret_cast<unsigned short*>(mcb_smem + sp.queue),
-                                  reinterpret_cast<float*>(mcb_smem + sp.tile), reinterpret_cast<float*>(mcb_smem + sp.redf), s_R);
+      const float* M;
+      if constexpr (KIND == kMcbKindStored) {  // scored by the round's batch_score_custom_kernel into slot p
+        M = reinterpret_cast<const float*>(ba.scratch + (size_t)p * ba.scratch_stride);
+      } else {
+        const McbLayout L = mcb_layout(ba.max_m, DD);
+        unsigned char* sc = ba.scratch + (size_t)blockIdx.x * ba.scratch_stride;
+        float* Ms = reinterpret_cast<float*>(sc + L.M);
+        batch_score_pairs<KIND, DD>(Q.sp, ba.D1 + Q.sp.d1_off, ba.D2 + Q.sp.d2_off, ba.A, ba.p0, ba.p1, ba.p2, ba.p3,
+                                    ba.affinityeps, ba.error, reinterpret_cast<double*>(sc + L.E1),
+                                    reinterpret_cast<double*>(sc + L.E2), reinterpret_cast<float4*>(sc + L.F1),
+                                    reinterpret_cast<float4*>(sc + L.F2), reinterpret_cast<int*>(sc + L.A), Ms,
+                                    reinterpret_cast<unsigned*>(mcb_smem + sp.cnt),
+                                    reinterpret_cast<unsigned short*>(mcb_smem + sp.queue),
+                                    reinterpret_cast<float*>(mcb_smem + sp.tile), reinterpret_cast<float*>(mcb_smem + sp.redf), s_R);
+        M = Ms;
+      }
       const int ld = (m + 127) / 128 * 128;
       for (int i = warp; i < m; i += kBatchWarps) {  // mc_adjacency_kernel's rule: the sign bits of row i, no diagonal
         const float* row = M + (size_t)i * ld;

@@ -834,7 +834,7 @@ int score(clp_handle h, bool on_device, int kind, const double* D1, int d, long 
   const void* custom = nullptr;
   if (kind == 2) {  // compiled and loaded before anything of the handle changes: a failure leaves its matrix as it was
     std::string err;
-    if (int rc = jit_score_kernel(inv->source, d, h->storage == CLP_STORE_F64, h->world == 1, h->device, &custom, &err))
+    if (int rc = jit_score_kernel(JitKernel::kScoreTile, inv->source, d, h->storage == CLP_STORE_F64, h->world == 1, h->device, &custom, &err))
       return fail(h, rc, err);
     CLP_CUDA(h, h->inv_prm.ensure(CLP_INV_MAX_PARAMS * sizeof(double)));
     if (inv->nprm > 0)
@@ -1903,6 +1903,7 @@ struct clp_batch_s {
   int sm_count = 0, smem_optin = 0;
   DevBuf in_d1, in_d2, in_a, in_u0, out_u, probs, outs, nnz, sync, scratch, prof;
   DevBuf mat_in;  // batched matrices: column pointers | values | u0 | row indices | problem table
+  DevBuf custom_in;  // batches scored with a caller's invariant: parameters | work units | problem table
   // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
   DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
   int prof_on = env_int("CLP_PROF_BATCH", 0);
@@ -1959,15 +1960,100 @@ void batch_results(const clp_params& P, const std::vector<Prob>& probs, const do
   }
 }
 
-// Inputs of the batch C-ABI calls.  Scored problems: D1, n1, D2, n2, A, m and the invariant's parameters p; graphs
-// given as strictly-upper CSC patterns: m, colptr and rowidx.
+// Inputs of the batch C-ABI calls.  Scored problems: D1, n1, D2, n2, A, m and the invariant's parameters p, or for
+// clp_batch_*_custom the caller's invariant inv; graphs given as strictly-upper CSC patterns: m, colptr and rowidx.
 struct BatchInput {
   const double* const* D1 = nullptr; const int64_t* n1 = nullptr;
   const double* const* D2 = nullptr; const int64_t* n2 = nullptr;
   const int32_t* const* A = nullptr; const int64_t* m = nullptr;
   const int64_t* const* colptr = nullptr; const int32_t* const* rowidx = nullptr;
   double p[4] = {0.0, 0.0, 0.0, 0.0};
+  const CustomInvariant* inv = nullptr;
 };
+
+// the `kind` of batch_solve and batch_max_clique for problems scored with a caller's invariant (clp_batch_*_custom):
+// the clique's prepare kernel reads the stored matrix (0, 1: the built-ins, kMcbKindGraph: graphs)
+constexpr int kBatchKindCustom = kMcbKindStored;
+
+// ---- batches scored with a caller's invariant ---------------------------------------------------------------------
+// The scoring is compiled at run time (batch_score_custom_kernel, clp_jit.cpp); the build, the solve and the clique
+// steps are the nvcc-built kernels.  The problems go in rounds over the scratch slots batch_grid sized: round r gathers
+// and scores problems [rG, rG + G) into slots 0 .. G - 1 with the whole grid, then the stored-matrix kernel runs one CTA
+// per problem of the round.  Every round is enqueued on the batch's stream; the results are read once at the end.
+
+// the checks of a custom batch that come before everything else (CLP_ERR_INVALID): the source, the parameter count,
+// the dimension and every problem's m (stage_points repeats the last)
+int custom_check(clp_batch b, const CustomInvariant& inv, int32_t nprob, int dd, const BatchInput& in) {
+  if (!inv.source || !*inv.source) return fail(b, CLP_ERR_INVALID, "empty invariant source");
+  if (inv.nprm < 0 || inv.nprm > CLP_INV_MAX_PARAMS || (inv.nprm > 0 && !inv.prm))
+    return fail(b, CLP_ERR_INVALID, "invariant parameters: 0 to " + std::to_string(CLP_INV_MAX_PARAMS) + " doubles");
+  if (dd < 1) return fail(b, CLP_ERR_INVALID, "dimension must be positive");
+  for (int p = 0; p < nprob; ++p) {
+    if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
+    const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
+    const long long mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
+    if (mp <= 0 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
+  }
+  return CLP_OK;
+}
+
+// the compiled scoring of a custom batch and what its rounds read
+struct CustomRounds {
+  const void* fn = nullptr;      // batch_score_custom_kernel<D> for the caller's source
+  BatchScoreArgs sa{};
+  std::vector<long long> units;  // host copy of sa.units
+  int max_m = 1;
+};
+
+// compiles (or finds in the cache) the scoring kernel for inv and dimension d: CLP_ERR_INVALID with the compiler's log
+int custom_compile(clp_batch b, const CustomInvariant& inv, int d, CustomRounds* cr) {
+  std::string err;
+  if (int rc = jit_score_kernel(JitKernel::kBatchScore, inv.source, d, false, true, b->device, &cr->fn, &err))
+    return fail(b, rc, err);
+  return CLP_OK;
+}
+
+// uploads the parameters, the running count of work units and the problem table, and sets the arguments every round
+// shares: slots of `stride` bytes at `scratch`, their regions at the offsets of batch_layout / mcb_layout
+int custom_stage(clp_batch b, const CustomInvariant& inv, int d, const std::vector<BatchProblem>& probs, unsigned char* scratch,
+                 size_t stride, size_t e1, size_t e2, size_t a, size_t mat, CustomRounds* cr) {
+  const size_t nprob = probs.size();
+  cr->units.assign(nprob + 1, 0);
+  for (size_t p = 0; p < nprob; ++p) {
+    cr->units[p + 1] = cr->units[p] + batch_tile_units(probs[p].m);
+    cr->max_m = std::max(cr->max_m, probs[p].m);
+  }
+  const size_t units_at = CLP_INV_MAX_PARAMS * 8, table_at = batch_align(units_at + (nprob + 1) * 8);
+  std::vector<unsigned char> h(table_at + nprob * sizeof(BatchProblem));
+  if (inv.nprm > 0) std::memcpy(h.data(), inv.prm, (size_t)inv.nprm * 8);
+  std::memcpy(h.data() + units_at, cr->units.data(), (nprob + 1) * 8);
+  std::memcpy(h.data() + table_at, probs.data(), nprob * sizeof(BatchProblem));
+  CLP_CUDA(b, b->custom_in.ensure(h.size()));
+  CLP_CUDA(b, cudaMemcpyAsync(b->custom_in.p, h.data(), h.size(), cudaMemcpyHostToDevice, b->stream));
+  BatchScoreArgs& sa = cr->sa;
+  unsigned char* base = b->custom_in.as<unsigned char>();
+  sa.prob = reinterpret_cast<const BatchProblem*>(base + table_at);
+  sa.units = reinterpret_cast<const long long*>(base + units_at);
+  sa.D1 = b->in_d1.as<double>(); sa.D2 = b->in_d2.as<double>(); sa.A = b->in_a.as<int>();
+  sa.scratch = scratch; sa.stride = stride;
+  sa.e1 = e1; sa.e2 = e2; sa.a = a; sa.mat = mat;
+  sa.d = d; sa.affinityeps = b->prm.affinityeps;
+  sa.prm = reinterpret_cast<const double*>(base);
+  sa.error = &b->sync.as<SyncBlock>()->error;
+  return CLP_OK;
+}
+
+// enqueues the gather and the scoring of problems [first, first + count) into slots 0 .. count - 1
+int custom_score_round(clp_batch b, CustomRounds& cr, int first, int count) {
+  cr.sa.first = first; cr.sa.count = count;
+  batch_gather_kernel<<<dim3((unsigned)((cr.max_m + kBatchThreads - 1) / kBatchThreads), (unsigned)count), kBatchThreads, 0,
+                        b->stream>>>(cr.sa);
+  CLP_CUDA(b, cudaGetLastError());
+  const long long units = cr.units[(size_t)(first + count)] - cr.units[(size_t)first];
+  void* args[] = {&cr.sa};
+  CLP_CUDA(b, cudaLaunchKernel(cr.fn, dim3((unsigned)units), dim3(kThreads), args, 0, b->stream));
+  return CLP_OK;
+}
 
 // Point clouds of a scored batch: checks every problem (association indices included), fills its BatchProblem (offsets
 // of D1, D2 and A; m = n1 n2 where A, A[p] or m[p] is empty: the all-to-all hypothesis; u_off 0) and uploads D1, D2
@@ -2082,13 +2168,22 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
                 double* const* u_out, int32_t* const* nodes_out) {
   if (!b) return CLP_ERR_INVALID;
   if (nprob <= 0 || !in.D1 || !in.n1 || !in.D2 || !in.n2 || !in.m || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
-  if (!((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
+  const bool custom = kind == kBatchKindCustom;
+  if (custom) {
+    for (int p = 0; p < nprob; ++p)
+      if (!u0[p]) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null u0)");
+    if (int rc = custom_check(b, *in.inv, nprob, dd, in)) return rc;
+  } else if (!((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6))) {
     return fail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
+  }
   const clp_params& P = b->prm;
   if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
   if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
   const auto t_begin = std::chrono::steady_clock::now();
   CLP_CUDA(b, cudaSetDevice(b->device));
+  CustomRounds cr;
+  if (custom)
+    if (int rc = custom_compile(b, *in.inv, dd, &cr)) return rc;
   // ---- problem table and concatenated inputs
   for (int p = 0; p < nprob; ++p)
     if (!u0[p]) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null u0)");
@@ -2125,8 +2220,14 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
   const BatchSmem bs = batch_smem_plan(max_m);
   if ((long long)bs.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
   int occ = 0;
-  int rc = (kind == 1) ? batch_occupancy<1, 6>(b, bs.total, &occ) : (dd == 3 ? batch_occupancy<0, 3>(b, bs.total, &occ) : batch_occupancy<0, 2>(b, bs.total, &occ));
-  if (rc) return rc;
+  int rc = CLP_OK;
+  if (custom) {
+    CLP_CUDA(b, cudaFuncSetAttribute(batch_stored_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bs.total));
+    CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, batch_stored_solve_kernel, kBatchThreads, bs.total));
+  } else {
+    rc = (kind == 1) ? batch_occupancy<1, 6>(b, bs.total, &occ) : (dd == 3 ? batch_occupancy<0, 3>(b, bs.total, &occ) : batch_occupancy<0, 2>(b, bs.total, &occ));
+    if (rc) return rc;
+  }
   if (occ < 1) return fail(b, CLP_ERR_CUDA, "batch kernel does not fit an SM");
   const BatchLayout L = batch_layout(max_m, dd);
   int grid = 0;
@@ -2144,6 +2245,17 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
   ba.p0 = in.p[0]; ba.p1 = in.p[1]; ba.p2 = in.p[2]; ba.p3 = in.p[3]; ba.affinityeps = P.affinityeps;
   ba.sb = b->sync.as<SyncBlock>(); ba.spin_limit = 4LL * 1900000000LL;
   if (b->prof_on) { CLP_CUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  if (custom) {
+    if ((rc = custom_stage(b, *in.inv, dd, probs, ba.scratch, L.total, L.E1, L.E2, L.A, L.M, &cr))) return rc;
+    CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
+    for (int first = 0; first < nprob; first += grid) {
+      const int count = std::min(grid, nprob - first);
+      if ((rc = custom_score_round(b, cr, first, count))) return rc;
+      batch_stored_solve_kernel<<<count, kBatchThreads, bs.total, b->stream>>>(ba, first);
+      CLP_CUDA(b, cudaGetLastError());
+    }
+    return batch_finish(b, "batch custom", "count", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+  }
   CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   rc = (kind == 1) ? batch_launch<1, 6>(b, ba, grid, bs.total) : (dd == 3 ? batch_launch<0, 3>(b, ba, grid, bs.total) : batch_launch<0, 2>(b, ba, grid, bs.total));
   if (rc) return rc;
@@ -2391,9 +2503,12 @@ int batch_solve_dense_dev(clp_batch b, int32_t nprob, const int64_t* m, int dtyp
 
 // ---- batched maximum clique (clp_batch_clique.cuh) ----------------------------------------------------------------
 // kind 0 / 1: scored problems (EuclideanDistance d = 2, 3 / PointNormalDistance); kind 2: graphs given as strictly-upper
-// CSC patterns.  Phase A, then for EXACT with a positive time limit phases B and C: two host synchronisations.
+// CSC patterns; kBatchKindCustom: scored with a caller's invariant, phase A in rounds (gather and score, then the
+// prepare kernel on the stored matrices).  Phase A, then for EXACT with a positive time limit phases B and C: two host
+// synchronisations.
 const void* mcb_prepare_fn(int kind, int dd) {
   if (kind == kMcbKindGraph) return (const void*)mc_batch_prepare_kernel<kMcbKindGraph, 1>;
+  if (kind == kMcbKindStored) return (const void*)mc_batch_prepare_kernel<kMcbKindStored, 1>;
   if (kind == 1) return (const void*)mc_batch_prepare_kernel<1, 6>;
   return dd == 3 ? (const void*)mc_batch_prepare_kernel<0, 3> : (const void*)mc_batch_prepare_kernel<0, 2>;
 }
@@ -2404,17 +2519,23 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   const auto t_begin = std::chrono::steady_clock::now();
   if (nprob <= 0 || !infos || !in.m) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return fail(b, CLP_ERR_INVALID, "unknown maximum-clique method");
-  const bool graph = kind == kMcbKindGraph;
+  const bool graph = kind == kMcbKindGraph, custom = kind == kBatchKindCustom;
   if (graph ? (!in.colptr || !in.rowidx) : (!in.D1 || !in.n1 || !in.D2 || !in.n2))
     return fail(b, CLP_ERR_INVALID, "bad batch arguments");
-  if (!graph && !((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6)))
+  if (custom) {
+    if (int rc = custom_check(b, *in.inv, nprob, dd, in)) return rc;
+  } else if (!graph && !((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6))) {
     return fail(b, CLP_ERR_UNSUPPORTED, "batched scoring supports EuclideanDistance with d = 2, 3 and PointNormalDistance");
+  }
   const bool search = method == CLP_MC_EXACT && time_limit_s > 0;
   CLP_CUDA(b, cudaSetDevice(b->device));
+  CustomRounds cr;
+  if (custom)
+    if (int rc = custom_compile(b, *in.inv, dd, &cr)) return rc;
   // ---- problem table and per-problem regions; scored inputs are checked and uploaded by stage_points, graphs here
   std::vector<McBatchProblem> probs((size_t)nprob);
+  std::vector<BatchProblem> pts;
   if (!graph) {
-    std::vector<BatchProblem> pts;
     size_t bytes_pts = 0;
     if (int rc = stage_points(b, dd, nprob, in, pts, &bytes_pts)) return rc;
     for (int p = 0; p < nprob; ++p) probs[(size_t)p].sp = pts[(size_t)p];
@@ -2483,7 +2604,8 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   int occ = 0;
   CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kBatchThreads, sm.total));
   if (occ < 1) return fail(b, CLP_ERR_CUDA, "batched maximum-clique kernel does not fit an SM");
-  const size_t pstride = graph ? 0 : mcb_layout(max_m, dd).total;
+  const McbLayout ML = mcb_layout(max_m, dd);
+  const size_t pstride = graph ? 0 : ML.total;
   int grid = 0;
   if (int rc = batch_grid(b, occ, nprob, pstride, b->mc_pscratch,
                           "batched maximum clique: not enough device memory for one problem's scoring scratch", &grid))
@@ -2498,10 +2620,23 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   ba.p0 = in.p[0]; ba.p1 = in.p[1]; ba.p2 = in.p[2]; ba.p3 = in.p[3]; ba.affinityeps = b->prm.affinityeps;
   ba.error = &b->sync.as<SyncBlock>()->error;
   ba.scratch = b->mc_pscratch.as<unsigned char>(); ba.scratch_stride = pstride; ba.max_m = max_m;
+  if (custom)
+    if (int rc = custom_stage(b, *in.inv, dd, pts, ba.scratch, pstride, ML.E1, ML.E2, ML.A, ML.M, &cr)) return rc;
   McEvents ev;
   for (cudaEvent_t& x : ev.e) CLP_CUDA(b, cudaEventCreate(&x));
   CLP_CUDA(b, cudaEventRecord(ev.e[0], b->stream));
-  {
+  if (custom) {  // rounds: problem first + k in slot k; the prepare kernel sees the round's problems as 0 .. count - 1
+    ba.scratch += ML.M;
+    for (int first = 0; first < nprob; first += grid) {
+      const int count = std::min(grid, nprob - first);
+      if (int rc = custom_score_round(b, cr, first, count)) return rc;
+      McBatchArgs ra = ba;
+      ra.prob = ba.prob + first; ra.out = ba.out + first; ra.nprob = count;
+      CLP_CUDA(b, cudaMemsetAsync(ba.next, 0, sizeof(int), b->stream));
+      void* args[] = {&ra};
+      CLP_CUDA(b, cudaLaunchKernel(fn, dim3((unsigned)count), dim3(kBatchThreads), args, sm.total, b->stream));
+    }
+  } else {
     void* args[] = {&ba};
     CLP_CUDA(b, cudaLaunchKernel(fn, dim3((unsigned)grid), dim3(kBatchThreads), args, sm.total, b->stream));
   }
@@ -2690,7 +2825,7 @@ int clp_batch_create(int device, clp_batch* out) {
 int clp_batch_destroy(clp_batch b) {
   if (!b) return CLP_OK;
   cudaSetDevice(b->device);
-  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in,
+  for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in, &b->custom_in,
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
                     &b->mc_pscratch, &b->mc_sscratch})
     d->release();
@@ -2795,6 +2930,26 @@ int clp_batch_max_clique_graphs(clp_batch b, int32_t nprob, const int64_t* m, co
   BatchInput in;
   in.m = m; in.colptr = colptr; in.rowidx = rowidx;
   return guarded(b, [&] { return batch_max_clique(b, kMcbKindGraph, 0, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
+}
+
+int clp_batch_solve_custom(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                           const double* const* D1, const int64_t* n1, const double* const* D2, const int64_t* n2,
+                           const int32_t* const* A, const int64_t* m, const double* const* u0,
+                           clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
+  const CustomInvariant inv{source, prm, nprm};
+  BatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m; in.inv = &inv;
+  return guarded(b, [&] { return batch_solve(b, kBatchKindCustom, d, nprob, in, u0, sols, u_out, nodes_out); });
+}
+
+int clp_batch_max_clique_custom(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                                const double* const* D1, const int64_t* n1, const double* const* D2, const int64_t* n2,
+                                const int32_t* const* A, const int64_t* m, int method, double time_limit_s,
+                                clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  const CustomInvariant inv{source, prm, nprm};
+  BatchInput in;
+  in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m; in.inv = &inv;
+  return guarded(b, [&] { return batch_max_clique(b, kBatchKindCustom, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
 }
 
 }  // extern "C"

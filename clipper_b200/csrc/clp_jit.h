@@ -4,12 +4,15 @@
 
 namespace clp {
 
-// score_tile_kernel<T, 2, D, MIRROR> (clp_score_tile.cuh) with the caller's clp_invariant, T = double if f64 else float,
-// D = d for 1 <= d <= 16, else 0 (runtime d).  Compiled once per (source, d, T, MIRROR, device) and kept for the life
-// of the process; the kernel is loaded for `device`, which must be current.  Returns 0 and *fn (a handle for
-// cudaLaunchKernel), CLP_ERR_INVALID with the compiler's log in *err when the source does not compile, or CLP_ERR_CUDA
-// when the module cannot be loaded.
-int jit_score_kernel(const std::string& source, int d, bool f64, bool mirror, int device, const void** fn,
+// the kernels of clp_score_tile.cuh a caller's invariant is compiled into
+enum class JitKernel { kScoreTile = 0, kBatchScore = 1 };
+
+// kScoreTile: score_tile_kernel<T, 2, D, MIRROR> with the caller's clp_invariant, T = double if f64 else float;
+// kBatchScore: batch_score_custom_kernel<D> (f64 and mirror are not used).  D = d for 1 <= d <= 16, else 0 (runtime
+// d).  Compiled once per (kind, source, D, T, MIRROR, device) and kept for the life of the process; the kernel is loaded
+// for `device`, which must be current.  Returns 0 and *fn (a handle for cudaLaunchKernel), CLP_ERR_INVALID with the
+// compiler's log in *err when the source does not compile, or CLP_ERR_CUDA when the module cannot be loaded.
+int jit_score_kernel(JitKernel kind, const std::string& source, int d, bool f64, bool mirror, int device, const void** fn,
                      std::string* err);
 
 // compiles the fp32 / MIRROR instance for dimension d without loading it (no device needed); 0 or CLP_ERR_INVALID, the

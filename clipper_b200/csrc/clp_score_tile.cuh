@@ -1,8 +1,9 @@
-// clp_score_tile.cuh -- the unscreened scoring kernel (K1) and what it depends on.
+// clp_score_tile.cuh -- the unscreened scoring kernel (K1), its batched form for caller's invariants, and what they
+// depend on.
 //
 // This header has no includes: nvcc compiles it inside clp_kernels.cuh, and the library embeds its text and compiles it
-// again with NVRTC at run time, followed by a caller's CUDA-source invariant (KIND 2, clp_score_custom).  Both
-// compilers therefore see the same kernel text.
+// again with NVRTC at run time, followed by a caller's CUDA-source invariant (KIND 2: clp_score_custom, and
+// batch_score_custom_kernel for clp_batch_*_custom).  Both compilers therefore see the same kernel text.
 #pragma once
 
 // KIND 2: the pairwise invariant a caller supplies as CUDA source (clp_score_custom), defined after this header in the
@@ -239,6 +240,129 @@ __global__ void __launch_bounds__(kThreads) score_tile_kernel(ScoreArgs a) {
 #pragma unroll
       for (int q = 0; q < kRowsPerWarp; ++q)
         if (r0 + q < j && r0 + q < a.ld) Mbase[(size_t)j * a.ld + r0 + q] = col[q];
+    }
+  }
+}
+
+// ---- batches scored with a caller's invariant (clp_batch_solve_custom, clp_batch_max_clique_custom) ---------------------
+struct BatchProblem {       // device array, one per problem; offsets into the concatenated input / output arrays
+  long long d1_off, d2_off; // in doubles
+  long long a_off;          // in int32 (column-major m x 2), -1: all-to-all hypothesis (utils.h:61-71)
+  long long u_off;          // in doubles: u0 in, final iterate out
+  int n1, n2, m, pad_;
+};
+
+// One round of such a batch: problems [first, first + count), problem first + k in scratch slot k.  batch_gather_kernel
+// (clp_batch.cuh) lays out each slot's endpoints and associations as gather_endpoints_kernel does for a handle, then
+// batch_score_custom_kernel scores them into the slot's fp32 matrix (rows_pad x ld, ld = round_up(m, 128), rows_pad =
+// round_up(m, 4): the layout of batch_score_pairs), which the nvcc-built solve or clique kernel reads next.
+struct BatchScoreArgs {
+  const BatchProblem* prob;
+  const long long* units;   // [nprob + 1] running count of the problems' work units (batch_tile_units)
+  int first, count;
+  const double* D1; const double* D2; const int* A;  // the batch's concatenated inputs
+  unsigned char* scratch; size_t stride;             // slot k at scratch + k * stride
+  size_t e1, e2, a, mat;    // byte offsets of the endpoint, association and matrix regions in a slot
+  int d;
+  double affinityeps;
+  const double* prm;        // the caller's parameters (device memory)
+  int* error;               // set to 2 by the gather for an association index out of range
+};
+
+// work units of an m-association problem: the 32 x 128 tiles of score_tile that touch the upper triangle, row tile by
+// row tile (row tile by holds column tiles by / 4 .. ld / 128 - 1)
+__host__ __device__ inline long long batch_tile_units(int m) {
+  const int nct = (m + 127) / 128, nrt = (m + kRowTile - 1) / kRowTile;
+  long long u = 0;
+  for (int by = 0; by < nrt; ++by) u += nct - by * kRowTile / 128;
+  return u;
+}
+
+// One CTA per work unit of the round, over the whole grid.  A unit is the tile (bx, by) of problem p that
+// score_tile_kernel<float, 2, D, true> runs for it on an fp32 handle, and its body is that kernel's for KIND 2 and
+// MIRROR: the same loads, calls with i < j, storage rule and stores, row-wise right of the diagonal and mirrored below
+// it.  So problem p's matrix holds the handle's bits.
+template <int D>
+__global__ void __launch_bounds__(kThreads) batch_score_custom_kernel(BatchScoreArgs b) {
+  const long long u = b.units[b.first] + blockIdx.x;
+  int p = b.first, hi = b.first + b.count - 1;  // the problem whose units hold u (every problem has at least one)
+  while (p < hi) {
+    const int mid = (p + hi + 1) >> 1;
+    if (b.units[mid] <= u) p = mid; else hi = mid - 1;
+  }
+  const int m = b.prob[p].m, nct = (m + 127) / 128;
+  const int ld = nct * 128, rows_pad = (m + 3) / 4 * 4;
+  long long t = u - b.units[p];
+  int by = 0;
+  while (t >= nct - by * kRowTile / 128) { t -= nct - by * kRowTile / 128; ++by; }
+  const int bx = by * kRowTile / 128 + (int)t;
+  unsigned char* sc = b.scratch + (size_t)(p - b.first) * b.stride;
+  const double* E1 = reinterpret_cast<const double*>(sc + b.e1);
+  const double* E2 = reinterpret_cast<const double*>(sc + b.e2);
+  const int* A0 = reinterpret_cast<const int*>(sc + b.a);
+  const int* A1 = A0 + m;
+  float* Mbase = reinterpret_cast<float*>(sc + b.mat);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int c0 = bx * 128 + lane * 4;
+  const int r0 = by * kRowTile + warp * kRowsPerWarp;
+  const int dd = (D > 0) ? D : b.d;
+
+  float out[kRowsPerWarp][4];
+#pragma unroll
+  for (int q = 0; q < kRowsPerWarp; ++q)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) out[q][e] = encode<float>(0.0, false);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int j = c0 + e;
+    if (j >= m || j <= r0) continue;  // column not right of any of this thread's rows
+    const int aj0 = __ldg(A0 + j), aj1 = __ldg(A1 + j);
+    double e1j[D > 0 ? D : 1], e2j[D > 0 ? D : 1];
+    if (D > 0) {
+#pragma unroll
+      for (int q = 0; q < D; ++q) { e1j[q] = __ldg(E1 + (size_t)j * D + q); e2j[q] = __ldg(E2 + (size_t)j * D + q); }
+    }
+#pragma unroll
+    for (int q = 0; q < kRowsPerWarp; ++q) {
+      const int i = r0 + q;
+      if (i >= m || i >= j) continue;  // the lower triangle is written as the mirror of (j, i)
+      const int ai0 = __ldg(A0 + i), ai1 = __ldg(A1 + i);
+      if (ai0 == aj0 || ai1 == aj1) continue;  // distinctness (ref clipper.cpp:35-38)
+      double scr;
+      if (D > 0) {
+        double e1i[D > 0 ? D : 1], e2i[D > 0 ? D : 1];
+#pragma unroll
+        for (int s = 0; s < D; ++s) { e1i[s] = __ldg(E1 + (size_t)i * D + s); e2i[s] = __ldg(E2 + (size_t)i * D + s); }
+        scr = clp_invariant(e1i, e1j, e2i, e2j, D, b.prm);
+      } else {
+        scr = clp_invariant(E1 + (size_t)i * dd, E1 + (size_t)j * dd, E2 + (size_t)i * dd, E2 + (size_t)j * dd, dd, b.prm);
+      }
+      if (keep_score(scr, b.affinityeps)) out[q][e] = encode<float>(scr, true);
+    }
+  }
+  // row-wise stores of the part right of the diagonal (and the diagonal itself) ...
+#pragma unroll
+  for (int q = 0; q < kRowsPerWarp; ++q) {
+    const int i = r0 + q;
+    if (i >= rows_pad || c0 >= ld) continue;
+    if (c0 > i) Quad<float>::store(Mbase + (size_t)i * ld + c0, out[q]);
+    else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        if (c0 + e >= i) Mbase[(size_t)i * ld + c0 + e] = out[q][e];
+    }
+  }
+  // ... and the mirror image: column j of this thread's 4 rows is 4 consecutive elements of row j
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    const int j = c0 + e;
+    if (j >= rows_pad) continue;
+    float col[4] = {out[0][e], out[1][e], out[2][e], out[3][e]};
+    if (r0 + 3 < j && r0 + 3 < ld) Quad<float>::store(Mbase + (size_t)j * ld + r0, col);
+    else {
+#pragma unroll
+      for (int q = 0; q < kRowsPerWarp; ++q)
+        if (r0 + q < j && r0 + q < ld) Mbase[(size_t)j * ld + r0 + q] = col[q];
     }
   }
 }

@@ -137,7 +137,8 @@ int clp_score_custom_dev(clp_handle h, const char* source, const double* prm, in
 /* Compiles `source` for dimension d as clp_score_custom would (no device needed, nothing loaded).  CLP_OK or
  * CLP_ERR_INVALID; the compiler's log (NUL-terminated, cut to log_bytes) goes to log, which may be NULL. */
 int clp_invariant_check(const char* source, int32_t d, char* log, int64_t log_bytes);
-/* run-time compilations of invariant sources in this process (clp_score_custom*, clp_invariant_check) and their total
+/* run-time compilations of invariant sources in this process (clp_score_custom*, clp_batch_*_custom, clp_invariant_check)
+ * and their total
  * wall-clock time in milliseconds; either pointer may be NULL */
 int clp_jit_stats(int64_t* compiles, double* compile_ms);
 
@@ -366,6 +367,33 @@ int clp_batch_max_clique_pointnormal(clp_batch b, int32_t nprob, const double* c
 int clp_batch_max_clique_graphs(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* colptr,
                                 const int32_t* const* rowidx, int method, double time_limit_s, clp_mc_info* infos,
                                 int32_t* const* nodes_out, int32_t* const* core_out);
+
+/* ---- batches scored with a CUDA-source invariant (the batched form of clp_score_custom) ---------------------------
+ * Problem p of a batch scored with `source` and its nprm parameters prm gets exactly what an fp32 handle gives after
+ * clp_score_custom(h, source, prm, nprm, D1[p], d, n1[p], D2[p], n2[p], A[p], m[p]) with clp_batch_set_params'
+ * affinityeps, then clp_solve (clp_batch_solve_custom; outputs, rounding and kernel_ms as for clp_batch_solve_*) or
+ * clp_max_clique (clp_batch_max_clique_custom; outputs as for clp_batch_max_clique_*).  The function is called once per
+ * distinct pair with i < j, as on the handle; the storage rules are the handle's.  One source, one d >= 1 and one
+ * parameter set per call; m[p] <= 4096, A[p] == NULL: all-to-all.  The source is compiled (NVRTC) before anything is
+ * uploaded or launched, once per (source, d, device) in a process (clp_jit_stats counts it).
+ * The device work goes in rounds of as many problems as the batch has scratch slots (clp_batch_info's CTAs): the
+ * run-time compiled scoring kernel fills their fp32 matrices using the whole device, then the nvcc-built kernel of the
+ * built-in batches runs one CTA per problem from the stored matrix.  Rounds are enqueued back to back; each waits for
+ * its slowest problem.  For the maximum clique, adjacency_ms, peel_ms and heuristic_ms split the rounds' time,
+ * scoring included, by the prepare kernel's in-kernel time.
+ * Errors, in this order: CLP_ERR_INVALID for an empty source, nprm outside [0, CLP_INV_MAX_PARAMS], bad sizes or
+ * pointers, d < 1, m[p] outside [1, 4096] (and, for the maximum clique, an unknown method); CLP_ERR_UNSUPPORTED for
+ * Rounding::DSD (solve only); CLP_ERR_INVALID with the compiler's log for a source that does not compile; then the checks
+ * of the built-in batches (association indices out of range: CLP_ERR_INVALID).  The handle stays usable after any of
+ * them. */
+int clp_batch_solve_custom(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                           const double* const* D1, const int64_t* n1, const double* const* D2, const int64_t* n2,
+                           const int32_t* const* A, const int64_t* m, const double* const* u0,
+                           clp_solution* sols, double* const* u_out, int32_t* const* nodes_out);
+int clp_batch_max_clique_custom(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                                const double* const* D1, const int64_t* n1, const double* const* D2, const int64_t* n2,
+                                const int32_t* const* A, const int64_t* m, int method, double time_limit_s,
+                                clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
 
 #ifdef __cplusplus
 }
