@@ -33,6 +33,8 @@ SYMBOLS = [
     "clp_batch_solve_matrices", "clp_set_dense_dev", "clp_batch_set_stream", "clp_batch_solve_dense_dev",
     "clp_score_custom", "clp_score_custom_dev", "clp_invariant_check", "clp_jit_stats",
     "clp_batch_solve_custom", "clp_batch_max_clique_custom",
+    "clp_batch_solve_euclidean_dev", "clp_batch_solve_pointnormal_dev", "clp_batch_solve_custom_dev",
+    "clp_batch_max_clique_euclidean_dev", "clp_batch_max_clique_pointnormal_dev", "clp_batch_max_clique_custom_dev",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
@@ -67,6 +69,15 @@ class ClpMcInfo(C.Structure):
         ("proven", C.c_int32), ("timed_out", C.c_int32), ("n_edges", C.c_int64), ("n_branches", C.c_int64),
         ("t", C.c_double), ("kernel_ms", C.c_double),
         ("adjacency_ms", C.c_double), ("peel_ms", C.c_double), ("heuristic_ms", C.c_double), ("search_ms", C.c_double),
+    ]
+
+
+class ClpPointsDev(C.Structure):
+    """clp_points_dev: point clouds and associations of a batch on the device (element strides), sizes on the host."""
+    _fields_ = [
+        ("D1", C.c_void_p), ("d1_strides", C.c_int64 * 3), ("D2", C.c_void_p), ("d2_strides", C.c_int64 * 3),
+        ("A", C.c_void_p), ("a_strides", C.c_int64 * 3),
+        ("n1", C.POINTER(C.c_int64)), ("n2", C.POINTER(C.c_int64)), ("m", C.POINTER(C.c_int64)),
     ]
 
 
@@ -164,6 +175,14 @@ def load():
                                          C.POINTER(ClpSolution), pp, pp]
     L.clp_batch_max_clique_custom.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, pp, lp, pp, lp, pp, lp, C.c_int, dbl,
                                               mip, pp, pp]
+    # batches on the device: clp_points_dev, device u0 / u (void*), host solutions and nodes
+    ptp, sp = C.POINTER(ClpPointsDev), C.POINTER(ClpSolution)
+    L.clp_batch_solve_euclidean_dev.argtypes = [vp, i32, i32, ptp, vp, i64, dbl, dbl, dbl, sp, vp, i64, pp]
+    L.clp_batch_solve_pointnormal_dev.argtypes = [vp, i32, ptp, vp, i64, dbl, dbl, dbl, dbl, sp, vp, i64, pp]
+    L.clp_batch_solve_custom_dev.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, ptp, vp, i64, sp, vp, i64, pp]
+    L.clp_batch_max_clique_euclidean_dev.argtypes = [vp, i32, i32, ptp, dbl, dbl, dbl, C.c_int, dbl, mip, pp, pp]
+    L.clp_batch_max_clique_pointnormal_dev.argtypes = [vp, i32, ptp, dbl, dbl, dbl, dbl, C.c_int, dbl, mip, pp, pp]
+    L.clp_batch_max_clique_custom_dev.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, ptp, C.c_int, dbl, mip, pp, pp]
     _lib = L
     return L
 

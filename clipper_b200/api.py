@@ -442,6 +442,52 @@ class CLIPPER:
             raise TypeError("invariant must derive from invariants.PairwiseInvariant")
         _capi.check(self._h, rc)
 
+    def score_pairwise_consistency_dev(self, D1, D2, A=None):
+        """score_pairwise_consistency from CUDA tensors on the handle's device (clp_score_*_dev, clp_score_custom_dev):
+        D1, D2: (d, n) float64; A: (m, 2) int32 or None for the all-to-all hypothesis.  Tensors whose layout differs
+        from the column-major one the library reads are copied on the device first.  A PairwiseInvariant other than the
+        built-ins and CudaInvariant runs on the host: TypeError.  Without a stream of the caller's, torch's current
+        stream is synchronised first."""
+        import torch
+        inv = self._invariant
+        if not isinstance(inv, (EuclideanDistance, PointNormalDistance, CudaInvariant)):
+            raise TypeError("score_pairwise_consistency_dev scores with EuclideanDistance, PointNormalDistance or a "
+                            "CudaInvariant; other invariants run on the host (score_pairwise_consistency)")
+        given = [("D1", D1, torch.float64), ("D2", D2, torch.float64)] + ([("A", A, torch.int32)] if A is not None else [])
+        for name, X, dt in given:
+            if not isinstance(X, torch.Tensor) or X.dtype != dt:
+                raise TypeError("%s must be a %s torch tensor" % (name, dt))
+        if D1.dim() != 2 or D2.dim() != 2 or D1.shape[0] != D2.shape[0]:
+            raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+        if A is not None and (A.dim() != 2 or A.shape[1] != 2):
+            raise ValueError("A must be (m, 2)")
+        for name, X, _ in given:
+            if not X.is_cuda or X.device.index != self._device:
+                raise ValueError("%s must be a CUDA tensor on cuda:%d, got one on %s" % (name, self._device, X.device))
+        d, n1, n2 = D1.shape[0], D1.shape[1], D2.shape[1]
+        if isinstance(inv, PointNormalDistance) and d != 6:
+            raise ValueError("PointNormalDistance expects 6 x n data (point; normal)")
+        self._sync_params()
+        # column-major (d, n) and (m, 2): row-major (n, d) and (2, m); contiguous() copies only when the layout differs
+        P1, P2 = D1.t().contiguous(), D2.t().contiguous()
+        At = A.t().contiguous() if A is not None and A.shape[0] > 0 else None
+        Ap, m = (At.data_ptr(), At.shape[1]) if At is not None else (None, 0)
+        _wait_for_torch(self._stream, D1.device)
+        self._A_custom = None
+        if isinstance(inv, EuclideanDistance):
+            p = inv.params()
+            rc = self._lib.clp_score_euclidean_dev(self._h, P1.data_ptr(), d, n1, P2.data_ptr(), n2, Ap, m,
+                                                   float(p.sigma), float(p.epsilon), float(p.mindist))
+        elif isinstance(inv, PointNormalDistance):
+            p = inv.params()
+            rc = self._lib.clp_score_pointnormal_dev(self._h, P1.data_ptr(), n1, P2.data_ptr(), n2, Ap, m,
+                                                     float(p.sigp), float(p.epsp), float(p.sign), float(p.epsn))
+        else:
+            prm = np.asarray(inv.params(), dtype=np.float64)
+            rc = self._lib.clp_score_custom_dev(self._h, inv.source().encode(), _dp(prm) if prm.size else None, prm.size,
+                                                P1.data_ptr(), d, n1, P2.data_ptr(), n2, Ap, m)
+        _capi.check(self._h, rc)
+
     def _score_custom(self, D1, D2, A):
         """Custom-invariant host path (SURVEY D9): a user functor cannot run inside a CUDA kernel,
         so it is evaluated per pair on the host exactly like clipper.cpp:31-56 and the dense

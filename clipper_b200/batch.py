@@ -7,7 +7,8 @@ synchronisation anywhere; results per problem are those of ``CLIPPER.score_pairw
 ``BatchCLIPPER.max_clique_many`` and ``maxclique_many`` solve each problem of such a list as a maximum clique
 (clp_batch_max_clique_*): per problem the answer of ``CLIPPER.solve_as_maximum_clique`` on an fp32 handle.  A
 ``BatchCLIPPER`` built with a ``CudaInvariant`` scores with the caller's CUDA source (clp_batch_*_custom): per problem
-what an fp32 ``CLIPPER`` with the same invariant gives.
+what an fp32 ``CLIPPER`` with the same invariant gives.  ``solve_many_dev`` and ``max_clique_many_dev`` take the point
+clouds and associations as padded CUDA tensors (clp_batch_*_dev) and give what the host calls give for the same values.
 ``MatrixBatchCLIPPER`` solves problems whose (M, C) the caller gives (clp_batch_solve_matrices): per problem the
 result of ``CLIPPER.set_sparse_matrix_data`` / ``set_matrix_data`` + ``solve`` on an fp32 handle.
 """
@@ -30,6 +31,8 @@ class BatchCLIPPER:
                             "CudaInvariant")
         self._lib = _capi.load()
         self._b = _new_batch(self._lib, device)
+        self._device = int(device)
+        self._stream = None   # a caller's stream set with set_stream, else the batch's own
         self._invariant = invariant
         self._params = params if params is not None else Params()
 
@@ -51,6 +54,12 @@ class BatchCLIPPER:
         a, b, c = C.c_int32(), C.c_int64(), C.c_int64()
         self._check(self._lib.clp_batch_info(self._b, C.byref(a), C.byref(b), C.byref(c)))
         return int(a.value), int(b.value), int(c.value)
+
+    def set_stream(self, cuda_stream):
+        """run on an existing CUDA stream (an int handle, e.g. torch.cuda.current_stream().cuda_stream); None or 0: the
+        batch's own stream"""
+        self._check(self._lib.clp_batch_set_stream(self._b, C.c_void_p(cuda_stream or None)))
+        self._stream = cuda_stream or None
 
     def max_clique_many(self, problems, params=None):
         """problems: the dicts of solve_many (u0 is not needed); params: MCParams (method, time_limit for the whole
@@ -119,6 +128,125 @@ class BatchCLIPPER:
                                                        float(q.epsn), sols, up, np_)
         self._check(rc)
         return _solutions(sols, n, u0s, us, nodes)
+
+    def solve_many_dev(self, D1, D2, A, u0, n1=None, n2=None, m=None):
+        """solve_many for problems already on the batch's device (clp_batch_solve_*_dev).  D1: (B, d, n1_max) and D2:
+        (B, d, n2_max) float64 CUDA tensors, any strides (an ``expand`` along B shares one cloud); A: (B, m_max, 2) int32
+        CUDA tensor, or None for the all-to-all hypothesis everywhere; u0: (B, k) float64 with unit column stride and k
+        at least every problem's association count.  n1, n2, m: B sizes (default: the padded dimensions; m[p] = 0: all-to-
+        all for problem p); nothing past them is read.  Returns one api.Solution per problem as solve_many fills it,
+        except that .u and .u0 are device tensor views.  Runs on the batch's stream (set_stream); without a stream of the
+        caller's, torch's current stream is synchronised first."""
+        import torch
+        d, nb, pts, ms, keep = _dev_points(self._device, D1, D2, A, n1, n2, m)  # keep: the host size arrays of pts
+        inv = self._invariant
+        if isinstance(inv, PointNormalDistance) and d != 6:
+            raise ValueError("PointNormalDistance expects 6 x n data")
+        if not isinstance(u0, torch.Tensor) or u0.dtype != torch.float64:
+            raise TypeError("u0 must be a float64 torch tensor")
+        if u0.dim() != 2 or u0.shape[0] != nb or u0.shape[1] < max(ms) or u0.stride(1) != 1:
+            raise ValueError("u0 must be (B, k) with unit column stride and k >= every problem's association count (%d), "
+                             "got shape %s" % (max(ms), tuple(u0.shape)))
+        _on_device(self._device, (u0,))
+        self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
+        _wait_for_torch(self._stream, D1.device)
+        u = torch.empty((nb, max(ms)), dtype=torch.float64, device=D1.device)
+        nodes = [np.zeros(mk, np.int32) for mk in ms]
+        np_ = (C.c_void_p * nb)(*[nk.ctypes.data for nk in nodes])
+        sols = (_capi.ClpSolution * nb)()
+        io = (u0.data_ptr(), u0.stride(0))
+        out = (sols, u.data_ptr(), u.stride(0), np_)
+        if isinstance(inv, CudaInvariant):
+            src, prm, nprm = _custom_args(inv)
+            rc = self._lib.clp_batch_solve_custom_dev(self._b, src, prm, nprm, nb, d, C.byref(pts), *io, *out)
+        elif isinstance(inv, EuclideanDistance):
+            q = inv.params()
+            rc = self._lib.clp_batch_solve_euclidean_dev(self._b, nb, d, C.byref(pts), *io, float(q.sigma),
+                                                         float(q.epsilon), float(q.mindist), *out)
+        else:
+            q = inv.params()
+            rc = self._lib.clp_batch_solve_pointnormal_dev(self._b, nb, C.byref(pts), *io, float(q.sigp), float(q.epsp),
+                                                           float(q.sign), float(q.epsn), *out)
+        self._check(rc)
+        return _solutions(sols, nb, [u0[k, :ms[k]] for k in range(nb)], [u[k, :ms[k]] for k in range(nb)], nodes)
+
+    def max_clique_many_dev(self, D1, D2, A, n1=None, n2=None, m=None, params=None):
+        """max_clique_many for problems already on the batch's device (clp_batch_max_clique_*_dev): D1, D2, A, n1, n2
+        and m as solve_many_dev takes them.  Returns what max_clique_many returns."""
+        d, nb, pts, ms, keep = _dev_points(self._device, D1, D2, A, n1, n2, m)  # keep: the host size arrays of pts
+        inv = self._invariant
+        if isinstance(inv, PointNormalDistance) and d != 6:
+            raise ValueError("PointNormalDistance expects 6 x n data")
+        params = params if params is not None else MCParams()
+        self._check(self._lib.clp_batch_set_params(self._b, C.byref(self._params._pod())))
+        _wait_for_torch(self._stream, D1.device)
+        out, args = _mc_outputs(ms, params)
+        if isinstance(inv, CudaInvariant):
+            src, prm, nprm = _custom_args(inv)
+            rc = self._lib.clp_batch_max_clique_custom_dev(self._b, src, prm, nprm, nb, d, C.byref(pts), *args)
+        elif isinstance(inv, EuclideanDistance):
+            q = inv.params()
+            rc = self._lib.clp_batch_max_clique_euclidean_dev(self._b, nb, d, C.byref(pts), float(q.sigma),
+                                                              float(q.epsilon), float(q.mindist), *args)
+        else:
+            q = inv.params()
+            rc = self._lib.clp_batch_max_clique_pointnormal_dev(self._b, nb, C.byref(pts), float(q.sigp), float(q.epsp),
+                                                                float(q.sign), float(q.epsn), *args)
+        self._check(rc)
+        return out()
+
+
+def _on_device(device, tensors):
+    """ValueError unless every tensor is a CUDA tensor on the batch's device"""
+    for X in tensors:
+        if not X.is_cuda:
+            raise ValueError("expected a CUDA tensor, got one on %s" % X.device)
+        if X.device.index != device:
+            raise ValueError("the tensor is on %s, the batch on cuda:%d" % (X.device, device))
+
+
+def _dev_points(device, D1, D2, A, n1, n2, m):
+    """the point clouds and associations of a batch on the device as clp_points_dev describes them: D1 (B, d, n1_max)
+    and D2 (B, d, n2_max) float64, A (B, m_max, 2) int32 or None, all CUDA tensors on the device; n1, n2, m: B sizes or
+    None for the padded dimensions (A None: m = 0 everywhere, the all-to-all hypothesis).  Returns (d, B, the
+    ClpPointsDev, every problem's association count, the host size arrays it points into).  TypeError / ValueError
+    before the library or a device is touched."""
+    import torch
+    tensors = (("D1", D1), ("D2", D2)) + ((("A", A),) if A is not None else ())
+    for name, X in tensors:
+        if not isinstance(X, torch.Tensor):
+            raise TypeError("%s must be a torch tensor, got %s" % (name, type(X).__name__))
+    if D1.dtype != torch.float64 or D2.dtype != torch.float64:
+        raise TypeError("D1 and D2 must be float64 (points are fp64 only), got %s and %s" % (D1.dtype, D2.dtype))
+    if A is not None and A.dtype != torch.int32:
+        raise TypeError("A must be int32, got %s" % A.dtype)
+    if D1.dim() != 3 or D2.dim() != 3 or D1.shape[:2] != D2.shape[:2] or D1.shape[0] == 0:
+        raise ValueError("D1 and D2 must be (B, d, n1_max) and (B, d, n2_max) with B >= 1, got %s and %s"
+                         % (tuple(D1.shape), tuple(D2.shape)))
+    nb, d = int(D1.shape[0]), int(D1.shape[1])
+    if A is not None and (A.dim() != 3 or A.shape[0] != nb or A.shape[2] != 2):
+        raise ValueError("A must be (B, m_max, 2), got %s" % (tuple(A.shape),))
+
+    def sizes(x, pad, name, lo):
+        v = [int(pad)] * nb if x is None else [int(k) for k in x]
+        if len(v) != nb or any(k < lo or k > pad for k in v):
+            raise ValueError("%s must hold B sizes in [%d, %d]" % (name, lo, pad))
+        return v
+
+    s1, s2 = sizes(n1, D1.shape[2], "n1", 1), sizes(n2, D2.shape[2], "n2", 1)
+    if A is None:
+        if m is not None and any(int(k) != 0 for k in m):
+            raise ValueError("m needs A: without A every problem takes the all-to-all hypothesis")
+        sm = [0] * nb
+    else:
+        sm = sizes(m, A.shape[1], "m", 0)
+    _on_device(device, [X for _, X in tensors])
+    keep = tuple((C.c_int64 * nb)(*v) for v in (s1, s2, sm))
+    pts = _capi.ClpPointsDev(D1.data_ptr(), tuple(D1.stride()), D2.data_ptr(), tuple(D2.stride()),
+                             A.data_ptr() if A is not None else None, tuple(A.stride()) if A is not None else (0, 0, 0),
+                             *keep)
+    ms = [k if k else a * b for k, a, b in zip(sm, s1, s2)]
+    return d, nb, pts, ms, keep
 
 
 def _custom_args(inv):
@@ -268,11 +396,7 @@ class MatrixBatchCLIPPER:
         self._check(self._lib.clp_batch_solve_matrices(self._b, n, m, *ptrs, u0p, sols, up, np_))
         return _solutions(sols, n, u0s, us, nodes)
 
-    def set_stream(self, cuda_stream):
-        """run on an existing CUDA stream (an int handle, e.g. torch.cuda.current_stream().cuda_stream); None or 0: the
-        batch's own stream"""
-        self._check(self._lib.clp_batch_set_stream(self._b, C.c_void_p(cuda_stream or None)))
-        self._stream = cuda_stream or None
+    set_stream = BatchCLIPPER.set_stream
 
     def solve_dense_dev(self, M, C_, u0, m=None):
         """Problems given as CUDA tensors on the batch's device (clp_batch_solve_dense_dev): M and C (B, m_max, m_max),

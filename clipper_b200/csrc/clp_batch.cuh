@@ -482,4 +482,62 @@ __global__ void __launch_bounds__(kBatchThreads, 3) batch_stored_solve_kernel(Ba
                     ba.u_out, ba.out, ba.sb, ba.spin_limit, ba.prof, t_begin, t_scored, sa);
 }
 
+// ---- point clouds and associations already on the device (clp_batch_*_dev) ------------------------------------------
+// batch_stage_points_kernel copies problem p from the caller's strided tensors into the batch's concatenated arrays, at
+// the offsets of its BatchProblem and in the layout the host path uploads: D1 and D2 column-major d x n (the d
+// coordinates of a point together), A column-major m x 2 and, for the solves, u0 at u_off.  Nothing past n1, n2 or m
+// is read.  Association indices are copied as given: the gathers clamp a bad one and set error 2.  The lowest problem
+// with an index out of range is kept in *bad as (kBatchBadIndex << 32 | ~p), the largest key winning, the key
+// batch_dense_solve_kernel uses for its bad values.
+constexpr unsigned long long kBatchBadIndex = 3;
+
+struct BatchStageArgs {
+  const unsigned char* prob; size_t prob_stride;  // BatchProblem of problem p at prob + p * prob_stride
+  int nprob, dd;
+  const double* D1; long long s1[3];              // coordinate k of point j of problem p: D1[p s1[0] + k s1[1] + j s1[2]]
+  const double* D2; long long s2[3];
+  const int* A; long long sa[3];                  // A(i, c): A[p sa[0] + i sa[1] + c sa[2]]
+  const double* u0_in; long long u0_stride;       // nullable: u0 of problem p at u0_in + p u0_stride
+  double* d1; double* d2; int* a; double* u0;
+  unsigned long long* bad;
+};
+
+__global__ void __launch_bounds__(kBatchThreads) batch_stage_points_kernel(BatchStageArgs g) {
+  const long long t0 = (long long)blockIdx.x * kBatchThreads + threadIdx.x, step = (long long)gridDim.x * kBatchThreads;
+  const int dd = g.dd;
+  for (int p = blockIdx.y; p < g.nprob; p += gridDim.y) {
+    const BatchProblem P = *reinterpret_cast<const BatchProblem*>(g.prob + (size_t)p * g.prob_stride);
+    for (long long t = t0; t < (long long)dd * P.n1; t += step) {
+      const long long j = t / dd, k = t - j * dd;
+      g.d1[P.d1_off + t] = g.D1[p * g.s1[0] + k * g.s1[1] + j * g.s1[2]];
+    }
+    for (long long t = t0; t < (long long)dd * P.n2; t += step) {
+      const long long j = t / dd, k = t - j * dd;
+      g.d2[P.d2_off + t] = g.D2[p * g.s2[0] + k * g.s2[1] + j * g.s2[2]];
+    }
+    int bad = 0;
+    if (P.a_off >= 0)
+      for (long long t = t0; t < 2LL * P.m; t += step) {
+        const int c = t < P.m ? 0 : 1;
+        const long long i = t - (long long)c * P.m;
+        const int x = g.A[p * g.sa[0] + i * g.sa[1] + c * g.sa[2]];
+        g.a[P.a_off + t] = x;
+        if (x < 0 || x >= (c ? P.n2 : P.n1)) bad = 1;
+      }
+    if (g.u0_in)
+      for (long long t = t0; t < P.m; t += step) g.u0[P.u_off + t] = g.u0_in[p * g.u0_stride + t];
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicMax(g.bad, (kBatchBadIndex << 32) | (0xffffffffu - (unsigned int)p));
+  }
+}
+
+// u of problem p from the batch's concatenated output (at u_off) to u_out + p * stride, m entries
+__global__ void __launch_bounds__(kBatchThreads) batch_copy_u_kernel(const BatchProblem* prob, int nprob, const double* u,
+                                                                     double* u_out, long long stride) {
+  for (int p = blockIdx.y; p < nprob; p += gridDim.y) {
+    const BatchProblem P = prob[p];
+    for (int i = blockIdx.x * kBatchThreads + threadIdx.x; i < P.m; i += gridDim.x * kBatchThreads)
+      u_out[p * stride + i] = u[P.u_off + i];
+  }
+}
+
 }  // namespace clp

@@ -1962,6 +1962,8 @@ void batch_results(const clp_params& P, const std::vector<Prob>& probs, const do
 
 // Inputs of the batch C-ABI calls.  Scored problems: D1, n1, D2, n2, A, m and the invariant's parameters p, or for
 // clp_batch_*_custom the caller's invariant inv; graphs given as strictly-upper CSC patterns: m, colptr and rowidx.
+// clp_batch_*_dev: the points and associations are in dev (n1, n2 and m are its host arrays), and the solves take u0
+// from u0_dev and write u to u_out_dev (nullable).
 struct BatchInput {
   const double* const* D1 = nullptr; const int64_t* n1 = nullptr;
   const double* const* D2 = nullptr; const int64_t* n2 = nullptr;
@@ -1969,7 +1971,25 @@ struct BatchInput {
   const int64_t* const* colptr = nullptr; const int32_t* const* rowidx = nullptr;
   double p[4] = {0.0, 0.0, 0.0, 0.0};
   const CustomInvariant* inv = nullptr;
+  const clp_points_dev* dev = nullptr;
+  const double* u0_dev = nullptr; int64_t u0_stride = 0;
+  double* u_out_dev = nullptr; int64_t u_out_stride = 0;
 };
+
+// problem p of a scored batch takes the all-to-all hypothesis: no associations are given for it
+bool all_to_all(const BatchInput& in, int p) {
+  return (in.dev ? in.dev->A == nullptr : (in.A == nullptr || in.A[p] == nullptr)) || in.m[p] == 0;
+}
+
+// the checks of problem p of a scored batch (CLP_ERR_INVALID): its data and its association count *mp (n1 n2 for the
+// all-to-all hypothesis)
+int point_problem_check(clp_batch b, const BatchInput& in, int p, long long* mp) {
+  if ((!in.dev && (!in.D1[p] || !in.D2[p])) || in.n1[p] <= 0 || in.n2[p] <= 0)
+    return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
+  *mp = all_to_all(in, p) ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
+  if (*mp <= 0 || *mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
+  return CLP_OK;
+}
 
 // the `kind` of batch_solve and batch_max_clique for problems scored with a caller's invariant (clp_batch_*_custom):
 // the clique's prepare kernel reads the stored matrix (0, 1: the built-ins, kMcbKindGraph: graphs)
@@ -1982,17 +2002,15 @@ constexpr int kBatchKindCustom = kMcbKindStored;
 // per problem of the round.  Every round is enqueued on the batch's stream; the results are read once at the end.
 
 // the checks of a custom batch that come before everything else (CLP_ERR_INVALID): the source, the parameter count,
-// the dimension and every problem's m (stage_points repeats the last)
+// the dimension and every problem's m (plan_points repeats the last)
 int custom_check(clp_batch b, const CustomInvariant& inv, int32_t nprob, int dd, const BatchInput& in) {
   if (!inv.source || !*inv.source) return fail(b, CLP_ERR_INVALID, "empty invariant source");
   if (inv.nprm < 0 || inv.nprm > CLP_INV_MAX_PARAMS || (inv.nprm > 0 && !inv.prm))
     return fail(b, CLP_ERR_INVALID, "invariant parameters: 0 to " + std::to_string(CLP_INV_MAX_PARAMS) + " doubles");
   if (dd < 1) return fail(b, CLP_ERR_INVALID, "dimension must be positive");
   for (int p = 0; p < nprob; ++p) {
-    if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
-    const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
-    const long long mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
-    if (mp <= 0 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
+    long long mp = 0;
+    if (int rc = point_problem_check(b, in, p, &mp)) return rc;
   }
   return CLP_OK;
 }
@@ -2055,19 +2073,25 @@ int custom_score_round(clp_batch b, CustomRounds& cr, int first, int count) {
   return CLP_OK;
 }
 
-// Point clouds of a scored batch: checks every problem (association indices included), fills its BatchProblem (offsets
-// of D1, D2 and A; m = n1 n2 where A, A[p] or m[p] is empty: the all-to-all hypothesis; u_off 0) and uploads D1, D2
-// and A to in_d1, in_d2 and in_a through pinned_points.  *bytes: the bytes uploaded.
-int stage_points(clp_batch b, int dd, int32_t nprob, const BatchInput& in, std::vector<BatchProblem>& probs, size_t* bytes) {
-  probs.assign((size_t)nprob, BatchProblem{});
+// The concatenated point inputs of a scored batch (in_d1, in_d2, in_a), decided once for both fills: one BatchProblem
+// per problem with the offsets of its D1, D2 and A (a_off -1 and m = n1 n2 for the all-to-all hypothesis; u_off 0),
+// and the element counts of the three arrays.
+struct PointsPlan {
+  std::vector<BatchProblem> probs;
+  long long nd1 = 0, nd2 = 0, na = 0;
+};
+
+// checks every problem, host association indices included (device ones are checked by batch_stage_points_kernel),
+// fills the plan and sizes in_d1, in_d2 and in_a
+int plan_points(clp_batch b, int dd, int32_t nprob, const BatchInput& in, PointsPlan* pl) {
+  pl->probs.assign((size_t)nprob, BatchProblem{});
   long long nd1 = 0, nd2 = 0, na = 0;
   for (int p = 0; p < nprob; ++p) {
-    BatchProblem& q = probs[(size_t)p];
-    if (!in.D1[p] || !in.D2[p] || in.n1[p] <= 0 || in.n2[p] <= 0) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null data)");
-    const bool a2a = (in.A == nullptr || in.A[p] == nullptr || in.m[p] == 0);
-    const long long mp = a2a ? (long long)in.n1[p] * in.n2[p] : (long long)in.m[p];
-    if (mp <= 0 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, "batched problems need 1 <= m <= 4096 associations");
-    if (!a2a)
+    BatchProblem& q = pl->probs[(size_t)p];
+    long long mp = 0;
+    if (int rc = point_problem_check(b, in, p, &mp)) return rc;
+    const bool a2a = all_to_all(in, p);
+    if (!a2a && !in.dev)
       for (long long i = 0; i < mp; ++i) {
         const int32_t a0 = in.A[p][i], a1 = in.A[p][mp + i];
         if (a0 < 0 || a0 >= in.n1[p] || a1 < 0 || a1 >= in.n2[p])
@@ -2077,24 +2101,66 @@ int stage_points(clp_batch b, int dd, int32_t nprob, const BatchInput& in, std::
     q.n1 = (int)in.n1[p]; q.n2 = (int)in.n2[p]; q.m = (int)mp;
     nd1 += (long long)dd * in.n1[p]; nd2 += (long long)dd * in.n2[p]; if (!a2a) na += 2 * mp;
   }
+  pl->nd1 = nd1; pl->nd2 = nd2; pl->na = na;
+  CLP_CUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
+  CLP_CUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
+  CLP_CUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
+  return CLP_OK;
+}
+
+// Fills the planned arrays, enqueued on the batch's stream: host inputs through pinned_points and three uploads;
+// device inputs (in.dev) with batch_stage_points_kernel, which reads the problem table at `table` (device, one entry
+// every table_stride bytes, u_off set) and also stages u0 into in_u0 when in.u0_dev is given.  *bytes: the bytes
+// uploaded.
+int fill_points(clp_batch b, int dd, const BatchInput& in, const PointsPlan& pl, const void* table, size_t table_stride,
+                size_t* bytes) {
+  const int nprob = (int)pl.probs.size();
+  if (in.dev) {
+    const clp_points_dev& s = *in.dev;
+    BatchStageArgs g;
+    std::memset(&g, 0, sizeof(g));
+    g.prob = static_cast<const unsigned char*>(table); g.prob_stride = table_stride;
+    g.nprob = nprob; g.dd = dd;
+    g.D1 = s.D1; g.D2 = s.D2; g.A = s.A;
+    for (int k = 0; k < 3; ++k) { g.s1[k] = s.d1_strides[k]; g.s2[k] = s.d2_strides[k]; g.sa[k] = s.a_strides[k]; }
+    g.u0_in = in.u0_dev; g.u0_stride = in.u0_stride;
+    g.d1 = b->in_d1.as<double>(); g.d2 = b->in_d2.as<double>(); g.a = b->in_a.as<int>(); g.u0 = b->in_u0.as<double>();
+    g.bad = &b->sync.as<SyncBlock>()->counts[1];
+    long long most = 1;
+    for (const BatchProblem& q : pl.probs) most = std::max({most, (long long)dd * std::max(q.n1, q.n2), 2LL * q.m});
+    const dim3 grid((unsigned)std::min<long long>(64, (most + kBatchThreads - 1) / kBatchThreads), (unsigned)std::min(nprob, 65535));
+    batch_stage_points_kernel<<<grid, kBatchThreads, 0, b->stream>>>(g);
+    CLP_CUDA(b, cudaGetLastError());
+    *bytes = 0;
+    return CLP_OK;
+  }
+  const long long nd1 = pl.nd1, nd2 = pl.nd2, na = pl.na;
   *bytes = (size_t)(nd1 + nd2) * 8 + (size_t)na * 4;
   CLP_CUDA(b, b->pinned_points.ensure(*bytes + 16));
   double* h_d1 = b->pinned_points.as<double>();
   double* h_d2 = h_d1 + nd1;
   int32_t* h_a = reinterpret_cast<int32_t*>(h_d2 + nd2);
   for (int p = 0; p < nprob; ++p) {
-    const BatchProblem& q = probs[(size_t)p];
+    const BatchProblem& q = pl.probs[(size_t)p];
     std::memcpy(h_d1 + q.d1_off, in.D1[p], (size_t)dd * q.n1 * 8);
     std::memcpy(h_d2 + q.d2_off, in.D2[p], (size_t)dd * q.n2 * 8);
     if (q.a_off >= 0) std::memcpy(h_a + q.a_off, in.A[p], (size_t)2 * q.m * 4);
   }
-  CLP_CUDA(b, b->in_d1.ensure((size_t)nd1 * 8 + 16));
-  CLP_CUDA(b, b->in_d2.ensure((size_t)nd2 * 8 + 16));
-  CLP_CUDA(b, b->in_a.ensure((size_t)na * 4 + 16));
   CLP_CUDA(b, cudaMemcpyAsync(b->in_d1.p, h_d1, (size_t)nd1 * 8, cudaMemcpyHostToDevice, b->stream));
   CLP_CUDA(b, cudaMemcpyAsync(b->in_d2.p, h_d2, (size_t)nd2 * 8, cudaMemcpyHostToDevice, b->stream));
   if (na) CLP_CUDA(b, cudaMemcpyAsync(b->in_a.p, h_a, (size_t)na * 4, cudaMemcpyHostToDevice, b->stream));
   return CLP_OK;
+}
+
+// the error of a problem a device check found bad: SyncBlock::counts[1] holds (kind << 32 | ~p) of the lowest such
+// problem p (0: none).  Kinds 1 and 2: a C or M value (batch_dense_solve_kernel); kBatchBadIndex: an association index
+// (batch_stage_points_kernel).
+int bad_problem(clp_batch b, unsigned long long key) {
+  if (key == 0) return CLP_OK;
+  const unsigned long long kind = key >> 32;
+  const std::string p = "problem " + std::to_string(0xffffffffu - (unsigned int)(key & 0xffffffffu));
+  if (kind == kBatchBadIndex) return fail(b, CLP_ERR_INVALID, p + ": association index out of range of D1/D2");
+  return fail(b, CLP_ERR_UNSUPPORTED, p + (kind == 2 ? ", M: affinity matrix has negative entries" : ", C: constraint matrix is not binary"));
 }
 
 // CTAs of a persistent batch launch, each with a scratch slot of `stride` bytes in `scratch` (stride 0: none): as many
@@ -2119,7 +2185,8 @@ int batch_grid(clp_batch b, int occ, int32_t nprob, size_t stride, DevBuf& scrat
 // problem and the sync block into the staging buffer with one synchronisation, prints the CLP_PROF_BATCH line, maps the
 // device's error words (batch_matrix_solve_kernel sets flags, batch_solve_kernel error 2, both time out with error 1),
 // and fills the results.  `label` names the call and `first` its first in-kernel phase in the profile line.
-// batch_dense_solve_kernel leaves its first bad problem in counts[1] (BatchDenseArgs::bad); it is reported first.
+// batch_dense_solve_kernel and batch_stage_points_kernel leave their first bad problem in counts[1] (bad_problem); it is
+// reported first.
 template <typename Prob>
 int batch_finish(clp_batch b, const char* label, const char* first, const std::vector<Prob>& probs, long long nu, int max_m,
                  int grid, size_t stride, size_t bytes_in, std::chrono::steady_clock::time_point t_begin, clp_solution* sols,
@@ -2147,12 +2214,7 @@ int batch_finish(clp_batch b, const char* label, const char* first, const std::v
                  "mean per problem: %s %.3f  build %.3f  solve %.3f  total %.3f ms\n",
                  label, nprob, max_m, grid, bytes_in, up_ms, ms, first, acc[0] / nprob, acc[1] / nprob, acc[2] / nprob, acc[3] / nprob);
   }
-  if (h_sb.counts[1] != 0) {
-    const bool neg = (h_sb.counts[1] >> 32) == 2;
-    const unsigned int p = 0xffffffffu - (unsigned int)(h_sb.counts[1] & 0xffffffffu);
-    return fail(b, CLP_ERR_UNSUPPORTED, "problem " + std::to_string(p) +
-                                            (neg ? ", M: affinity matrix has negative entries" : ", C: constraint matrix is not binary"));
-  }
+  if (int rc = bad_problem(b, h_sb.counts[1])) return rc;
   if (h_sb.flags != 0) return fail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
   if (h_sb.error == 2) return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
   if (h_sb.error != 0) return fail(b, CLP_ERR_TIMEOUT, "batch kernel: an in-kernel wait timed out");
@@ -2167,10 +2229,11 @@ int batch_finish(clp_batch b, const char* label, const char* first, const std::v
 int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& in, const double* const* u0, clp_solution* sols,
                 double* const* u_out, int32_t* const* nodes_out) {
   if (!b) return CLP_ERR_INVALID;
-  if (nprob <= 0 || !in.D1 || !in.n1 || !in.D2 || !in.n2 || !in.m || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (nprob <= 0 || (!in.dev && (!in.D1 || !in.D2 || !u0)) || !in.n1 || !in.n2 || !in.m || (in.dev && !in.u0_dev) || !sols)
+    return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   const bool custom = kind == kBatchKindCustom;
   if (custom) {
-    for (int p = 0; p < nprob; ++p)
+    for (int p = 0; p < nprob && !in.dev; ++p)
       if (!u0[p]) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null u0)");
     if (int rc = custom_check(b, *in.inv, nprob, dd, in)) return rc;
   } else if (!((kind == 0 && (dd == 2 || dd == 3)) || (kind == 1 && dd == 6))) {
@@ -2185,12 +2248,12 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
   if (custom)
     if (int rc = custom_compile(b, *in.inv, dd, &cr)) return rc;
   // ---- problem table and concatenated inputs
-  for (int p = 0; p < nprob; ++p)
+  for (int p = 0; p < nprob && !in.dev; ++p)
     if (!u0[p]) return fail(b, CLP_ERR_INVALID, "bad problem in the batch (null u0)");
   CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
-  std::vector<BatchProblem> probs;
-  size_t bytes_in = 0;
-  if (int rc = stage_points(b, dd, nprob, in, probs, &bytes_in)) return rc;
+  PointsPlan pl;
+  if (int rc = plan_points(b, dd, nprob, in, &pl)) return rc;
+  std::vector<BatchProblem>& probs = pl.probs;
   long long nu = 0;
   int max_m = 1;
   for (BatchProblem& q : probs) {
@@ -2198,24 +2261,28 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
     nu += (q.m + 1) & ~1LL;  // every problem's u0 / u slot starts on a 16-byte boundary (the kernels use 16-byte loads)
     max_m = std::max(max_m, q.m);
   }
-  const size_t bytes_table = (size_t)nu * 8 + (size_t)nprob * sizeof(BatchProblem);
+  // host u0 goes up with the table; device u0 is staged with the points
+  const long long nu0 = in.dev ? 0 : nu;
+  const size_t bytes_table = (size_t)nu0 * 8 + (size_t)nprob * sizeof(BatchProblem);
   const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
-  bytes_in += bytes_table;
   CLP_CUDA(b, b->pinned.ensure(std::max(bytes_table, bytes_out) + 4096));
   double* h_u0 = b->pinned.as<double>();
-  BatchProblem* h_pr = reinterpret_cast<BatchProblem*>(h_u0 + nu);
-  for (int p = 0; p < nprob; ++p) std::memcpy(h_u0 + probs[(size_t)p].u_off, u0[p], (size_t)probs[(size_t)p].m * 8);
+  BatchProblem* h_pr = reinterpret_cast<BatchProblem*>(h_u0 + nu0);
+  for (int p = 0; p < nprob && !in.dev; ++p) std::memcpy(h_u0 + probs[(size_t)p].u_off, u0[p], (size_t)probs[(size_t)p].m * 8);
   std::memcpy(h_pr, probs.data(), (size_t)nprob * sizeof(BatchProblem));
   CLP_CUDA(b, b->in_u0.ensure((size_t)nu * 8 + 16));
   CLP_CUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
   CLP_CUDA(b, b->probs.ensure((size_t)nprob * sizeof(BatchProblem)));
   CLP_CUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
   CLP_CUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
-  CLP_CUDA(b, cudaMemcpyAsync(b->in_u0.p, h_u0, (size_t)nu * 8, cudaMemcpyHostToDevice, b->stream));
+  if (nu0) CLP_CUDA(b, cudaMemcpyAsync(b->in_u0.p, h_u0, (size_t)nu0 * 8, cudaMemcpyHostToDevice, b->stream));
   CLP_CUDA(b, cudaMemcpyAsync(b->probs.p, h_pr, (size_t)nprob * sizeof(BatchProblem), cudaMemcpyHostToDevice, b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  size_t bytes_in = 0;
+  if (int rc = fill_points(b, dd, in, pl, b->probs.p, sizeof(BatchProblem), &bytes_in)) return rc;
+  bytes_in += bytes_table;
   // ---- grid: as many CTAs as are co-resident (and as there are problems), each with its own scratch slot
   const BatchSmem bs = batch_smem_plan(max_m);
   if ((long long)bs.total > (long long)b->smem_optin) return fail(b, CLP_ERR_UNSUPPORTED, "batch: shared memory plan exceeds the device limit");
@@ -2245,6 +2312,15 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
   ba.p0 = in.p[0]; ba.p1 = in.p[1]; ba.p2 = in.p[2]; ba.p3 = in.p[3]; ba.affinityeps = P.affinityeps;
   ba.sb = b->sync.as<SyncBlock>(); ba.spin_limit = 4LL * 1900000000LL;
   if (b->prof_on) { CLP_CUDA(b, b->prof.ensure((size_t)nprob * 4 * sizeof(unsigned long long))); ba.prof = b->prof.as<unsigned long long>(); }
+  // after the launches: device u out (clp_batch_solve_*_dev), then the common tail
+  auto finish = [&](const char* label, const char* first) -> int {
+    if (in.u_out_dev) {
+      const dim3 g((unsigned)((max_m + kBatchThreads - 1) / kBatchThreads), (unsigned)std::min(nprob, 65535));
+      batch_copy_u_kernel<<<g, kBatchThreads, 0, b->stream>>>(ba.prob, nprob, ba.u_out, in.u_out_dev, in.u_out_stride);
+      CLP_CUDA(b, cudaGetLastError());
+    }
+    return batch_finish(b, label, first, probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+  };
   if (custom) {
     if ((rc = custom_stage(b, *in.inv, dd, probs, ba.scratch, L.total, L.E1, L.E2, L.A, L.M, &cr))) return rc;
     CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
@@ -2254,12 +2330,12 @@ int batch_solve(clp_batch b, int kind, int dd, int32_t nprob, const BatchInput& 
       batch_stored_solve_kernel<<<count, kBatchThreads, bs.total, b->stream>>>(ba, first);
       CLP_CUDA(b, cudaGetLastError());
     }
-    return batch_finish(b, "batch custom", "count", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+    return finish("batch custom", "count");
   }
   CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   rc = (kind == 1) ? batch_launch<1, 6>(b, ba, grid, bs.total) : (dd == 3 ? batch_launch<0, 3>(b, ba, grid, bs.total) : batch_launch<0, 2>(b, ba, grid, bs.total));
   if (rc) return rc;
-  return batch_finish(b, "batch", "score", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+  return finish("batch", "score");
 }
 
 // ---- batched solve of given matrices (clp_batch_matrix.cuh) -------------------------------------------------------
@@ -2520,7 +2596,7 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   if (nprob <= 0 || !infos || !in.m) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   if (method < CLP_MC_EXACT || method > CLP_MC_KCORE) return fail(b, CLP_ERR_INVALID, "unknown maximum-clique method");
   const bool graph = kind == kMcbKindGraph, custom = kind == kBatchKindCustom;
-  if (graph ? (!in.colptr || !in.rowidx) : (!in.D1 || !in.n1 || !in.D2 || !in.n2))
+  if (graph ? (!in.colptr || !in.rowidx) : ((!in.dev && (!in.D1 || !in.D2)) || !in.n1 || !in.n2))
     return fail(b, CLP_ERR_INVALID, "bad batch arguments");
   if (custom) {
     if (int rc = custom_check(b, *in.inv, nprob, dd, in)) return rc;
@@ -2532,12 +2608,13 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   CustomRounds cr;
   if (custom)
     if (int rc = custom_compile(b, *in.inv, dd, &cr)) return rc;
-  // ---- problem table and per-problem regions; scored inputs are checked and uploaded by stage_points, graphs here
+  // ---- problem table and per-problem regions; scored inputs are checked by plan_points and staged by fill_points
+  // once the table is on the device, graphs are checked here
   std::vector<McBatchProblem> probs((size_t)nprob);
-  std::vector<BatchProblem> pts;
+  PointsPlan pl;
+  const std::vector<BatchProblem>& pts = pl.probs;
   if (!graph) {
-    size_t bytes_pts = 0;
-    if (int rc = stage_points(b, dd, nprob, in, pts, &bytes_pts)) return rc;
+    if (int rc = plan_points(b, dd, nprob, in, &pl)) return rc;
     for (int p = 0; p < nprob; ++p) probs[(size_t)p].sp = pts[(size_t)p];
   }
   long long ne = 0, nadj = 0, nv = 0, nt = 0;
@@ -2595,6 +2672,11 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   if (graph) CLP_CUDA(b, cudaMemsetAsync(b->mc_adj.p, 0, (size_t)nadj * 4, b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->mc_out.p, 0, (size_t)nprob * sizeof(McBatchOut), b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  if (!graph) {
+    size_t bytes_pts = 0;
+    const void* table = b->mc_probs.as<unsigned char>() + offsetof(McBatchProblem, sp);
+    if (int rc = fill_points(b, dd, in, pl, table, sizeof(McBatchProblem), &bytes_pts)) return rc;
+  }
 
   // ---- phase A: one CTA per problem, as many CTAs as are co-resident and, for scored problems, fit their scratch
   const McbSmem sm = mcb_smem_plan(max_m);
@@ -2646,6 +2728,7 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   CLP_CUDA(b, cudaMemcpyAsync(outs.data(), b->mc_out.p, (size_t)nprob * sizeof(McBatchOut), cudaMemcpyDeviceToHost, b->stream));
   CLP_CUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
   CLP_CUDA(b, cudaStreamSynchronize(b->stream));
+  if (int rc = bad_problem(b, h_sb.counts[1])) return rc;
   if (h_sb.error == 2) return fail(b, CLP_ERR_INVALID, "association index out of range of D1/D2 in a batched problem");
   b->last_ctas = grid;
   b->last_scratch = (long long)grid * (long long)pstride;
@@ -2791,6 +2874,42 @@ int batch_max_clique(clp_batch b, int kind, int dd, int32_t nprob, const BatchIn
   }
   const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
   for (int p = 0; p < nprob; ++p) infos[p].t = wall / nprob;
+  return CLP_OK;
+}
+
+// ---- points and associations on the device (clp_batch_*_dev) -----------------------------------------------------
+// The checks these calls make before those of their host twins (CLP_ERR_INVALID): pointers, strides and sizes of pts,
+// every problem's association count (*max_m: the largest).  Then in is set up for batch_solve / batch_max_clique.
+int points_dev_check(clp_batch b, int32_t nprob, const clp_points_dev* pts, BatchInput& in, long long* max_m) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !pts || !pts->D1 || !pts->D2 || !pts->n1 || !pts->n2 || !pts->m) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  auto strides_ok = [](const int64_t* s) { return s[0] >= 0 && s[1] >= 1 && s[2] >= 1; };
+  if (!strides_ok(pts->d1_strides) || !strides_ok(pts->d2_strides) || (pts->A && !strides_ok(pts->a_strides)))
+    return fail(b, CLP_ERR_INVALID, "bad strides (coordinate, point, row and column strides must be >= 1, batch strides >= 0)");
+  *max_m = 1;
+  for (int p = 0; p < nprob; ++p) {
+    const std::string tag = "problem " + std::to_string(p) + ": ";
+    const int64_t n1 = pts->n1[p], n2 = pts->n2[p], m = pts->m[p];
+    if (n1 < 1 || n2 < 1 || n1 > INT32_MAX || n2 > INT32_MAX || m < 0)
+      return fail(b, CLP_ERR_INVALID, tag + "bad sizes (n1, n2 >= 1, m >= 0)");
+    const long long mp = (!pts->A || m == 0) ? (long long)n1 * n2 : (long long)m;
+    if (mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, tag + "batched problems need 1 <= m <= 4096 associations");
+    *max_m = std::max(*max_m, mp);
+  }
+  in.dev = pts; in.n1 = pts->n1; in.n2 = pts->n2; in.m = pts->m;
+  return CLP_OK;
+}
+
+// the solves' device u0 and u: u0_dev + p u0_stride (u0_stride >= 1), u_out_dev + p u_out_stride (nullable,
+// u_out_stride >= the largest m)
+int solve_dev_check(clp_batch b, int32_t nprob, const clp_points_dev* pts, const double* u0_dev, int64_t u0_stride,
+                    double* u_out_dev, int64_t u_out_stride, BatchInput& in) {
+  long long max_m = 0;
+  if (int rc = points_dev_check(b, nprob, pts, in, &max_m)) return rc;
+  if (!u0_dev) return fail(b, CLP_ERR_INVALID, "null u0");
+  if (u0_stride < 1 || (u_out_dev && u_out_stride < max_m))
+    return fail(b, CLP_ERR_INVALID, "bad strides (u0_stride >= 1; u_out_stride >= the largest m)");
+  in.u0_dev = u0_dev; in.u0_stride = u0_stride; in.u_out_dev = u_out_dev; in.u_out_stride = u_out_stride;
   return CLP_OK;
 }
 }  // namespace
@@ -2950,6 +3069,77 @@ int clp_batch_max_clique_custom(clp_batch b, const char* source, const double* p
   BatchInput in;
   in.D1 = D1; in.n1 = n1; in.D2 = D2; in.n2 = n2; in.A = A; in.m = m; in.inv = &inv;
   return guarded(b, [&] { return batch_max_clique(b, kBatchKindCustom, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out); });
+}
+
+int clp_batch_solve_euclidean_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts, const double* u0_dev,
+                                  int64_t u0_stride, double sigma, double epsilon, double mindist, clp_solution* sols,
+                                  double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out) {
+  return guarded(b, [&] {
+    BatchInput in;
+    if (int rc = solve_dev_check(b, nprob, pts, u0_dev, u0_stride, u_out_dev, u_out_stride, in)) return rc;
+    in.p[0] = sigma; in.p[1] = epsilon; in.p[2] = mindist;
+    return batch_solve(b, 0, d, nprob, in, nullptr, sols, nullptr, nodes_out);
+  });
+}
+
+int clp_batch_solve_pointnormal_dev(clp_batch b, int32_t nprob, const clp_points_dev* pts, const double* u0_dev,
+                                    int64_t u0_stride, double sigp, double epsp, double sign, double epsn,
+                                    clp_solution* sols, double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out) {
+  return guarded(b, [&] {
+    BatchInput in;
+    if (int rc = solve_dev_check(b, nprob, pts, u0_dev, u0_stride, u_out_dev, u_out_stride, in)) return rc;
+    in.p[0] = sigp; in.p[1] = epsp; in.p[2] = sign; in.p[3] = epsn;
+    return batch_solve(b, 1, 6, nprob, in, nullptr, sols, nullptr, nodes_out);
+  });
+}
+
+int clp_batch_solve_custom_dev(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                               const clp_points_dev* pts, const double* u0_dev, int64_t u0_stride, clp_solution* sols,
+                               double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out) {
+  const CustomInvariant inv{source, prm, nprm};
+  return guarded(b, [&] {
+    BatchInput in;
+    if (int rc = solve_dev_check(b, nprob, pts, u0_dev, u0_stride, u_out_dev, u_out_stride, in)) return rc;
+    in.inv = &inv;
+    return batch_solve(b, kBatchKindCustom, d, nprob, in, nullptr, sols, nullptr, nodes_out);
+  });
+}
+
+int clp_batch_max_clique_euclidean_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts, double sigma,
+                                       double epsilon, double mindist, int method, double time_limit_s,
+                                       clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  return guarded(b, [&] {
+    BatchInput in;
+    long long max_m = 0;
+    if (int rc = points_dev_check(b, nprob, pts, in, &max_m)) return rc;
+    in.p[0] = sigma; in.p[1] = epsilon; in.p[2] = mindist;
+    return batch_max_clique(b, 0, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out);
+  });
+}
+
+int clp_batch_max_clique_pointnormal_dev(clp_batch b, int32_t nprob, const clp_points_dev* pts, double sigp, double epsp,
+                                         double sign, double epsn, int method, double time_limit_s, clp_mc_info* infos,
+                                         int32_t* const* nodes_out, int32_t* const* core_out) {
+  return guarded(b, [&] {
+    BatchInput in;
+    long long max_m = 0;
+    if (int rc = points_dev_check(b, nprob, pts, in, &max_m)) return rc;
+    in.p[0] = sigp; in.p[1] = epsp; in.p[2] = sign; in.p[3] = epsn;
+    return batch_max_clique(b, 1, 6, nprob, in, method, time_limit_s, infos, nodes_out, core_out);
+  });
+}
+
+int clp_batch_max_clique_custom_dev(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob,
+                                    int32_t d, const clp_points_dev* pts, int method, double time_limit_s,
+                                    clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out) {
+  const CustomInvariant inv{source, prm, nprm};
+  return guarded(b, [&] {
+    BatchInput in;
+    long long max_m = 0;
+    if (int rc = points_dev_check(b, nprob, pts, in, &max_m)) return rc;
+    in.inv = &inv;
+    return batch_max_clique(b, kBatchKindCustom, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out);
+  });
 }
 
 }  // extern "C"

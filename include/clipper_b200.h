@@ -395,6 +395,51 @@ int clp_batch_max_clique_custom(clp_batch b, const char* source, const double* p
                                 const int32_t* const* A, const int64_t* m, int method, double time_limit_s,
                                 clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
 
+/* ---- scored batches whose point clouds and associations are already on the batch's device -------------------------
+ * The device twins of clp_batch_solve_* and clp_batch_max_clique_* (custom included), e.g. for torch tensors D1
+ * [nprob, d, n1_max], D2 [nprob, d, n2_max] and A [nprob, m_max, 2].  pts describes them in element units; the sizes
+ * stay on the host:
+ *   coordinate k of point j of problem p: D1[p * d1_strides[0] + k * d1_strides[1] + j * d1_strides[2]] (D2 alike);
+ *   association i of problem p: (A[p * a_strides[0] + i * a_strides[1]], A[p * a_strides[0] + i * a_strides[1] +
+ *   a_strides[2]]); A == NULL: all-to-all for every problem, m[p] == 0: all-to-all for problem p.
+ * Points are fp64 only and associations int32 only.  Coordinate, point, row and column strides must be >= 1; a batch
+ * stride may be 0 (every problem reads the same cloud: a torch expand).  Nothing past n1[p], n2[p] or m[p] is read.
+ * The solves take u0 of problem p as m[p] doubles at u0_dev + p * u0_stride (u0_stride >= 1) and write u to u_out_dev +
+ * p * u_out_stride (device, nullable; u_out_stride >= the largest m); sols, infos, nodes_out and core_out are host
+ * arrays as in the host calls.  Problem p gets exactly, bit for bit, what the host-pointer call gives for the same
+ * values: u, score, d_final, ifinal, n_evals, n_inner and nodes, clp_batch_info's kept-entry count, and for the clique
+ * the cores, bounds, proven flag and nodes.
+ * Errors, in this order: CLP_ERR_INVALID for bad sizes (n1[p], n2[p] >= 1, m[p] >= 0, every problem's association count
+ * in [1, 4096]), NULL pointers or bad strides; then the host calls' checks in their order (the invariant kind and d,
+ * Rounding::DSD for the solves, the method for the clique, the source compile for custom); then, found on the device,
+ * CLP_ERR_INVALID naming the lowest problem with an association index out of range.  After an error the other outputs
+ * are unspecified and the handle stays usable.  Runs on the batch's stream (clp_batch_set_stream) and returns when the
+ * results are host-visible. */
+typedef struct clp_points_dev {
+  const double* D1; int64_t d1_strides[3];
+  const double* D2; int64_t d2_strides[3];
+  const int32_t* A; int64_t a_strides[3];
+  const int64_t* n1; const int64_t* n2; const int64_t* m; /* host arrays of nprob */
+} clp_points_dev;
+int clp_batch_solve_euclidean_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts, const double* u0_dev,
+                                  int64_t u0_stride, double sigma, double epsilon, double mindist, clp_solution* sols,
+                                  double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out);
+int clp_batch_solve_pointnormal_dev(clp_batch b, int32_t nprob, const clp_points_dev* pts, const double* u0_dev,
+                                    int64_t u0_stride, double sigp, double epsp, double sign, double epsn,
+                                    clp_solution* sols, double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out);
+int clp_batch_solve_custom_dev(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob, int32_t d,
+                               const clp_points_dev* pts, const double* u0_dev, int64_t u0_stride, clp_solution* sols,
+                               double* u_out_dev, int64_t u_out_stride, int32_t* const* nodes_out);
+int clp_batch_max_clique_euclidean_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts, double sigma,
+                                       double epsilon, double mindist, int method, double time_limit_s,
+                                       clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
+int clp_batch_max_clique_pointnormal_dev(clp_batch b, int32_t nprob, const clp_points_dev* pts, double sigp, double epsp,
+                                         double sign, double epsn, int method, double time_limit_s, clp_mc_info* infos,
+                                         int32_t* const* nodes_out, int32_t* const* core_out);
+int clp_batch_max_clique_custom_dev(clp_batch b, const char* source, const double* prm, int32_t nprm, int32_t nprob,
+                                    int32_t d, const clp_points_dev* pts, int method, double time_limit_s,
+                                    clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
+
 #ifdef __cplusplus
 }
 #endif
