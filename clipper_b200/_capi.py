@@ -35,9 +35,11 @@ SYMBOLS = [
     "clp_batch_solve_custom", "clp_batch_max_clique_custom",
     "clp_batch_solve_euclidean_dev", "clp_batch_solve_pointnormal_dev", "clp_batch_solve_custom_dev",
     "clp_batch_max_clique_euclidean_dev", "clp_batch_max_clique_pointnormal_dev", "clp_batch_max_clique_custom_dev",
+    "clp_sdp_default_params", "clp_sdp_solve", "clp_batch_sdp_matrices",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
+SDP_MAX_M = 128
 
 
 class ClpParams(C.Structure):
@@ -69,6 +71,21 @@ class ClpMcInfo(C.Structure):
         ("proven", C.c_int32), ("timed_out", C.c_int32), ("n_edges", C.c_int64), ("n_branches", C.c_int64),
         ("t", C.c_double), ("kernel_ms", C.c_double),
         ("adjacency_ms", C.c_double), ("peel_ms", C.c_double), ("heuristic_ms", C.c_double), ("search_ms", C.c_double),
+    ]
+
+
+class ClpSdpParams(C.Structure):
+    """clp_sdp_params: parameters of the semidefinite relaxation (clp_sdp_solve, clp_batch_sdp_matrices)."""
+    _fields_ = [("max_iters", C.c_int32), ("eps_abs", C.c_double), ("eps_rel", C.c_double), ("time_limit_s", C.c_double)]
+
+
+class ClpSdpInfo(C.Structure):
+    """clp_sdp_info: outcome and statistics of one relaxation."""
+    _fields_ = [
+        ("iters", C.c_int32), ("converged", C.c_int32), ("timed_out", C.c_int32), ("n_nodes", C.c_int32),
+        ("value", C.c_double), ("bound", C.c_double), ("res_pri", C.c_double), ("res_dual", C.c_double),
+        ("rho", C.c_double), ("thr", C.c_double), ("n_sweeps", C.c_int64),
+        ("t", C.c_double), ("kernel_ms", C.c_double), ("proj_ms", C.c_double),
     ]
 
 
@@ -183,6 +200,10 @@ def load():
     L.clp_batch_max_clique_euclidean_dev.argtypes = [vp, i32, i32, ptp, dbl, dbl, dbl, C.c_int, dbl, mip, pp, pp]
     L.clp_batch_max_clique_pointnormal_dev.argtypes = [vp, i32, ptp, dbl, dbl, dbl, dbl, C.c_int, dbl, mip, pp, pp]
     L.clp_batch_max_clique_custom_dev.argtypes = [vp, C.c_char_p, dp, i32, i32, i32, ptp, C.c_int, dbl, mip, pp, pp]
+    L.clp_sdp_default_params.argtypes = [C.POINTER(ClpSdpParams)]; L.clp_sdp_default_params.restype = None
+    L.clp_sdp_solve.argtypes = [vp, C.POINTER(ClpSdpParams), C.POINTER(ClpSdpInfo), ip, dp, dp, dp]
+    L.clp_batch_sdp_matrices.argtypes = [vp, i32, lp, pp, pp, pp, pp, pp, pp, C.POINTER(ClpSdpParams),
+                                         C.POINTER(ClpSdpInfo), pp, pp, pp, pp]
     _lib = L
     return L
 

@@ -15,8 +15,10 @@ Differences that are deliberate and additive:
   * ``solve_as_maximum_clique(MCParams())`` runs on the GPU (clp_max_clique: KCORE, HEU, EXACT) instead of
     PMC; its Solution carries the call's statistics in ``mc_info``.  Without params this mirror still behaves
     like a build without PMC (warning, nothing selected), as it always did.  ``core_numbers()`` is additive.
-  * ``solve_as_msrc_sdr`` behaves like a reference build without SCS (sdp.cpp:298-302): it prints a
-    warning and selects nothing.
+  * ``solve_as_msrc_sdr(SDPParams())`` solves the semidefinite relaxation on the GPU (clp_sdp_solve: ADMM with a
+    Jacobi eigensolver, m <= 128) instead of SCS; its Solution carries X, lambdas, evec1, thr and the call's
+    statistics in ``sdp_info``.  Without params it still behaves like a reference build without SCS
+    (sdp.cpp:298-302): a warning, nothing selected.
 """
 import ctypes as C
 import types
@@ -297,7 +299,9 @@ class MCParams:
 
 
 class SDPParams:
-    """reference sdp.h:39-52 (kept for source compatibility; SCS is not part of the hot path)"""
+    """reference sdp.h:39-52 (same fields and defaults).  max_iters, eps_abs, eps_rel and time_limit_secs steer the GPU
+    relaxation; acceleration_interval, acceleration_lookback and eps_infeas are SCS settings and have no effect (the
+    relaxation is always feasible and bounded)."""
 
     def __init__(self):
         self.verbose = False
@@ -311,6 +315,35 @@ class SDPParams:
 
     def __repr__(self):
         return "<CLIPPER SDP Parameters>"
+
+
+def sdp_params(p):
+    """clp_sdp_params of an SDPParams"""
+    out = _capi.ClpSdpParams()
+    out.max_iters, out.eps_abs = int(p.max_iters), float(p.eps_abs)
+    out.eps_rel, out.time_limit_s = float(p.eps_rel), float(p.time_limit_secs)
+    return out
+
+
+def sdp_solution(info, nodes, X, lambdas, evec1, m, u0):
+    """Solution of solve_as_msrc_sdr (ref clipper.cpp:101-113): nodes, t, u = 0, score = -1, ifinal = 0, sdp_info"""
+    s = Solution()
+    s.t = info.t
+    s.nodes = nodes[: info.n_nodes].tolist()
+    s.u0 = u0
+    s.u = np.zeros(m)
+    s.score = -1
+    s.kernel_ms = info.kernel_ms
+    d = {name: getattr(info, name) for name, _ in _capi.ClpSdpInfo._fields_}
+    d.update(X=np.array(X), lambdas=np.array(lambdas), evec1=np.array(evec1), pobj=-info.value, dobj=-info.bound)
+    s.sdp_info = d
+    return s
+
+
+def sdp_summary(m, info):
+    return ("sdp: n %d iters %d%s%s value %.9g bound %.9g rho %g sweeps %d nodes %d | kernel %.3f ms, eig+proj %.3f ms"
+            % (m, info.iters, " converged" if info.converged else "", " (time limit)" if info.timed_out else "",
+               info.value, info.bound, info.rho, info.n_sweeps, info.n_nodes, info.kernel_ms, info.proj_ms))
 
 
 class Solution:
@@ -331,6 +364,7 @@ class Solution:
         self.kernel_ms = 0.0
         self.prof_ms = (0.0, 0.0, 0.0)  # in-kernel split: dense passes, combine loops, exchange
         self.mc_info = None  # solve_as_maximum_clique: the clp_mc_info fields as a dict
+        self.sdp_info = None  # solve_as_msrc_sdr: X, lambdas, evec1, thr, iters, pobj, dobj and the clp_sdp_info fields
 
     def __repr__(self):
         return "<CLIPPER Solution>"
@@ -575,9 +609,25 @@ class CLIPPER:
         return out[: self._m()].copy()
 
     def solve_as_msrc_sdr(self, params=None):
-        """reference clipper.cpp:101-113 with a build lacking SCS (sdp.cpp:298-302)"""
-        print("Warning: clipper_b200 does not bundle SCS; SDR solver unavailable.")
-        self._finish_unavailable()
+        """reference clipper.cpp:101-113: the semidefinite relaxation of the handle's M and C on the GPU
+        (clp_sdp_solve, m <= 128).  The solution holds the nodes ascending, u = 0, score = -1, and in sdp_info X,
+        lambdas, evec1, thr, iters, pobj = -value, dobj = -bound and the clp_sdp_info fields.
+        Called without params, this mirror keeps its earlier behaviour (a build without SCS: a warning, nothing
+        selected, score = -1); pass SDPParams() to run the solver."""
+        if params is None:
+            print("Warning: clipper_b200 does not bundle SCS; SDR solver unavailable.")
+            self._finish_unavailable()
+            return
+        m = self._m()
+        k = max(m, 1)
+        nodes, X = np.zeros(k, dtype=np.int32), np.zeros((k, k), order="F")
+        lam, ev = np.zeros(k), np.zeros(k)
+        info = _capi.ClpSdpInfo()
+        _capi.check(self._h, self._lib.clp_sdp_solve(self._h, C.byref(sdp_params(params)), C.byref(info), _ip(nodes),
+                                                     _dp(X), _dp(lam), _dp(ev)))
+        self._soln = sdp_solution(info, nodes, X[:m, :m] if m else X[:0, :0], lam[:m], ev[:m], m, self._soln.u0)
+        if params.verbose:
+            print(sdp_summary(m, info))
 
     def _finish_unavailable(self):
         s = Solution()

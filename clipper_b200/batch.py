@@ -18,7 +18,7 @@ import numpy as np
 
 from . import _capi
 from .api import (CudaInvariant, EuclideanDistance, MCParams, PointNormalDistance, Params, Solution, _check_f64,
-                  _dev_matrix_dtype, _wait_for_torch)
+                  _dev_matrix_dtype, _wait_for_torch, sdp_params, sdp_solution)
 
 
 class BatchCLIPPER:
@@ -395,6 +395,45 @@ class MatrixBatchCLIPPER:
         sols = (_capi.ClpSolution * n)()
         self._check(self._lib.clp_batch_solve_matrices(self._b, n, m, *ptrs, u0p, sols, up, np_))
         return _solutions(sols, n, u0s, us, nodes)
+
+    def sdr_many(self, problems, params):
+        """Semidefinite relaxations of many problems in one launch (clp_batch_sdp_matrices): problems as solve_many
+        takes them, without u0 (m <= 128 each); params: SDPParams, one set for the whole call (time_limit_secs bounds
+        the call).  Returns one api.Solution per problem as CLIPPER.solve_as_msrc_sdr on an fp32 handle fills it."""
+        problems = list(problems)
+        n = len(problems)
+        if n == 0:
+            return []
+        vp = C.c_void_p
+        ptrs = [(vp * n)() for _ in range(6)]
+        m = (C.c_int64 * n)()
+        keep, outs = [], []
+        outp = [(vp * n)() for _ in range(4)]
+        for k, p in enumerate(problems):
+            csc = matrices_to_csc(p["M"], p["C"])
+            mk = csc[0]
+            keep.append(csc)
+            m[k] = mk
+            for q in range(6):
+                a = csc[1 + q]
+                ptrs[q][k] = a.ctypes.data if a.size else None
+            o = (np.zeros(max(mk, 1), np.int32), np.zeros((max(mk, 1), max(mk, 1)), order="F"), np.zeros(max(mk, 1)),
+                 np.zeros(max(mk, 1)))
+            outs.append(o)
+            for q in range(4):
+                outp[q][k] = o[q].ctypes.data
+        infos = (_capi.ClpSdpInfo * n)()
+        self._check(self._lib.clp_batch_sdp_matrices(self._b, n, m, *ptrs, C.byref(sdp_params(params)), infos, *outp))
+        out = []
+        for k in range(n):
+            mk = int(m[k])
+            nodes, X, lam, ev = outs[k]
+            out.append(sdp_solution(infos[k], nodes, X[:mk, :mk], lam[:mk], ev[:mk], mk, np.zeros(0)))
+        if params.verbose:
+            print("sdp batch: %d problems, converged %d, timed out %d | kernel %.3f ms"
+                  % (n, sum(infos[k].converged for k in range(n)), sum(infos[k].timed_out for k in range(n)),
+                     infos[0].kernel_ms))
+        return out
 
     set_stream = BatchCLIPPER.set_stream
 

@@ -187,6 +187,50 @@ std::vector<int> max_clique_on(clp_handle h, const maxclique::Params& params)
   return std::vector<int>(nodes.begin(), nodes.begin() + info.n_nodes);
 }
 
+// the semidefinite relaxation of the matrix a handle holds (clp_sdp_solve) as an sdp::Solution; t_parse starts at
+// parse_s (host set-up the caller did), and the SCS timers map to the device call: t_scs its wall time, t_scs_solve the
+// kernel, t_scs_cone the eigendecompositions and projections
+sdp::Solution sdp_on(clp_handle h, const sdp::Params& params, double parse_s)
+{
+  utils::Timer tim;
+  tim.start();
+  int64_t m = 0;
+  check(h, clp_num_associations(h, &m), "clp_num_associations");
+  sdp::Solution s;
+  clp_sdp_params p;
+  clp_sdp_default_params(&p);
+  p.max_iters = params.max_iters; p.eps_abs = params.eps_abs; p.eps_rel = params.eps_rel;
+  p.time_limit_s = params.time_limit_secs;
+  std::vector<int32_t> nodes((size_t)std::max<int64_t>(m, 1));
+  s.X = Eigen::MatrixXd::Zero(m, m);
+  s.lambdas = Eigen::VectorXd::Zero(m);
+  s.evec1 = Eigen::VectorXd::Zero(m);
+  clp_sdp_info info;
+  tim.stop();
+  s.t_parse = parse_s + tim.getElapsedSeconds();
+  check(h, clp_sdp_solve(h, &p, &info, nodes.data(), s.X.data(), s.lambdas.data(), s.evec1.data()), "clp_sdp_solve");
+  tim.reset();
+  tim.start();
+  s.nodes.assign(nodes.begin(), nodes.begin() + info.n_nodes);
+  s.thr = info.thr;
+  s.iters = info.iters;
+  s.pobj = (float)-info.value;  // SCS minimises -<M, X>
+  s.dobj = (float)-info.bound;
+  s.t_scs = info.t;
+  s.t_scs_solve = 1e-3 * info.kernel_ms;
+  s.t_scs_cone = 1e-3 * info.proj_ms;
+  s.t_scs_setup = s.t_scs_linsys = s.t_scs_accel = 0;
+  tim.stop();
+  s.t_extract = tim.getElapsedSeconds();
+  s.t = s.t_parse + s.t_scs + s.t_extract;
+  if (params.verbose)
+    std::cout << "sdp: n " << m << " iters " << info.iters << (info.converged ? " converged" : "")
+              << (info.timed_out ? " (time limit)" : "") << " value " << info.value << " bound " << info.bound << " rho "
+              << info.rho << " sweeps " << info.n_sweeps << " nodes " << info.n_nodes << " | kernel " << info.kernel_ms
+              << " ms, eig+proj " << info.proj_ms << " ms" << std::endl;
+  return s;
+}
+
 }  // namespace
 
 // reference clipper.cpp:82-97, on the graph already in HBM (no dense round trip); params.threads is not used
@@ -206,16 +250,30 @@ void CLIPPER::solveAsMaximumClique(const maxclique::Params& params)
   soln_.score = -1;
 }
 
-// reference clipper.cpp:101-113
-void CLIPPER::solveAsMSRCSDR(const sdp::Params& params)
+// reference clipper.cpp:101-113 without params: a build without SCS (sdp::solve(M, C) selects nothing)
+void CLIPPER::solveAsMSRCSDR()
 {
   Eigen::MatrixXd M = getAffinityMatrix();
   Eigen::MatrixXd C = getConstraintMatrix();
-  sdp::Solution soln = sdp::solve(M, C, params);
+  sdp::Solution soln = sdp::solve(M, C);
   soln_.t = soln.t;
   soln_.ifinal = 0;
   std::swap(soln_.nodes, soln.nodes);
   soln_.u = Eigen::VectorXd::Zero(M.cols());
+  soln_.score = -1;
+}
+
+// reference clipper.cpp:101-113 with params: the relaxation on the GPU, of the matrix already in HBM
+void CLIPPER::solveAsMSRCSDR(const sdp::Params& params)
+{
+  clp_handle h = static_cast<clp_handle>(handle());
+  int64_t m = 0;
+  check(h, clp_num_associations(h, &m), "clp_num_associations");
+  sdp::Solution soln = sdp_on(h, params, 0.0);
+  soln_.t = soln.t;
+  soln_.ifinal = 0;
+  std::swap(soln_.nodes, soln.nodes);
+  soln_.u = Eigen::VectorXd::Zero(m);
   soln_.score = -1;
 }
 
@@ -372,10 +430,27 @@ std::vector<int> solve(const SpAffinity& Ain, const std::vector<int>& S)
 }  // namespace dsd
 
 namespace sdp {
-Solution solve(const Eigen::MatrixXd&, const Eigen::MatrixXd&, const Params&)
+Solution solve(const Eigen::MatrixXd&, const Eigen::MatrixXd&)
 {
   std::cout << "Warning: clipper was not built with SCS; SDR solver unavailable." << std::endl;
   return {};
+}
+
+// reference sdp.cpp:88-296 on a temporary fp64 handle on device 0: the strict upper triangles of M and C are used
+Solution solve(const Eigen::MatrixXd& M, const Eigen::MatrixXd& C, const Params& params)
+{
+  utils::Timer tim;
+  tim.start();
+  const int64_t n = (int64_t)M.rows();
+  if (M.cols() != M.rows() || C.rows() != M.rows() || C.cols() != M.cols())
+    throw std::runtime_error("clipper_b200: sdp::solve expects square M and C of the same size");
+  clp_handle h = nullptr;
+  if (clp_create(0, CLP_STORE_F64, &h) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_create: ") + clp_last_error(nullptr));
+  std::shared_ptr<void> guard(h, [](void* p) { clp_destroy(static_cast<clp_handle>(p)); });
+  check(h, clp_set_dense(h, M.data(), C.data(), n), "clp_set_dense");
+  tim.stop();
+  return sdp_on(h, params, tim.getElapsedSeconds());
 }
 }  // namespace sdp
 

@@ -7,6 +7,7 @@
 #include "clp_clique.cuh"
 #include "clp_batch_clique.cuh"
 #include "clp_batch_matrix.cuh"
+#include "clp_sdp.cuh"
 #include "clp_host_utils.h"
 #include "clp_jit.h"
 #include "../../include/clipper_b200.h"
@@ -156,6 +157,8 @@ struct clp_handle_s {
   // maximum clique (clp_clique.cuh): the bitset adjacency is built on the first call and dropped with the matrix
   DevBuf mc_adj, mc_work, mc_scratch;
   bool mc_adj_valid = false;
+  // semidefinite relaxation (clp_sdp.cuh): problem table | X offset | counter | SdpOut | p | evec1 | X | scratch slot
+  DevBuf sdp_buf;
 
   size_t esize() const { return storage == CLP_STORE_F64 ? 8 : 4; }
   int entry_bytes() const { return sp.packed ? 4 : (int)esize() + 2; }  // compact copy: bytes per stored entry
@@ -1359,6 +1362,94 @@ int mc_solve(clp_handle h, int method, double time_limit_s, int32_t* nodes_out, 
   return CLP_OK;
 }
 
+// ---- semidefinite relaxation (clp_sdp.cuh) ------------------------------------------------------------------------
+template <typename H>
+int sdp_check_params(H* h, const clp_sdp_params* p, const void* info) {
+  if (!p || !info) return fail(h, CLP_ERR_INVALID, "sdp: params and info are required");
+  if (p->max_iters < 1) return fail(h, CLP_ERR_INVALID, "sdp: max_iters must be >= 1");
+  if (!(p->eps_abs >= 0.0) || !(p->eps_rel >= 0.0) || !(p->time_limit_s >= 0.0))
+    return fail(h, CLP_ERR_INVALID, "sdp: eps_abs, eps_rel and time_limit_s must be >= 0 and not NaN");
+  return CLP_OK;
+}
+
+// the in-kernel time limit: what is left of the call's budget at the launch (0: none)
+unsigned long long sdp_limit_ns(const clp_sdp_params& p, std::chrono::steady_clock::time_point t0) {
+  if (!(p.time_limit_s > 0.0)) return 0;
+  const double left = p.time_limit_s - std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  return (unsigned long long)std::max(1.0, std::min(left * 1e9, 1e18));
+}
+
+// the answer read out of the last iterate (ref sdp.cpp:249-262): thr = max|evec1| / 2, nodes = {i : |evec1_i| > thr};
+// lambdas = p ascending.  info->t is left to the caller.
+void sdp_result(const SdpOut& o, int m, const double* pv, const double* ev, float ms, clp_sdp_info* info, int32_t* nodes_out,
+                double* lambdas_out, double* evec1_out) {
+  double mx = 0.0;
+  for (int i = 0; i < m; ++i) mx = std::max(mx, std::fabs(ev[i]));
+  const double thr = mx / 2;
+  int nn = 0;
+  for (int i = 0; i < m; ++i)
+    if (std::fabs(ev[i]) > thr) { if (nodes_out) nodes_out[nn] = i; ++nn; }
+  if (lambdas_out) { std::memcpy(lambdas_out, pv, (size_t)m * 8); std::sort(lambdas_out, lambdas_out + m); }
+  if (evec1_out) std::memcpy(evec1_out, ev, (size_t)m * 8);
+  std::memset(info, 0, sizeof(*info));
+  info->iters = o.iters; info->converged = o.converged; info->timed_out = o.timed_out; info->n_nodes = nn;
+  info->value = o.value; info->bound = o.bound; info->res_pri = o.res_pri; info->res_dual = o.res_dual; info->rho = o.rho;
+  info->thr = thr; info->n_sweeps = o.n_sweeps; info->kernel_ms = ms; info->proj_ms = 1e-6 * (double)o.ns_proj;
+}
+
+int sdp_solve(clp_handle h, const clp_sdp_params* prm, clp_sdp_info* info, int32_t* nodes_out, double* X_out,
+              double* lambdas_out, double* evec1_out) {
+  const auto t0 = std::chrono::steady_clock::now();
+  if (!h->has_matrix) return fail(h, CLP_ERR_INVALID, "sdp: no affinity matrix has been scored or set");
+  if (int rc = sdp_check_params(h, prm, info)) return rc;
+  if (h->world > 1) return fail(h, CLP_ERR_UNSUPPORTED, "sdp: not available on a sharded handle");
+  if (h->m > kSdpMaxM)
+    return fail(h, CLP_ERR_UNSUPPORTED, "sdp: m = " + std::to_string(h->m) + " exceeds CLP_SDP_MAX_M = " + std::to_string(kSdpMaxM));
+  CLP_CUDA(h, cudaSetDevice(h->device));
+  const int m = (int)h->m;
+  const size_t nv = (size_t)((m + 1) & ~1);
+  // device layout: problem table (0) | X offset (64) | counter (128) | SdpOut (256) | p | evec1 | X | scratch slot
+  const size_t o_p = 512, o_e = o_p + nv * 8, o_x = o_e + nv * 8, o_slot = (o_x + (size_t)m * m * 8 + 255) & ~(size_t)255;
+  CLP_CUDA(h, h->sdp_buf.ensure(o_slot + sdp_slot_bytes(m)));
+  char* d = h->sdp_buf.as<char>();
+  unsigned char hdr[256] = {};
+  BatchMatProblem P{};
+  P.m = m;
+  std::memcpy(hdr, &P, sizeof(P));
+  CLP_CUDA(h, cudaMemcpyAsync(d, hdr, sizeof(hdr), cudaMemcpyHostToDevice, h->stream));
+  SdpArgs a{};
+  a.prob = reinterpret_cast<const BatchMatProblem*>(d); a.x_off = reinterpret_cast<const long long*>(d + 64); a.nprob = 1;
+  a.store = h->Mbuf.p; a.ld = h->ld;
+  a.x_out = reinterpret_cast<double*>(d + o_x); a.p_out = reinterpret_cast<double*>(d + o_p);
+  a.e_out = reinterpret_cast<double*>(d + o_e); a.out = reinterpret_cast<SdpOut*>(d + 256);
+  a.next = reinterpret_cast<int*>(d + 128);
+  a.scratch = reinterpret_cast<unsigned char*>(d + o_slot); a.scratch_stride = sdp_slot_bytes(m); a.max_m = m;
+  a.max_iters = prm->max_iters; a.eps_abs = prm->eps_abs; a.eps_rel = prm->eps_rel;
+  const size_t smem = sdp_smem_bytes(m);
+  int rc = with_storage(h, [&](auto t) -> int {
+    using T = decltype(t);
+    CLP_CUDA(h, cudaFuncSetAttribute(sdp_solve_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    a.limit_ns = sdp_limit_ns(*prm, t0);
+    CLP_CUDA(h, cudaEventRecord(h->ev0, h->stream));
+    sdp_solve_kernel<T><<<1, kSdpThreads, smem, h->stream>>>(a);
+    CLP_CUDA(h, cudaGetLastError());
+    CLP_CUDA(h, cudaEventRecord(h->ev1, h->stream));
+    return CLP_OK;
+  });
+  if (rc) return rc;
+  SdpOut o;
+  std::vector<double> pe(2 * nv);
+  CLP_CUDA(h, cudaMemcpyAsync(&o, d + 256, sizeof(o), cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaMemcpyAsync(pe.data(), d + o_p, 2 * nv * 8, cudaMemcpyDeviceToHost, h->stream));
+  if (X_out) CLP_CUDA(h, cudaMemcpyAsync(X_out, d + o_x, (size_t)m * m * 8, cudaMemcpyDeviceToHost, h->stream));
+  CLP_CUDA(h, cudaStreamSynchronize(h->stream));
+  float ms = 0.f;
+  CLP_CUDA(h, cudaEventElapsedTime(&ms, h->ev0, h->ev1));
+  sdp_result(o, m, pe.data(), pe.data() + nv, ms, info, nodes_out, lambdas_out, evec1_out);
+  info->t = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+  return CLP_OK;
+}
+
 }  // namespace
 
 // ==========================================================================================
@@ -1430,7 +1521,7 @@ int clp_destroy(clp_handle h) {
   h->comm.release();
   for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->inv_prm, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
-                    &h->mc_adj, &h->mc_work, &h->mc_scratch})
+                    &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf})
     b->release();
   h->pinned.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1697,6 +1788,17 @@ int clp_max_clique(clp_handle h, int method, double time_limit_s, int32_t* nodes
   return guarded(h, [&] { return mc_solve(h, method, time_limit_s, nodes_out, info); });
 }
 
+void clp_sdp_default_params(clp_sdp_params* p) {
+  if (!p) return;
+  p->max_iters = 2000; p->eps_abs = 1e-3; p->eps_rel = 1e-3; p->time_limit_s = 0.0;
+}
+
+int clp_sdp_solve(clp_handle h, const clp_sdp_params* p, clp_sdp_info* info, int32_t* nodes_out, double* X_out,
+                  double* lambdas_out, double* evec1_out) {
+  if (!h) return CLP_ERR_INVALID;
+  return guarded(h, [&] { return sdp_solve(h, p, info, nodes_out, X_out, lambdas_out, evec1_out); });
+}
+
 int clp_core_numbers(clp_handle h, int32_t* core_out) {
   if (!h || !core_out) return CLP_ERR_INVALID;
   return guarded(h, [&] {
@@ -1906,6 +2008,7 @@ struct clp_batch_s {
   DevBuf custom_in;  // batches scored with a caller's invariant: parameters | work units | problem table
   // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
   DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
+  DevBuf sdp_out;  // batched relaxation: X offsets | SdpOut | p | evec1 | X
   int prof_on = env_int("CLP_PROF_BATCH", 0);
   PinnedBuf pinned;         // the caller's other inputs, then the results
   PinnedBuf pinned_points;  // D1 | D2 | A of scored problems (stage_points)
@@ -2382,19 +2485,24 @@ int batch_launch_matrices(clp_batch b, BatchMatArgs& ba, int grid, size_t smem) 
   return CLP_OK;
 }
 
-int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* cpM, const int32_t* const* riM,
-                         const double* const* vM, const int64_t* const* cpC, const int32_t* const* riC,
-                         const double* const* vC, const double* const* u0, clp_solution* sols, double* const* u_out,
-                         int32_t* const* nodes_out) {
-  if (!b) return CLP_ERR_INVALID;
-  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
-  const clp_params& P = b->prm;
-  if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
-  if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
-  const auto t_begin = std::chrono::steady_clock::now();
-  CLP_CUDA(b, cudaSetDevice(b->device));
+// The host path of the batches given as CSC matrices (clp_batch_solve_matrices, clp_batch_sdp_matrices): the problem
+// table, the checks in their order, the staging (column pointers | values | u0 | row indices | problem table) and one
+// upload to mat_in after ev_up.  u0 == nullptr: the call takes none (no u0 region, no u0 check).  m[p] > m_limit is
+// CLP_ERR_UNSUPPORTED with limit_msg, after the range check of m[p].  The pinned buffer holds at least bytes_out.
+struct MatStaging {
+  std::vector<BatchMatProblem> probs;
+  long long nu = 0;
+  int max_m = 1;
+  size_t o_val = 0, o_u0 = 0, o_ri = 0, o_pr = 0, bytes_in = 0;
+};
+
+int stage_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* cpM, const int32_t* const* riM,
+                   const double* const* vM, const int64_t* const* cpC, const int32_t* const* riC, const double* const* vC,
+                   const double* const* u0, int m_limit, const char* limit_msg, size_t bytes_out_per_u, size_t bytes_out_per_prob,
+                   MatStaging* st) {
   // ---- problem table: sizes and column pointers (the entries are checked while they are copied)
-  std::vector<BatchMatProblem> probs((size_t)nprob);
+  std::vector<BatchMatProblem>& probs = st->probs;
+  probs.assign((size_t)nprob, BatchMatProblem{});
   long long ncp = 0, ne = 0, nu = 0;
   int max_m = 1;
   for (int p = 0; p < nprob; ++p) {
@@ -2402,7 +2510,8 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
     const std::string tag = "problem " + std::to_string(p) + ": ";
     const long long mp = (long long)m[p];
     if (mp < 1 || mp > kBatchMaxM) return fail(b, CLP_ERR_INVALID, tag + "batched problems need 1 <= m <= 4096");
-    if (!u0[p]) return fail(b, CLP_ERR_INVALID, tag + "null u0");
+    if (mp > m_limit) return fail(b, CLP_ERR_UNSUPPORTED, tag + limit_msg);
+    if (u0 && !u0[p]) return fail(b, CLP_ERR_INVALID, tag + "null u0");
     long long nz[2] = {0, 0};
     for (int which = 0; which < 2; ++which) {
       const int64_t* cp = which ? cpC[p] : cpM[p];
@@ -2421,10 +2530,11 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
     max_m = std::max(max_m, (int)mp);
   }
   // ---- staging: column pointers | values | u0 | row indices | problem table, one upload
-  const size_t o_val = (size_t)ncp * 8, o_u0 = (o_val + (size_t)ne * 8 + 15) & ~(size_t)15, o_ri = o_u0 + (size_t)nu * 8;
+  const long long nu0 = u0 ? nu : 0;
+  const size_t o_val = (size_t)ncp * 8, o_u0 = (o_val + (size_t)ne * 8 + 15) & ~(size_t)15, o_ri = o_u0 + (size_t)nu0 * 8;
   const size_t o_pr = (o_ri + (size_t)ne * 4 + 15) & ~(size_t)15;
   const size_t bytes_in = o_pr + (size_t)nprob * sizeof(BatchMatProblem);
-  const size_t bytes_out = (size_t)nu * 8 + (size_t)nprob * (sizeof(SolverOut) + 4);
+  const size_t bytes_out = (size_t)nu * bytes_out_per_u + (size_t)nprob * bytes_out_per_prob;
   CLP_CUDA(b, b->pinned.ensure(std::max(bytes_in, bytes_out) + 4096));
   char* hp = b->pinned.as<char>();
   int64_t* h_cp = reinterpret_cast<int64_t*>(hp);
@@ -2438,7 +2548,7 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
       const BatchMatProblem& q = probs[(size_t)p];
       std::memcpy(h_cp + q.cpM_off, cpM[p], (size_t)(q.m + 1) * 8);
       std::memcpy(h_cp + q.cpC_off, cpC[p], (size_t)(q.m + 1) * 8);
-      std::memcpy(h_u0 + q.u_off, u0[p], (size_t)q.m * 8);
+      if (u0) std::memcpy(h_u0 + q.u_off, u0[p], (size_t)q.m * 8);
       MatCheck cm, cc;
       mat_check_copy(p, "M", 0, q.m, cpM[p], riM[p], vM[p], h_ri + q.eM_off, h_val + q.eM_off, cm);
       if (cm.kind != 0) mat_check_copy(p, "C", 1, q.m, cpC[p], riC[p], vC[p], h_ri + q.eC_off, h_val + q.eC_off, cc);
@@ -2461,11 +2571,34 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   std::memcpy(hp + o_pr, probs.data(), (size_t)nprob * sizeof(BatchMatProblem));
   // the device copy keeps the staging offsets (u0 starts on a 16-byte boundary, the base is cudaMalloc-aligned)
   CLP_CUDA(b, b->mat_in.ensure(bytes_in + 16));
+  CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(b->mat_in.p, hp, bytes_in, cudaMemcpyHostToDevice, b->stream));
+  st->nu = nu; st->max_m = max_m;
+  st->o_val = o_val; st->o_u0 = o_u0; st->o_ri = o_ri; st->o_pr = o_pr; st->bytes_in = bytes_in;
+  return CLP_OK;
+}
+
+int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* cpM, const int32_t* const* riM,
+                         const double* const* vM, const int64_t* const* cpC, const int32_t* const* riC,
+                         const double* const* vC, const double* const* u0, clp_solution* sols, double* const* u_out,
+                         int32_t* const* nodes_out) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC || !u0 || !sols) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  const clp_params& P = b->prm;
+  if (P.rounding == CLP_ROUND_DSD) return fail(b, CLP_ERR_UNSUPPORTED, "Rounding::DSD is not available in a batch");
+  if (P.maxlsiters < 1) return fail(b, CLP_ERR_INVALID, "maxlsiters must be >= 1");
+  const auto t_begin = std::chrono::steady_clock::now();
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  MatStaging st;
+  if (int rc = stage_matrices(b, nprob, m, cpM, riM, vM, cpC, riC, vC, u0, kBatchMaxM, "", 8, sizeof(SolverOut) + 4, &st))
+    return rc;
+  const std::vector<BatchMatProblem>& probs = st.probs;
+  const long long nu = st.nu;
+  const int max_m = st.max_m;
+  const size_t o_val = st.o_val, o_u0 = st.o_u0, o_ri = st.o_ri, o_pr = st.o_pr, bytes_in = st.bytes_in;
   CLP_CUDA(b, b->out_u.ensure((size_t)nu * 8 + 16));
   CLP_CUDA(b, b->outs.ensure((size_t)nprob * sizeof(SolverOut)));
   CLP_CUDA(b, b->nnz.ensure((size_t)nprob * 4 + 16));
-  CLP_CUDA(b, cudaEventRecord(b->ev_up, b->stream));
-  CLP_CUDA(b, cudaMemcpyAsync(b->mat_in.p, hp, bytes_in, cudaMemcpyHostToDevice, b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->nnz.p, 0, (size_t)nprob * 4 + 16, b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->outs.p, 0, (size_t)nprob * sizeof(SolverOut), b->stream));
   CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
@@ -2495,6 +2628,83 @@ int batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int
   CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
   if (int rc = batch_launch_matrices(b, ba, grid, bs.total)) return rc;
   return batch_finish(b, "batch matrices", "scatter", probs, nu, max_m, grid, L.total, bytes_in, t_begin, sols, u_out, nodes_out);
+}
+
+// ---- batched semidefinite relaxations of given matrices (clp_sdp.cuh) ---------------------------------------------
+// The host path of clp_batch_solve_matrices (stage_matrices), then sdp_solve_kernel<float> with the CSC inputs: each
+// CTA scatters its problem into an fp32 store as clp_set_sparse_upper does, so problem p gets what an fp32 handle gets.
+int batch_sdp_matrices(clp_batch b, int32_t nprob, const int64_t* m, const int64_t* const* cpM, const int32_t* const* riM,
+                       const double* const* vM, const int64_t* const* cpC, const int32_t* const* riC, const double* const* vC,
+                       const clp_sdp_params* prm, clp_sdp_info* infos, int32_t* const* nodes_out, double* const* X_out,
+                       double* const* lambdas_out, double* const* evec1_out) {
+  if (!b) return CLP_ERR_INVALID;
+  if (nprob <= 0 || !m || !cpM || !riM || !vM || !cpC || !riC || !vC) return fail(b, CLP_ERR_INVALID, "bad batch arguments");
+  if (int rc = sdp_check_params(b, prm, infos)) return rc;
+  const auto t_begin = std::chrono::steady_clock::now();
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  // read back: p and evec1 (2 per u slot), X (m^2 <= 128 * slot), SdpOut
+  MatStaging st;
+  const std::string limit_msg = "the relaxation needs m <= CLP_SDP_MAX_M = " + std::to_string(kSdpMaxM);
+  if (int rc = stage_matrices(b, nprob, m, cpM, riM, vM, cpC, riC, vC, nullptr, kSdpMaxM, limit_msg.c_str(),
+                              (2 + kSdpMaxM) * 8, sizeof(SdpOut), &st))
+    return rc;
+  const long long nu = st.nu;
+  std::vector<long long> x_off((size_t)nprob);
+  long long nx = 0;
+  for (int p = 0; p < nprob; ++p) { x_off[(size_t)p] = nx; nx += (long long)st.probs[(size_t)p].m * st.probs[(size_t)p].m; }
+  // device outputs: X offsets | SdpOut | p | evec1 | X
+  const size_t o_out = ((size_t)nprob * 8 + 255) & ~(size_t)255, o_p = o_out + (((size_t)nprob * sizeof(SdpOut) + 255) & ~(size_t)255);
+  const size_t o_e = o_p + (size_t)nu * 8, o_x = o_e + (size_t)nu * 8, bytes_out = o_x + (size_t)nx * 8;
+  CLP_CUDA(b, b->sdp_out.ensure(bytes_out));
+  char* d = b->sdp_out.as<char>();
+  CLP_CUDA(b, cudaMemcpyAsync(d, x_off.data(), (size_t)nprob * 8, cudaMemcpyHostToDevice, b->stream));
+  CLP_CUDA(b, cudaMemsetAsync(b->sync.p, 0, sizeof(SyncBlock), b->stream));
+  const size_t smem = sdp_smem_bytes(st.max_m);
+  int occ = 0;
+  CLP_CUDA(b, cudaFuncSetAttribute(sdp_solve_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  CLP_CUDA(b, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, sdp_solve_kernel<float>, kSdpThreads, smem));
+  if (occ < 1) return fail(b, CLP_ERR_CUDA, "sdp kernel does not fit an SM");
+  int grid = 0;
+  if (int rc = batch_grid(b, occ, nprob, sdp_slot_bytes(st.max_m), b->scratch, nullptr, &grid)) return rc;
+  const char* din = b->mat_in.as<char>();
+  SdpArgs a{};
+  a.prob = reinterpret_cast<const BatchMatProblem*>(din + st.o_pr); a.x_off = reinterpret_cast<const long long*>(d);
+  a.nprob = nprob;
+  a.colptr = reinterpret_cast<const long long*>(din); a.val = reinterpret_cast<const double*>(din + st.o_val);
+  a.rowidx = reinterpret_cast<const int*>(din + st.o_ri);
+  a.x_out = reinterpret_cast<double*>(d + o_x); a.p_out = reinterpret_cast<double*>(d + o_p);
+  a.e_out = reinterpret_cast<double*>(d + o_e); a.out = reinterpret_cast<SdpOut*>(d + o_out);
+  a.next = reinterpret_cast<int*>(&b->sync.as<SyncBlock>()->counts[0]);
+  a.flags = &b->sync.as<SyncBlock>()->flags;
+  a.scratch = b->scratch.as<unsigned char>(); a.scratch_stride = sdp_slot_bytes(st.max_m); a.max_m = st.max_m;
+  a.max_iters = prm->max_iters; a.eps_abs = prm->eps_abs; a.eps_rel = prm->eps_rel;
+  a.limit_ns = sdp_limit_ns(*prm, t_begin);
+  CLP_CUDA(b, cudaEventRecord(b->ev0, b->stream));
+  sdp_solve_kernel<float><<<grid, kSdpThreads, smem, b->stream>>>(a);
+  CLP_CUDA(b, cudaGetLastError());
+  CLP_CUDA(b, cudaEventRecord(b->ev1, b->stream));
+  char* hp = b->pinned.as<char>();
+  SyncBlock h_sb;
+  CLP_CUDA(b, cudaMemcpyAsync(hp, d + o_out, bytes_out - o_out, cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaMemcpyAsync(&h_sb, b->sync.p, sizeof(SyncBlock), cudaMemcpyDeviceToHost, b->stream));
+  CLP_CUDA(b, cudaStreamSynchronize(b->stream));
+  if (h_sb.flags != 0) return fail(b, CLP_ERR_CUDA, "batched matrices: the device found an entry the host check passed");
+  float ms = 0.f;
+  CLP_CUDA(b, cudaEventElapsedTime(&ms, b->ev0, b->ev1));
+  b->last_ctas = grid; b->last_scratch = (long long)grid * (long long)a.scratch_stride; b->last_nnz = 0;
+  const SdpOut* h_out = reinterpret_cast<const SdpOut*>(hp);
+  const double* h_p = reinterpret_cast<const double*>(hp + (o_p - o_out));
+  const double* h_e = h_p + nu;
+  const double* h_x = h_e + nu;
+  for (int p = 0; p < nprob; ++p) {
+    const BatchMatProblem& q = st.probs[(size_t)p];
+    sdp_result(h_out[p], q.m, h_p + q.u_off, h_e + q.u_off, ms, &infos[p], nodes_out ? nodes_out[p] : nullptr,
+               lambdas_out ? lambdas_out[p] : nullptr, evec1_out ? evec1_out[p] : nullptr);
+    if (X_out && X_out[p]) std::memcpy(X_out[p], h_x + x_off[(size_t)p], (size_t)q.m * q.m * 8);
+  }
+  const double wall = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  for (int p = 0; p < nprob; ++p) infos[p].t = wall / nprob;
+  return CLP_OK;
 }
 
 // ---- batched solve of dense device tensors (batch_dense_solve_kernel) ---------------------------------------------
@@ -2946,7 +3156,7 @@ int clp_batch_destroy(clp_batch b) {
   cudaSetDevice(b->device);
   for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in, &b->custom_in,
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
-                    &b->mc_pscratch, &b->mc_sscratch})
+                    &b->mc_pscratch, &b->mc_sscratch, &b->sdp_out})
     d->release();
   b->pinned.release();
   b->pinned_points.release();
@@ -2993,6 +3203,17 @@ int clp_batch_solve_matrices(clp_batch b, int32_t nprob, const int64_t* m,
                              const double* const* u0, clp_solution* sols, double* const* u_out, int32_t* const* nodes_out) {
   return guarded(b, [&] {
     return batch_solve_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, u0, sols, u_out, nodes_out);
+  });
+}
+
+int clp_batch_sdp_matrices(clp_batch b, int32_t nprob, const int64_t* m,
+                           const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
+                           const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
+                           const clp_sdp_params* p, clp_sdp_info* infos, int32_t* const* nodes_out,
+                           double* const* X_out, double* const* lambdas_out, double* const* evec1_out) {
+  return guarded(b, [&] {
+    return batch_sdp_matrices(b, nprob, m, colptrM, rowidxM, valM, colptrC, rowidxC, valC, p, infos, nodes_out, X_out,
+                              lambdas_out, evec1_out);
   });
 }
 

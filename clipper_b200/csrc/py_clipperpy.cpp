@@ -7,6 +7,7 @@
 // pybind11/eigen.h requires the real Eigen).  D1, D2, A, u0, M, C are "noconvert" like upstream:
 // float64 / int32 numpy arrays are required.
 #include <cstring>
+#include <optional>
 #include <sstream>
 
 #include <pybind11/numpy.h>
@@ -249,7 +250,13 @@ PYBIND11_MODULE(clipperpy, m)
     .def("solve", [](clipper::CLIPPER& c, const py::array& u0) { c.solve(to_vector(u0, "u0")); },
          "u0"_a.noconvert() = arr_d(0))
     .def("solve_as_maximum_clique", &clipper::CLIPPER::solveAsMaximumClique, "params"_a = clipper::maxclique::Params{})
-    .def("solve_as_msrc_sdr", &clipper::CLIPPER::solveAsMSRCSDR, "params"_a = clipper::sdp::Params{})
+    // without params: a build without SCS (nothing selected); with params: the GPU relaxation
+    .def("solve_as_msrc_sdr",
+         [](clipper::CLIPPER& c, std::optional<clipper::sdp::Params> params) {
+           if (params) c.solveAsMSRCSDR(*params);
+           else c.solveAsMSRCSDR();
+         },
+         "params"_a = py::none())
     .def("get_initial_associations", [](clipper::CLIPPER& c) { return from_assoc(c.getInitialAssociations()); })
     .def("get_selected_associations", [](clipper::CLIPPER& c) { return from_assoc(c.getSelectedAssociations()); })
     .def("get_solution", &clipper::CLIPPER::getSolution)

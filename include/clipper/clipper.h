@@ -75,7 +75,9 @@ namespace clipper {
     void solve(const Eigen::VectorXd& u0 = Eigen::VectorXd());
 
     void solveAsMaximumClique(const maxclique::Params& params = {});
-    void solveAsMSRCSDR(const sdp::Params& params = {});
+    /// without params: a build without SCS (nothing selected); with params: the relaxation on the GPU (m <= 128)
+    void solveAsMSRCSDR();
+    void solveAsMSRCSDR(const sdp::Params& params);
 
     const Solution& getSolution() const { return soln_; }
     Affinity getAffinityMatrix();

@@ -1,9 +1,14 @@
 /**
  * @file sdp.h
  * @brief Semidefinite relaxation front-end (mirror of reference sdp.h:20-57).
- *        The relaxation is solved by the third-party SCS library in the reference
- *        (CMakeLists.txt:83-86); it is not part of the GPU hot path and SCS is not bundled, so
- *        solve() behaves like a reference build without CLIPPER_HAS_SCS (sdp.cpp:298-302).
+ *        The reference solves the relaxation with the third-party SCS library (CMakeLists.txt:83-86).
+ *        Here solve(M, C, params) solves it on the GPU (clp_sdp_solve: ADMM with a Jacobi eigensolver
+ *        in shared memory, m <= 128, on a temporary fp64 handle on device 0) and fills every field:
+ *        pobj = -<M, X> and dobj = -bound (SCS's sign), t_scs the device call, t_scs_solve its kernel,
+ *        t_scs_cone its eigendecompositions and projections; t_scs_setup, t_scs_linsys and
+ *        t_scs_accel are 0.  acceleration_interval, acceleration_lookback and eps_infeas are SCS
+ *        settings without effect: the relaxation is always feasible and bounded.  solve(M, C)
+ *        without params behaves like a reference build without CLIPPER_HAS_SCS (sdp.cpp:298-302).
  */
 #pragma once
 #include <vector>
@@ -37,7 +42,8 @@ namespace sdp {
     float time_limit_secs = 0;
   };
 
-  Solution solve(const Eigen::MatrixXd& M, const Eigen::MatrixXd& C, const Params& params = Params{});
+  Solution solve(const Eigen::MatrixXd& M, const Eigen::MatrixXd& C);
+  Solution solve(const Eigen::MatrixXd& M, const Eigen::MatrixXd& C, const Params& params);
 
 } // ns sdp
 } // ns clipper

@@ -440,6 +440,57 @@ int clp_batch_max_clique_custom_dev(clp_batch b, const char* source, const doubl
                                     int32_t d, const clp_points_dev* pts, int method, double time_limit_s,
                                     clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
 
+/* ---- semidefinite relaxation (solveAsMSRCSDR / sdp::solve, ref clipper.cpp:101-113, sdp.cpp:88-296) ---------------
+ * Solves  maximise <M, X>  subject to  X PSD, tr X = 1, X_ij = 0 where C_ij = 0, X_ij >= 0 where C_ij != 0  on the
+ * device by two-block ADMM (X in the spectraplex, Z in the polyhedral set), with a Jacobi eigensolver in shared memory
+ * and the whole iteration inside one kernel (DESIGN §3 "SDR" states every step).  It is not SCS: the iterates and the
+ * iteration counts differ from the reference's; the problem and the read-out of the answer are the reference's.
+ * The relaxation is always feasible and bounded (X = e_i e_i' is feasible, C has a unit diagonal), so there is no
+ * infeasibility detection.  Stopping: the primal and dual residuals (max norm) within eps_abs + eps_rel * scale, and
+ * |value - bound| within eps_abs + eps_rel * max(|value|, |bound|), where bound is a dual upper bound on the optimum.
+ * Outputs of the last iterate: X (m x m, PSD with trace 1; the polyhedral constraints hold to res_pri), lambdas = the
+ * eigenvalues of X ascending, evec1 = the eigenvector of the largest one (its largest-magnitude entry, lowest index
+ * among equals, made positive), thr = max|evec1| / 2 and the nodes {i : |evec1_i| > thr} ascending (sdp.cpp:249-262).
+ * m <= CLP_SDP_MAX_M.  A repeated call gives bit-identical outputs. */
+#define CLP_SDP_MAX_M 128
+typedef struct clp_sdp_params {
+  int32_t max_iters;   /* 2000 (reference sdp.h defaults) */
+  double eps_abs;      /* 1e-3 */
+  double eps_rel;      /* 1e-3 */
+  double time_limit_s; /* 0: none; else the call returns its last iterate with timed_out = 1 once this has passed */
+} clp_sdp_params;
+void clp_sdp_default_params(clp_sdp_params* p);
+typedef struct clp_sdp_info {
+  int32_t iters, converged, timed_out, n_nodes;
+  double value;     /* <M, X>                                                                  */
+  double bound;     /* dual upper bound on the optimum                                         */
+  double res_pri;   /* max |X - Z|                                                             */
+  double res_dual;  /* rho * max |Z - Z_previous|                                              */
+  double rho;       /* final ADMM penalty                                                      */
+  double thr;       /* node threshold max|evec1| / 2                                           */
+  int64_t n_sweeps; /* Jacobi sweeps, all iterations and bound evaluations                     */
+  double t;         /* wall-clock seconds of the call (batches: divided by nprob)              */
+  double kernel_ms; /* device time of the launch (CUDA events; batches: the whole launch)      */
+  double proj_ms;   /* in-kernel time in the eigendecompositions and simplex projections       */
+} clp_sdp_info;
+/* The handle's M and C, exactly as clp_get_dense(h, 0 / 1) returns them, gathered on the device; the handle's matrix is
+ * left as it was.  nodes_out (m int32), X_out (m * m, column-major), lambdas_out (m) and evec1_out (m) may be NULL.
+ * CLP_ERR_INVALID: no matrix, NULL p or info, max_iters < 1, a negative or NaN eps or time limit.
+ * CLP_ERR_UNSUPPORTED: m > CLP_SDP_MAX_M, a sharded handle.  m = 1 gives X = [1] and nodes {0}. */
+int clp_sdp_solve(clp_handle h, const clp_sdp_params* p, clp_sdp_info* info, int32_t* nodes_out, double* X_out,
+                  double* lambdas_out, double* evec1_out);
+/* Many relaxations in one launch (one CTA per problem, problems drawn from a counter).  Problems as
+ * clp_batch_solve_matrices takes them (strictly-upper CSC M and C), checked in the same order with the same messages,
+ * and then CLP_ERR_UNSUPPORTED for m[p] > CLP_SDP_MAX_M naming the problem.  Problem p gets bit for bit what an fp32
+ * handle gives after clp_set_sparse_upper and clp_sdp_solve with the same parameters.  time_limit_s bounds the whole
+ * call: a problem cut off returns its last iterate with timed_out = 1.  infos[p].kernel_ms is the whole launch, t the
+ * wall-clock time divided by nprob.  Output arrays and their entries may be NULL. */
+int clp_batch_sdp_matrices(clp_batch b, int32_t nprob, const int64_t* m,
+                           const int64_t* const* colptrM, const int32_t* const* rowidxM, const double* const* valM,
+                           const int64_t* const* colptrC, const int32_t* const* rowidxC, const double* const* valC,
+                           const clp_sdp_params* p, clp_sdp_info* infos, int32_t* const* nodes_out,
+                           double* const* X_out, double* const* lambdas_out, double* const* evec1_out);
+
 #ifdef __cplusplus
 }
 #endif
