@@ -36,10 +36,12 @@ SYMBOLS = [
     "clp_batch_solve_euclidean_dev", "clp_batch_solve_pointnormal_dev", "clp_batch_solve_custom_dev",
     "clp_batch_max_clique_euclidean_dev", "clp_batch_max_clique_pointnormal_dev", "clp_batch_max_clique_custom_dev",
     "clp_sdp_default_params", "clp_sdp_solve", "clp_batch_sdp_matrices",
+    "clp_correspondences", "clp_correspondences_dev",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 SDP_MAX_M = 128
+KNN_MAX_K, KNN_MAX_D = 32, 64
 
 
 class ClpParams(C.Structure):
@@ -204,6 +206,8 @@ def load():
     L.clp_sdp_solve.argtypes = [vp, C.POINTER(ClpSdpParams), C.POINTER(ClpSdpInfo), ip, dp, dp, dp]
     L.clp_batch_sdp_matrices.argtypes = [vp, i32, lp, pp, pp, pp, pp, pp, pp, C.POINTER(ClpSdpParams),
                                          C.POINTER(ClpSdpInfo), pp, pp, pp, pp]
+    L.clp_correspondences.argtypes = [vp, dp, i32, i64, dp, i64, i32, dbl, C.c_int, ip, i64, lp]
+    L.clp_correspondences_dev.argtypes = [vp, vp, i32, i64, vp, i64, i32, dbl, C.c_int, vp, i64, lp]
     _lib = L
     return L
 

@@ -4,6 +4,7 @@ Names, argument meaning and defaults follow reference bindings/python/py_clipper
   invariants.{Invariant, PairwiseInvariant, EuclideanDistanceParams, EuclideanDistance,
               PointNormalDistanceParams, PointNormalDistance}
   utils.{create_all_to_all, k2ij}      dsd.{solve, create_all_to_all, k2ij}
+  utils.distance_based_correspondences(_dev) (additive: putative associations by exact kNN on the GPU)
   Rounding, Params, Solution, MCParams, SDPParams, CLIPPER (11 methods)
 
 Differences that are deliberate and additive:
@@ -205,6 +206,106 @@ def create_all_to_all(n1, n2):
     return A
 
 
+_knn_handles = {}   # (device, on_device) -> a handle kept for clp_correspondences(_dev)
+
+
+class _KnnHandle:
+    def __init__(self, device):
+        self._lib = _capi.load()
+        self.h = C.c_void_p()
+        rc = self._lib.clp_create(int(device), STORE_F32, C.byref(self.h))
+        if rc != _capi.OK:
+            msg = self._lib.clp_last_error(None)
+            raise ClipperError(rc, msg.decode() if msg else "clp_create failed")
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self._lib.clp_destroy(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+
+def _knn_handle(device, on_device):
+    key = (int(device), bool(on_device))
+    if key not in _knn_handles:
+        _knn_handles[key] = _KnnHandle(device)
+    return _knn_handles[key].h
+
+
+def _knn_args(knn, d):
+    knn, d = int(knn), int(d)
+    if knn < 1 or d < 1:
+        raise ValueError("knn and d must be >= 1, got knn=%d, d=%d" % (knn, d))
+    return min(knn, 2 ** 31 - 1)
+
+
+def _knn_rows(n1, n2, knn):
+    """rows of the output buffer: n1 * min(knn, n2).  knn above the cap is left for the C-ABI to reject
+    (CLP_ERR_UNSUPPORTED), so the buffer is sized for the cap, not for knn."""
+    return n1 * min(knn, _capi.KNN_MAX_K, n2)
+
+
+_CUDA_STREAM_LEGACY = 1   # cudaStreamLegacy
+
+
+def distance_based_correspondences(D1, D2, knn, radius, enforce_1to1):
+    """putative associations by exact k-nearest-neighbour matching on the GPU (device 0; clp_correspondences; the
+    reference's benchmarks/bm_utils.cpp:147-232 for any d <= 64): D1 (d, n1) and D2 (d, n2) float64 -> (m, 2) int32.
+    Column i of D1 goes to its min(knn, n2) nearest columns of D2 by squared distance (ties to the lower index), and
+    (i, j) is kept when that distance is <= radius * radius.  Rows by i, then rank; with enforce_1to1 every j keeps its
+    nearest i (ties to the smallest i), rows by j."""
+    D1 = np.asfortranarray(_check_f64(D1, "D1"))
+    D2 = np.asfortranarray(_check_f64(D2, "D2"))
+    if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
+        raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+    (d, n1), n2 = D1.shape, D2.shape[1]
+    knn = _knn_args(knn, d)
+    cap = _knn_rows(n1, n2, knn)
+    A = np.zeros(2 * max(cap, 1), dtype=np.int32)
+    h = _knn_handle(0, False)
+    m = C.c_int64()
+    _capi.check(h, _capi.load().clp_correspondences(h, _dp(D1), d, n1, _dp(D2), n2, knn, float(radius),
+                                                    int(bool(enforce_1to1)), _ip(A), cap, C.byref(m)))
+    m = int(m.value)
+    return np.asfortranarray(A[:2 * m].reshape(2, m).T)
+
+
+def distance_based_correspondences_dev(D1, D2, knn, radius, enforce_1to1):
+    """distance_based_correspondences of CUDA tensors D1 (d, n1), D2 (d, n2) float64 on their device and torch's current
+    stream (clp_correspondences_dev) -> (m, 2) int32 CUDA tensor, column-major (strides (1, m)): the layout
+    CLIPPER.score_pairwise_consistency_dev reads without a copy.  Tensors of another layout are copied on the device
+    first.  Returns once m is known (the stream is synchronised)."""
+    import torch
+    for name, X in (("D1", D1), ("D2", D2)):
+        if not isinstance(X, torch.Tensor) or X.dtype != torch.float64:
+            raise TypeError("%s must be a torch.float64 tensor" % name)
+        if not X.is_cuda:
+            raise ValueError("%s must be a CUDA tensor, got one on %s" % (name, X.device))
+    if D1.device != D2.device:
+        raise ValueError("D1 and D2 must be on the same device, got %s and %s" % (D1.device, D2.device))
+    if D1.dim() != 2 or D2.dim() != 2 or D1.shape[0] != D2.shape[0]:
+        raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+    (d, n1), n2 = D1.shape, D2.shape[1]
+    knn = _knn_args(knn, d)
+    cap = _knn_rows(n1, n2, knn)
+    device = D1.device.index
+    P1, P2 = D1.t().contiguous(), D2.t().contiguous()   # column-major (d, n) is row-major (n, d)
+    A = torch.empty(2 * max(cap, 1), dtype=torch.int32, device=D1.device)
+    h = _knn_handle(device, True)
+    lib = _capi.load()
+    # torch's default stream reports the handle 0, which clp_set_stream reads as "a stream of the handle's own": name
+    # the legacy default stream instead, so the kernels stay ordered after torch's work (the copies above included)
+    stream = torch.cuda.current_stream(D1.device).cuda_stream or _CUDA_STREAM_LEGACY
+    _capi.check(h, lib.clp_set_stream(h, C.c_void_p(stream)))
+    m = C.c_int64()
+    _capi.check(h, lib.clp_correspondences_dev(h, P1.data_ptr(), d, n1, P2.data_ptr(), n2, knn, float(radius),
+                                               int(bool(enforce_1to1)), A.data_ptr(), cap, C.byref(m)))
+    m = int(m.value)
+    return A[:2 * m].view(2, m).t()
+
+
 def k2ij(k, n):
     """reference utils.cpp:87-97"""
     i, j = C.c_uint64(), C.c_uint64()
@@ -243,7 +344,9 @@ def dsd_solve(A, S=()):
 
 utils = types.SimpleNamespace(create_all_to_all=create_all_to_all, k2ij=k2ij,
                               find_indices_of_k_largest=find_indices_of_k_largest,
-                              find_indices_where_above_threshold=find_indices_where_above_threshold)
+                              find_indices_where_above_threshold=find_indices_where_above_threshold,
+                              distance_based_correspondences=distance_based_correspondences,
+                              distance_based_correspondences_dev=distance_based_correspondences_dev)
 dsd = types.SimpleNamespace(solve=dsd_solve, create_all_to_all=create_all_to_all, k2ij=k2ij)
 
 

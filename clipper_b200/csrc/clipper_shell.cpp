@@ -15,7 +15,9 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 #include <iostream>
+#include <memory>
 #include <random>
 #include <stdexcept>
 #include <string>
@@ -367,6 +369,29 @@ Association createAllToAll(size_t n1, size_t n2)
 {
   Association A(n1 * n2, 2);
   if (n1 * n2 > 0) clp_create_all_to_all((int64_t)n1, (int64_t)n2, reinterpret_cast<int32_t*>(A.data()));
+  return A;
+}
+
+// bm_utils.cpp:147-232 on the GPU (clp_correspondences) with a temporary handle on device 0
+Association distanceBasedCorrespondences(const invariants::Data& D1, const invariants::Data& D2, size_t knn, double radius,
+                                         bool enforce1to1)
+{
+  if (D1.rows() != D2.rows())
+    throw std::runtime_error("clipper_b200: distanceBasedCorrespondences expects D1 and D2 with the same number of rows");
+  const int32_t k = (int32_t)std::min<size_t>(knn, (size_t)INT32_MAX);  // the C-ABI checks the range
+  const int64_t n1 = (int64_t)D1.cols(), n2 = (int64_t)D2.cols();
+  // sized for the cap, not for knn: a knn above it is rejected by the C-ABI (CLP_ERR_UNSUPPORTED) before anything is written
+  const int64_t cap = n1 * std::min<int64_t>({(int64_t)std::max<int32_t>(k, 0), (int64_t)CLP_KNN_MAX_K, n2});
+  clp_handle h = nullptr;
+  if (clp_create(0, CLP_STORE_F32, &h) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_create: ") + clp_last_error(nullptr));
+  std::shared_ptr<void> guard(h, [](void* p) { clp_destroy(static_cast<clp_handle>(p)); });
+  std::vector<int32_t> buf((size_t)std::max<int64_t>(2 * cap, 1));
+  int64_t m = 0;
+  check(h, clp_correspondences(h, D1.data(), (int32_t)D1.rows(), n1, D2.data(), n2, k, radius,
+                               enforce1to1 ? 1 : 0, buf.data(), cap, &m), "clp_correspondences");
+  Association A(m, 2);
+  if (m > 0) std::memcpy(A.data(), buf.data(), sizeof(int32_t) * (size_t)(2 * m));
   return A;
 }
 

@@ -8,6 +8,7 @@
 #include "clp_batch_clique.cuh"
 #include "clp_batch_matrix.cuh"
 #include "clp_sdp.cuh"
+#include "clp_knn.cuh"
 #include "clp_host_utils.h"
 #include "clp_jit.h"
 #include "../../include/clipper_b200.h"
@@ -159,6 +160,8 @@ struct clp_handle_s {
   bool mc_adj_valid = false;
   // semidefinite relaxation (clp_sdp.cuh): problem table | X offset | counter | SdpOut | p | evec1 | X | scratch slot
   DevBuf sdp_buf;
+  // putative associations (clp_knn.cuh): staged clouds | partial lists | merged lists | counts and scans | staged A
+  DevBuf knn_buf;
 
   size_t esize() const { return storage == CLP_STORE_F64 ? 8 : 4; }
   int entry_bytes() const { return sp.packed ? 4 : (int)esize() + 2; }  // compact copy: bytes per stored entry
@@ -1450,6 +1453,150 @@ int sdp_solve(clp_handle h, const clp_sdp_params* prm, clp_sdp_info* info, int32
   return CLP_OK;
 }
 
+// ---- putative associations (clp_knn.cuh) --------------------------------------------------------------------------
+static_assert(kKnnMaxK == CLP_KNN_MAX_K && kKnnMaxD == CLP_KNN_MAX_D, "clp_knn.cuh and clipper_b200.h disagree on the caps");
+template <int D, int K>
+cudaError_t knn_partial(dim3 grid, size_t smem, cudaStream_t s, const KnnArgs& a) {
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(knn_partial_kernel<D, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  knn_partial_kernel<D, K><<<grid, kKnnThreads, smem, s>>>(a);
+  return cudaGetLastError();
+}
+
+template <int D>
+cudaError_t knn_partial_k(int K, dim3 grid, size_t smem, cudaStream_t s, const KnnArgs& a) {
+  switch (K) {
+    case 1: return knn_partial<D, 1>(grid, smem, s, a);
+    case 2: return knn_partial<D, 2>(grid, smem, s, a);
+    case 4: return knn_partial<D, 4>(grid, smem, s, a);
+    case 8: return knn_partial<D, 8>(grid, smem, s, a);
+    case 16: return knn_partial<D, 16>(grid, smem, s, a);
+    default: return knn_partial<D, 32>(grid, smem, s, a);
+  }
+}
+
+cudaError_t knn_merge(int K, unsigned blocks, cudaStream_t s, const KnnArgs& a, double r2, double* lsd, int* lj, int* cnt) {
+  switch (K) {
+    case 1: knn_merge_kernel<1><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+    case 2: knn_merge_kernel<2><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+    case 4: knn_merge_kernel<4><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+    case 8: knn_merge_kernel<8><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+    case 16: knn_merge_kernel<16><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+    default: knn_merge_kernel<32><<<blocks, 256, 0, s>>>(a, r2, lsd, lj, cnt); break;
+  }
+  return cudaGetLastError();
+}
+
+// clp_correspondences(_dev): D1, D2 on the host (staged in knn_buf, A read back into A_out) or on the device (A written
+// into A_out).  Nothing of the handle but knn_buf, its stream and its error string is touched.
+int correspondences(clp_handle h, bool on_device, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2,
+                    int32_t knn, double radius, int enforce_1to1, int32_t* A_out, int64_t capacity, int64_t* m_out) {
+  if (!h) return CLP_ERR_INVALID;
+  if (!m_out) return fail(h, CLP_ERR_INVALID, "correspondences: m_out is required");
+  *m_out = 0;
+  if (knn < 1) return fail(h, CLP_ERR_INVALID, "correspondences: knn must be >= 1");
+  if (d < 1) return fail(h, CLP_ERR_INVALID, "correspondences: d must be >= 1");
+  if (n1 < 0 || n2 < 0) return fail(h, CLP_ERR_INVALID, "correspondences: negative n1 or n2");
+  if ((n1 > 0 && !D1) || (n2 > 0 && !D2)) return fail(h, CLP_ERR_INVALID, "correspondences: NULL point cloud");
+  if (knn > kKnnMaxK)
+    return fail(h, CLP_ERR_UNSUPPORTED, "correspondences: knn = " + std::to_string(knn) + " exceeds CLP_KNN_MAX_K = " +
+                                            std::to_string(kKnnMaxK));
+  if (d > kKnnMaxD)
+    return fail(h, CLP_ERR_UNSUPPORTED, "correspondences: d = " + std::to_string(d) + " exceeds CLP_KNN_MAX_D = " +
+                                            std::to_string(kKnnMaxD));
+  if (n1 >= kKnnNone || n2 >= kKnnNone)
+    return fail(h, CLP_ERR_UNSUPPORTED, "correspondences: n1 and n2 must be below 2^31 - 1 (int32 indices)");
+  const int kk = (int)std::min<int64_t>(knn, n2);
+  const long long rows = (long long)n1 * kk;
+  if (capacity < rows || (rows > 0 && !A_out))
+    return fail(h, CLP_ERR_INVALID, "correspondences: A_out holds " + std::to_string(capacity) + " rows, n1 * min(knn, n2) = " +
+                                        std::to_string(rows) + " are required");
+  if (rows == 0) return CLP_OK;
+  CLP_CUDA(h, cudaSetDevice(h->device));
+  const cudaStream_t st = h->stream;
+  int K = 1;
+  while (K < kk) K *= 2;
+  const int D = d <= 3 ? d : 0;
+  const int T = D > 0 ? kKnnTileReg : kKnnTileGen;
+  // candidate slices: enough CTAs for every SM several times over, each slice at least 1024 candidates
+  const long long qblocks = (n1 + kKnnThreads - 1) / kKnnThreads;
+  const long long want = (4LL * h->sm_count + qblocks - 1) / qblocks;
+  const long long nsplit0 = std::max<long long>(1, std::min<long long>({want, (n2 + 1023) / 1024, 1024}));
+  const long long chunk = round_up((n2 + nsplit0 - 1) / nsplit0, T);
+  const int nsplit = (int)((n2 + chunk - 1) / chunk);
+  // scratch layout, every region 256-byte aligned
+  const long long nmax = std::max<long long>(n1, n2);
+  const long long nb = (nmax + kKnnScanItems - 1) / kKnnScanItems;
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_d1 = on_device ? 0 : take((size_t)d * n1 * 8), o_d2 = on_device ? 0 : take((size_t)d * n2 * 8);
+  const size_t lsize = (size_t)nsplit * kk * n1;
+  const size_t o_psd = take(lsize * 8), o_pj = take(lsize * 4);
+  const size_t o_lsd = nsplit > 1 ? take((size_t)kk * n1 * 8) : o_psd, o_lj = nsplit > 1 ? take((size_t)kk * n1 * 4) : o_pj;
+  const size_t o_cnt = take((size_t)nmax * 4), o_off = take((size_t)nmax * 8), o_bsum = take((size_t)nb * 8), o_tot = take(8);
+  const size_t o_best = enforce_1to1 ? take((size_t)n2 * 8) : 0, o_c0 = enforce_1to1 ? take((size_t)n2 * 4) : 0;
+  const size_t o_a = on_device ? 0 : take((size_t)2 * rows * 4);
+  CLP_CUDA(h, h->knn_buf.ensure(at));
+  char* base = h->knn_buf.as<char>();
+  auto at_ = [&](size_t o) { return reinterpret_cast<void*>(base + o); };
+  if (!on_device) {
+    CLP_CUDA(h, cudaMemcpyAsync(at_(o_d1), D1, (size_t)d * n1 * 8, cudaMemcpyHostToDevice, st));
+    CLP_CUDA(h, cudaMemcpyAsync(at_(o_d2), D2, (size_t)d * n2 * 8, cudaMemcpyHostToDevice, st));
+    D1 = static_cast<const double*>(at_(o_d1)); D2 = static_cast<const double*>(at_(o_d2));
+  }
+  int32_t* A = on_device ? A_out : static_cast<int32_t*>(at_(o_a));
+  KnnArgs a{};
+  a.D1 = D1; a.D2 = D2; a.d = d; a.n1 = n1; a.n2 = n2; a.kk = kk; a.nsplit = nsplit; a.chunk = chunk;
+  a.part_sd = static_cast<double*>(at_(o_psd)); a.part_j = static_cast<int*>(at_(o_pj));
+  double* lsd = static_cast<double*>(at_(o_lsd));
+  int* lj = static_cast<int*>(at_(o_lj));
+  int* cnt = static_cast<int*>(at_(o_cnt));
+  long long* off = static_cast<long long*>(at_(o_off));
+  long long* bsum = static_cast<long long*>(at_(o_bsum));
+  long long* total = static_cast<long long*>(at_(o_tot));
+  const dim3 grid((unsigned)qblocks, (unsigned)nsplit);
+  const size_t smem = knn_partial_smem(D, d);
+  cudaError_t e;
+  switch (D) {
+    case 1: e = knn_partial_k<1>(K, grid, smem, st, a); break;
+    case 2: e = knn_partial_k<2>(K, grid, smem, st, a); break;
+    case 3: e = knn_partial_k<3>(K, grid, smem, st, a); break;
+    default: e = knn_partial_k<0>(K, grid, smem, st, a); break;
+  }
+  CLP_CUDA(h, e);
+  const double r2 = radius * radius;  // bm_utils.cpp:192: NaN keeps nothing, inf keeps every neighbour
+  const unsigned b1 = (unsigned)((n1 + 255) / 256), b2 = (unsigned)((n2 + 255) / 256);
+  CLP_CUDA(h, knn_merge(K, b1, st, a, r2, lsd, lj, cnt));
+  if (!enforce_1to1) {
+    knn_scan_blocks_kernel<<<(unsigned)((n1 + kKnnScanItems - 1) / kKnnScanItems), 256, 0, st>>>(cnt, n1, off, bsum);
+    knn_scan_top_kernel<<<1, 1024, 0, st>>>(bsum, (n1 + kKnnScanItems - 1) / kKnnScanItems, total);
+    knn_write_kernel<<<b1, 256, 0, st>>>(cnt, off, bsum, lj, n1, total, A);
+  } else {
+    auto* best = static_cast<unsigned long long*>(at_(o_best));
+    auto* c0best = static_cast<unsigned int*>(at_(o_c0));
+    CLP_CUDA(h, cudaMemsetAsync(best, 0xff, (size_t)n2 * 8, st));
+    CLP_CUDA(h, cudaMemsetAsync(c0best, 0xff, (size_t)n2 * 4, st));
+    knn_best_sd_kernel<<<b1, 256, 0, st>>>(cnt, lsd, lj, n1, best);
+    knn_best_c0_kernel<<<b1, 256, 0, st>>>(cnt, lsd, lj, n1, best, c0best);
+    knn_flag_kernel<<<b2, 256, 0, st>>>(c0best, n2, cnt);
+    knn_scan_blocks_kernel<<<(unsigned)((n2 + kKnnScanItems - 1) / kKnnScanItems), 256, 0, st>>>(cnt, n2, off, bsum);
+    knn_scan_top_kernel<<<1, 1024, 0, st>>>(bsum, (n2 + kKnnScanItems - 1) / kKnnScanItems, total);
+    knn_write_1to1_kernel<<<b2, 256, 0, st>>>(c0best, off, bsum, n2, total, A);
+  }
+  CLP_CUDA(h, cudaGetLastError());
+  long long m = 0;
+  CLP_CUDA(h, cudaMemcpyAsync(&m, total, sizeof(m), cudaMemcpyDeviceToHost, st));
+  CLP_CUDA(h, cudaStreamSynchronize(st));
+  if (!on_device && m > 0) {
+    CLP_CUDA(h, cudaMemcpyAsync(A_out, A, (size_t)2 * m * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CLP_CUDA(h, cudaStreamSynchronize(st));
+  }
+  *m_out = m;
+  return CLP_OK;
+}
+
 }  // namespace
 
 // ==========================================================================================
@@ -1521,7 +1668,7 @@ int clp_destroy(clp_handle h) {
   h->comm.release();
   for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->inv_prm, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
-                    &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf})
+                    &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf, &h->knn_buf})
     b->release();
   h->pinned.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
@@ -1797,6 +1944,18 @@ int clp_sdp_solve(clp_handle h, const clp_sdp_params* p, clp_sdp_info* info, int
                   double* lambdas_out, double* evec1_out) {
   if (!h) return CLP_ERR_INVALID;
   return guarded(h, [&] { return sdp_solve(h, p, info, nodes_out, X_out, lambdas_out, evec1_out); });
+}
+
+int clp_correspondences(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2, int32_t knn,
+                        double radius, int enforce_1to1, int32_t* A_out, int64_t capacity, int64_t* m) {
+  return guarded(h, [&] { return correspondences(h, false, D1, d, n1, D2, n2, knn, radius, enforce_1to1, A_out, capacity, m); });
+}
+
+int clp_correspondences_dev(clp_handle h, const double* D1_dev, int32_t d, int64_t n1, const double* D2_dev, int64_t n2,
+                            int32_t knn, double radius, int enforce_1to1, int32_t* A_dev, int64_t capacity, int64_t* m) {
+  return guarded(h, [&] {
+    return correspondences(h, true, D1_dev, d, n1, D2_dev, n2, knn, radius, enforce_1to1, A_dev, capacity, m);
+  });
 }
 
 int clp_core_numbers(clp_handle h, int32_t* core_out) {

@@ -156,6 +156,18 @@ void pybind_utils(py::module& m)
         "Maps a flat index k to coordinate of a square nxn symmetric matrix");
 }
 
+// additive: putative associations by exact kNN on the GPU (registered on utils only, not on the dsd alias)
+void pybind_correspondences(py::module& m)
+{
+  m.def("distance_based_correspondences",
+        [](const py::array& D1, const py::array& D2, size_t knn, double radius, bool enforce_1to1) {
+          return from_assoc(clipper::utils::distanceBasedCorrespondences(to_matrix(D1, "D1"), to_matrix(D2, "D2"), knn,
+                                                                         radius, enforce_1to1));
+        },
+        "D1"_a, "D2"_a, "knn"_a, "radius"_a, "enforce_1to1"_a,
+        "Associations (m, 2) int32: every column of D1 (d x n1) to its knn nearest columns of D2 within radius, on the GPU.");
+}
+
 void pybind_dsd(py::module& m)
 {
   // the reference registers pybind_utils on this submodule by mistake (py_clipper.cpp:127-128, SURVEY D8b);
@@ -173,6 +185,7 @@ PYBIND11_MODULE(clipperpy, m)
   pybind_invariants(m_invariants);
   py::module m_utils = m.def_submodule("utils");
   pybind_utils(m_utils);
+  pybind_correspondences(m_utils);
   py::module m_dsd = m.def_submodule("dsd");
   pybind_utils(m_dsd);
   pybind_dsd(m_dsd);

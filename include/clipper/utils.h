@@ -38,6 +38,16 @@ namespace utils {
   /// flat index k of the strict upper triangle -> (row, col) (utils.cpp:87-97)
   std::tuple<size_t,size_t> k2ij(size_t k, size_t n);
 
+  /**
+   * @brief Putative associations by exact k-nearest-neighbour matching on the GPU (device 0, a temporary handle);
+   * the reference's benchmarks/bm_utils.cpp:147-232 for any d <= CLP_KNN_MAX_D.  Column i of D1 is matched to its
+   * min(knn, n2) nearest columns of D2 (squared distance, ties to the lower index); a pair is kept when its squared
+   * distance is <= radius * radius.  Rows (c0, c1) by c0 then rank; with enforce1to1 every c1 keeps its nearest c0
+   * (ties to the smallest), rows by c1.  Semantics in full: include/clipper_b200.h, clp_correspondences.
+   */
+  Association distanceBasedCorrespondences(const invariants::Data& D1, const invariants::Data& D2, size_t knn,
+                                           double radius, bool enforce1to1);
+
   /// simple named profiling timer (utils.h:107-163)
   class Timer
   {

@@ -199,6 +199,34 @@ int32_t clp_find_above(const double* x, int64_t n, double thr, int32_t* out);   
 /* exact densest subgraph restricted to S (dsd.cpp:274-320); A is dense column-major n x n */
 int32_t clp_dsd_dense(const double* A, int64_t n, const int32_t* S, int32_t nS, int32_t* out);
 
+/* ---- putative associations by nearest-neighbour matching (ref benchmarks/bm_utils.cpp:147-232) ----------------------
+ * The association set A that scoring takes, built on the device by exact brute force (clp_knn.cuh).  D1 (d x n1) and D2
+ * (d x n2) are fp64 in the layout of the scoring calls.  For query i of D1 and candidate j of D2
+ *   sd(i, j) = sum_k (D1[k,i] - D2[k,j])^2, accumulated for k = 0 .. d-1 in order, every subtract, multiply and add
+ *   rounded on its own (no FMA).  For d = 3 this is nanoflann's L2 tail loop; the reference's own bits depend on whether
+ *   its compiler contracted that loop to FMAs.
+ * Neighbours of i: the min(knn, n2) candidates of least (sd, j) in lexicographic order: on equal sd the lower j wins (the
+ *   reference's order among ties is that of its tree walk), and knn > n2 gives n2 neighbours (the reference reads
+ *   uninitialised memory there).  A NaN sd is never a neighbour (nanoflann's strict <), so a query may have fewer.
+ * Radius: the pair (i, j) is kept when sd <= radius * radius (fp64, bm_utils.cpp:192,201): radius = inf gives plain kNN,
+ *   a NaN radius keeps nothing.
+ * Without 1-to-1 the rows come in the order i ascending, then neighbour rank.  With enforce_1to1 != 0 the kept pairs are
+ *   grouped by c1 = j: each c1 keeps the c0 = i of least sd, the smallest c0 among equal ones (the reference keeps the
+ *   first pushed), and the rows come in c1 ascending order.
+ * A_out receives the m rows column-major with leading dimension m (c0 in A_out[0 .. m), c1 in A_out[m .. 2m)): the layout
+ * clp_score_*_dev reads.  capacity (rows) must be at least n1 * min(knn, n2); *m receives m.  n1 = 0 or n2 = 0 gives
+ * m = 0 (A_out may then be NULL).  The handle's device, stream (clp_set_stream) and error string are used; its matrix and
+ * state stay as they were.  The call returns when m (and, for the host call, A_out) is available.
+ * Errors: CLP_ERR_INVALID for a NULL m, knn < 1, d < 1, a negative n1 or n2 or a NULL cloud; then CLP_ERR_UNSUPPORTED for
+ * knn > CLP_KNN_MAX_K, d > CLP_KNN_MAX_D or n1, n2 >= 2^31 - 1; then CLP_ERR_INVALID for capacity < n1 * min(knn, n2). */
+#define CLP_KNN_MAX_K 32
+#define CLP_KNN_MAX_D 64
+int clp_correspondences(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2, int32_t knn,
+                        double radius, int enforce_1to1, int32_t* A_out, int64_t capacity, int64_t* m);
+/* D1_dev, D2_dev and A_dev on the handle's device; enqueued on the handle's stream, which is synchronised to read m. */
+int clp_correspondences_dev(clp_handle h, const double* D1_dev, int32_t d, int64_t n1, const double* D2_dev, int64_t n2,
+                            int32_t knn, double radius, int enforce_1to1, int32_t* A_dev, int64_t capacity, int64_t* m);
+
 /* ---- multi-GPU: row-block sharding, one process (or one handle) per GPU ------------------- */
 /* SURVEY 8e.  Rank r of `world` keeps rows [row0,row0+rows) x all columns of M in its HBM
  * (clp_shard_rows gives the partition; scoring needs no communication).  clp_solve*() then runs
