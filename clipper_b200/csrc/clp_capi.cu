@@ -75,6 +75,15 @@ static int env_int(const char* name, int dflt) {
   return (v && *v) ? std::atoi(v) : dflt;
 }
 
+// Rounding::DSD_HEU keeps the round(F) largest entries of u (ref clipper.cpp:302-308).  The reference converts with
+// (int)std::round(F), which is undefined for NaN (u0 = 0) and for F >= 2^31 (weights near 1e10); here round(F) is
+// clamped to [0, m] first and NaN keeps no node.
+static int32_t heu_omega(double F, int64_t m) {
+  const double r = std::round(F);
+  if (!(r >= 1.0)) return 0;
+  return r >= (double)m ? (int32_t)m : (int32_t)r;
+}
+
 struct clp_handle_s {
   int device = 0;
   int storage = CLP_STORE_F32;
@@ -1042,9 +1051,9 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
     nodes.resize((size_t)h->m);
     nodes.resize((size_t)clp_find_above(u, h->m, 0.0, nodes.data()));
   } else if (P.rounding == CLP_ROUND_DSD_HEU) {
-    const int omega = (int)std::round(so.F);
+    const int32_t omega = heu_omega(so.F, h->m);
     if (omega >= 1) {
-      nodes.resize((size_t)std::min<long long>(omega, h->m));
+      nodes.resize((size_t)omega);
       nodes.resize((size_t)clp_find_k_largest(u, h->m, omega, nodes.data()));
     }
   } else if (P.rounding == CLP_ROUND_DSD) {
@@ -2205,9 +2214,9 @@ void batch_results(const clp_params& P, const std::vector<Prob>& probs, const do
       nodes.resize((size_t)q.m);
       nodes.resize((size_t)clp_find_above(u, q.m, 0.0, nodes.data()));
     } else {  // DSD_HEU, ref clipper.cpp:302-308
-      const int omega = (int)std::round(so.F);
+      const int32_t omega = heu_omega(so.F, q.m);
       if (omega >= 1) {
-        nodes.resize((size_t)std::min<long long>(omega, q.m));
+        nodes.resize((size_t)omega);
         nodes.resize((size_t)clp_find_k_largest(u, q.m, omega, nodes.data()));
       }
     }

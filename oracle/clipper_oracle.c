@@ -710,7 +710,10 @@ int orc_solve(const orc_problem *p, const double *u0, const orc_params *P, orc_s
   if (P->rounding == 0) {
     n_nodes = orc_find_above(u, n, 0.0, nodes_out);
   } else if (P->rounding == 2) {
-    const int omega = (int)round(F);
+    /* the reference's (int)std::round(F) is undefined for NaN and F >= 2^31: round(F) is clamped to [0, n] first
+     * and NaN keeps no node (a defined divergence, DESIGN section 5) */
+    const double r = round(F);
+    const int32_t omega = !(r >= 1.0) ? 0 : (r >= (double)n ? (int32_t)n : (int32_t)r);
     n_nodes = orc_find_k_largest(u, n, omega, nodes_out);
   } else {
     /* Rounding::DSD (clipper.cpp:294-300): densest subgraph of M_ restricted to support(u) */
