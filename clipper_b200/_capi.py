@@ -37,6 +37,7 @@ SYMBOLS = [
     "clp_batch_max_clique_euclidean_dev", "clp_batch_max_clique_pointnormal_dev", "clp_batch_max_clique_custom_dev",
     "clp_sdp_default_params", "clp_sdp_solve", "clp_batch_sdp_matrices",
     "clp_correspondences", "clp_correspondences_dev",
+    "clp_batch_correspondences", "clp_batch_correspondences_dev",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
@@ -208,6 +209,8 @@ def load():
                                          C.POINTER(ClpSdpInfo), pp, pp, pp, pp]
     L.clp_correspondences.argtypes = [vp, dp, i32, i64, dp, i64, i32, dbl, C.c_int, ip, i64, lp]
     L.clp_correspondences_dev.argtypes = [vp, vp, i32, i64, vp, i64, i32, dbl, C.c_int, vp, i64, lp]
+    L.clp_batch_correspondences.argtypes = [vp, i32, i32, pp, lp, pp, lp, i32, dbl, C.c_int, pp, i64, lp]
+    L.clp_batch_correspondences_dev.argtypes = [vp, i32, i32, vp, lp, lp, vp, lp, lp, i32, dbl, C.c_int, vp, lp, i64, lp]
     _lib = L
     return L
 

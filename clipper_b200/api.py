@@ -5,6 +5,7 @@ Names, argument meaning and defaults follow reference bindings/python/py_clipper
               PointNormalDistanceParams, PointNormalDistance}
   utils.{create_all_to_all, k2ij}      dsd.{solve, create_all_to_all, k2ij}
   utils.distance_based_correspondences(_dev) (additive: putative associations by exact kNN on the GPU)
+  utils.distance_based_correspondences_many(_dev) (additive: the same for a batch of cloud pairs in one call)
   Rounding, Params, Solution, MCParams, SDPParams, CLIPPER (11 methods)
 
 Differences that are deliberate and additive:
@@ -306,6 +307,118 @@ def distance_based_correspondences_dev(D1, D2, knn, radius, enforce_1to1):
     return A[:2 * m].view(2, m).t()
 
 
+_knn_batches = {}   # (device, on_device) -> a batch kept for clp_batch_correspondences(_dev)
+
+
+class _KnnBatch:
+    def __init__(self, device):
+        self._lib = _capi.load()
+        self.b = C.c_void_p()
+        rc = self._lib.clp_batch_create(int(device), C.byref(self.b))
+        if rc != _capi.OK:
+            msg = self._lib.clp_batch_last_error(None)
+            raise ClipperError(rc, msg.decode() if msg else "clp_batch_create failed")
+
+    def __del__(self):
+        try:
+            if getattr(self, "b", None):
+                self._lib.clp_batch_destroy(self.b)
+                self.b = None
+        except Exception:
+            pass
+
+    def check(self, rc):
+        if rc != _capi.OK:
+            msg = self._lib.clp_batch_last_error(self.b)
+            raise ClipperError(rc, msg.decode() if msg else "")
+
+
+def _knn_batch(device, on_device):
+    key = (int(device), bool(on_device))
+    if key not in _knn_batches:
+        _knn_batches[key] = _KnnBatch(device)
+    return _knn_batches[key]
+
+
+def distance_based_correspondences_many(D1s, D2s, knn, radius, enforce_1to1):
+    """distance_based_correspondences of every pair (D1s[p], D2s[p]) in one batched call on the GPU (device 0;
+    clp_batch_correspondences): lists of (d, n1[p]) and (d, n2[p]) float64 arrays, one d for all -> a list of (m[p], 2)
+    int32 arrays, entry p exactly what distance_based_correspondences(D1s[p], D2s[p], ...) returns."""
+    D1s, D2s = list(D1s), list(D2s)
+    if len(D1s) != len(D2s):
+        raise ValueError("D1s and D2s must have the same length, got %d and %d" % (len(D1s), len(D2s)))
+    if not D1s:
+        return []
+    P1 = [np.asfortranarray(_check_f64(X, "D1s[%d]" % k)) for k, X in enumerate(D1s)]
+    P2 = [np.asfortranarray(_check_f64(X, "D2s[%d]" % k)) for k, X in enumerate(D2s)]
+    d = P1[0].shape[0] if P1[0].ndim == 2 else -1
+    for k, (X, Y) in enumerate(zip(P1, P2)):
+        if X.ndim != 2 or Y.ndim != 2 or X.shape[0] != d or Y.shape[0] != d:
+            raise ValueError("pair %d: D1s and D2s must hold (d, n1) and (d, n2) arrays of one d" % k)
+    knn = _knn_args(knn, d)
+    nb = len(P1)
+    n1 = [X.shape[1] for X in P1]
+    n2 = [Y.shape[1] for Y in P2]
+    cap = max(_knn_rows(a, b, knn) for a, b in zip(n1, n2))
+    outs = [np.zeros(2 * max(cap, 1), dtype=np.int32) for _ in range(nb)]
+    vp, i64 = C.c_void_p, C.c_int64
+    m = (i64 * nb)()
+    kb = _knn_batch(0, False)
+    kb.check(_capi.load().clp_batch_correspondences(
+        kb.b, nb, d, (vp * nb)(*[X.ctypes.data for X in P1]), (i64 * nb)(*n1), (vp * nb)(*[Y.ctypes.data for Y in P2]),
+        (i64 * nb)(*n2), knn, float(radius), int(bool(enforce_1to1)), (vp * nb)(*[A.ctypes.data for A in outs]), cap, m))
+    return [np.asfortranarray(A[:2 * int(mk)].reshape(2, int(mk)).T) for A, mk in zip(outs, m)]
+
+
+def distance_based_correspondences_many_dev(D1, D2, knn, radius, enforce_1to1, n1=None, n2=None):
+    """distance_based_correspondences of a batch of cloud pairs in GPU memory, in one call on torch's current stream
+    (clp_batch_correspondences_dev).  D1 (B, d, n1_max) and D2 (B, d, n2_max): float64 CUDA tensors on one device, any
+    strides (an ``expand`` along B shares one cloud); n1, n2: B sizes in [0, the padded dimension] (default: the padded
+    dimensions); nothing past them is read.  Returns (A, m): A a (B, cap, 2) int32 tensor with strides (2 cap, 1, cap),
+    cap = the largest n1[p] * min(knn, n2[p]), whose first m[p] rows of problem p are exactly what
+    distance_based_correspondences_dev gives for (D1[p, :, :n1[p]], D2[p, :, :n2[p]]); m a list of B ints.  These are
+    the A and m that BatchCLIPPER.solve_many_dev and max_clique_many_dev take without a copy -- except that there m[p] = 0
+    means all-to-all and m[p] > 4096 is refused, so a problem without rows (or with too many) must be left out.
+    Returns once m is known (the stream is synchronised)."""
+    import torch
+    for name, X in (("D1", D1), ("D2", D2)):
+        if not isinstance(X, torch.Tensor) or X.dtype != torch.float64:
+            raise TypeError("%s must be a torch.float64 tensor" % name)
+    if D1.dim() != 3 or D2.dim() != 3 or D1.shape[:2] != D2.shape[:2] or D1.shape[0] == 0:
+        raise ValueError("D1 and D2 must be (B, d, n1_max) and (B, d, n2_max) with B >= 1, got %s and %s"
+                         % (tuple(D1.shape), tuple(D2.shape)))
+    nb, d = int(D1.shape[0]), int(D1.shape[1])
+    knn = _knn_args(knn, d)
+
+    def sizes(x, pad, name):
+        v = [int(pad)] * nb if x is None else [int(k) for k in x]
+        if len(v) != nb or any(k < 0 or k > pad for k in v):
+            raise ValueError("%s must hold B sizes in [0, %d]" % (name, pad))
+        return v
+
+    s1, s2 = sizes(n1, D1.shape[2], "n1"), sizes(n2, D2.shape[2], "n2")
+    for name, X in (("D1", D1), ("D2", D2)):
+        if not X.is_cuda:
+            raise ValueError("%s must be a CUDA tensor, got one on %s" % (name, X.device))
+    if D1.device != D2.device:
+        raise ValueError("D1 and D2 must be on the same device, got %s and %s" % (D1.device, D2.device))
+    cap = max(_knn_rows(a, b, knn) for a, b in zip(s1, s2))
+    buf = torch.empty(2 * nb * max(cap, 1), dtype=torch.int32, device=D1.device)
+    A = buf.as_strided((nb, cap, 2), (2 * cap, 1, cap))
+    kb = _knn_batch(D1.device.index, True)
+    lib = _capi.load()
+    # as in distance_based_correspondences_dev: torch's default stream is named as the legacy default stream
+    stream = torch.cuda.current_stream(D1.device).cuda_stream or _CUDA_STREAM_LEGACY
+    kb.check(lib.clp_batch_set_stream(kb.b, C.c_void_p(stream)))
+    i64 = C.c_int64
+    m = (i64 * nb)()
+    kb.check(lib.clp_batch_correspondences_dev(
+        kb.b, nb, d, D1.data_ptr() or None, (i64 * 3)(*D1.stride()), (i64 * nb)(*s1), D2.data_ptr() or None,
+        (i64 * 3)(*D2.stride()), (i64 * nb)(*s2), knn, float(radius), int(bool(enforce_1to1)), buf.data_ptr(),
+        (i64 * 3)(2 * max(cap, 1), 1, max(cap, 1)), cap, m))
+    return A, [int(x) for x in m]
+
+
 def k2ij(k, n):
     """reference utils.cpp:87-97"""
     i, j = C.c_uint64(), C.c_uint64()
@@ -346,7 +459,9 @@ utils = types.SimpleNamespace(create_all_to_all=create_all_to_all, k2ij=k2ij,
                               find_indices_of_k_largest=find_indices_of_k_largest,
                               find_indices_where_above_threshold=find_indices_where_above_threshold,
                               distance_based_correspondences=distance_based_correspondences,
-                              distance_based_correspondences_dev=distance_based_correspondences_dev)
+                              distance_based_correspondences_dev=distance_based_correspondences_dev,
+                              distance_based_correspondences_many=distance_based_correspondences_many,
+                              distance_based_correspondences_many_dev=distance_based_correspondences_many_dev)
 dsd = types.SimpleNamespace(solve=dsd_solve, create_all_to_all=create_all_to_all, k2ij=k2ij)
 
 

@@ -395,6 +395,48 @@ Association distanceBasedCorrespondences(const invariants::Data& D1, const invar
   return A;
 }
 
+// every pair in one clp_batch_correspondences call with a temporary batch on device 0
+std::vector<Association> distanceBasedCorrespondencesBatch(const std::vector<invariants::Data>& D1s,
+                                                           const std::vector<invariants::Data>& D2s, size_t knn,
+                                                           double radius, bool enforce1to1)
+{
+  if (D1s.size() != D2s.size())
+    throw std::runtime_error("clipper_b200: distanceBasedCorrespondencesBatch expects as many D1s as D2s");
+  const size_t nprob = D1s.size();
+  if (nprob == 0) return {};
+  if (nprob > (size_t)INT32_MAX) throw std::runtime_error("clipper_b200: distanceBasedCorrespondencesBatch: too many pairs");
+  for (size_t p = 0; p < nprob; ++p)
+    if (D1s[p].rows() != D1s[0].rows() || D2s[p].rows() != D1s[0].rows())
+      throw std::runtime_error("clipper_b200: distanceBasedCorrespondencesBatch expects every cloud with the same number of rows");
+  const int32_t k = (int32_t)std::min<size_t>(knn, (size_t)INT32_MAX);  // the C-ABI checks the range
+  std::vector<int64_t> n1(nprob), n2(nprob), m(nprob, 0);
+  std::vector<const double*> p1(nprob), p2(nprob);
+  int64_t cap = 0;
+  for (size_t p = 0; p < nprob; ++p) {
+    n1[p] = (int64_t)D1s[p].cols(); n2[p] = (int64_t)D2s[p].cols();
+    p1[p] = D1s[p].data(); p2[p] = D2s[p].data();
+    // sized for the cap, not for knn: a knn above it is rejected by the C-ABI (CLP_ERR_UNSUPPORTED) before anything is written
+    cap = std::max(cap, n1[p] * std::min<int64_t>({(int64_t)std::max<int32_t>(k, 0), (int64_t)CLP_KNN_MAX_K, n2[p]}));
+  }
+  clp_batch b = nullptr;
+  if (clp_batch_create(0, &b) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_batch_create: ") + clp_batch_last_error(nullptr));
+  std::shared_ptr<void> guard(b, [](void* q) { clp_batch_destroy(static_cast<clp_batch>(q)); });
+  std::vector<std::vector<int32_t>> bufs(nprob);
+  std::vector<int32_t*> out(nprob);
+  for (size_t p = 0; p < nprob; ++p) { bufs[p].resize((size_t)std::max<int64_t>(2 * cap, 1)); out[p] = bufs[p].data(); }
+  const int rc = clp_batch_correspondences(b, (int32_t)nprob, (int32_t)D1s[0].rows(), p1.data(), n1.data(), p2.data(),
+                                           n2.data(), k, radius, enforce1to1 ? 1 : 0, out.data(), cap, m.data());
+  if (rc != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_batch_correspondences: ") + clp_batch_last_error(b));
+  std::vector<Association> As(nprob);
+  for (size_t p = 0; p < nprob; ++p) {
+    As[p].resize(m[p], 2);
+    if (m[p] > 0) std::memcpy(As[p].data(), bufs[p].data(), sizeof(int32_t) * (size_t)(2 * m[p]));
+  }
+  return As;
+}
+
 Eigen::VectorXd selectFromIndicator(const Eigen::VectorXd& x, const Eigen::VectorXi& ind)
 {
   long cnt = 0;

@@ -2177,6 +2177,9 @@ struct clp_batch_s {
   // batched maximum clique: problem table, edges, per-problem regions, per-problem search state, task rounds, scratch
   DevBuf mc_probs, mc_edges, mc_adj, mc_vint, mc_tpre, mc_out, mc_state, mc_rounds, mc_pscratch, mc_sscratch;
   DevBuf sdp_out;  // batched relaxation: X offsets | SdpOut | p | evec1 | X
+  // putative associations (clp_knn.cuh): problem table | staged clouds | lists | scan | counts | 1-to-1 | staged A
+  DevBuf knn_buf;
+  PinnedBuf knn_pinned;     // the table and host clouds going up, the counts and host A coming back
   int prof_on = env_int("CLP_PROF_BATCH", 0);
   PinnedBuf pinned;         // the caller's other inputs, then the results
   PinnedBuf pinned_points;  // D1 | D2 | A of scored problems (stage_points)
@@ -3290,6 +3293,236 @@ int solve_dev_check(clp_batch b, int32_t nprob, const clp_points_dev* pts, const
   in.u0_dev = u0_dev; in.u0_stride = u0_stride; in.u_out_dev = u_out_dev; in.u_out_stride = u_out_stride;
   return CLP_OK;
 }
+
+// ---- putative associations for a batch of cloud pairs (clp_knn.cuh) -------------------------------------------------
+template <int D, int K>
+cudaError_t knn_batch_partial(dim3 grid, size_t smem, cudaStream_t s, const KnnBatchArgs& a) {
+  if (smem > 48 * 1024) {
+    cudaError_t e = cudaFuncSetAttribute(knn_batch_partial_kernel<D, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  knn_batch_partial_kernel<D, K><<<grid, kKnnThreads, smem, s>>>(a);
+  return cudaGetLastError();
+}
+
+template <int D>
+cudaError_t knn_batch_partial_k(int K, dim3 grid, size_t smem, cudaStream_t s, const KnnBatchArgs& a) {
+  switch (K) {
+    case 1: return knn_batch_partial<D, 1>(grid, smem, s, a);
+    case 2: return knn_batch_partial<D, 2>(grid, smem, s, a);
+    case 4: return knn_batch_partial<D, 4>(grid, smem, s, a);
+    case 8: return knn_batch_partial<D, 8>(grid, smem, s, a);
+    case 16: return knn_batch_partial<D, 16>(grid, smem, s, a);
+    default: return knn_batch_partial<D, 32>(grid, smem, s, a);
+  }
+}
+
+cudaError_t knn_batch_merge(int K, unsigned blocks, cudaStream_t s, const KnnBatchArgs& a) {
+  switch (K) {
+    case 1: knn_batch_merge_kernel<1><<<blocks, kKnnThreads, 0, s>>>(a); break;
+    case 2: knn_batch_merge_kernel<2><<<blocks, kKnnThreads, 0, s>>>(a); break;
+    case 4: knn_batch_merge_kernel<4><<<blocks, kKnnThreads, 0, s>>>(a); break;
+    case 8: knn_batch_merge_kernel<8><<<blocks, kKnnThreads, 0, s>>>(a); break;
+    case 16: knn_batch_merge_kernel<16><<<blocks, kKnnThreads, 0, s>>>(a); break;
+    default: knn_batch_merge_kernel<32><<<blocks, kKnnThreads, 0, s>>>(a); break;
+  }
+  return cudaGetLastError();
+}
+
+// The clouds and outputs of clp_batch_correspondences(_dev): host arrays of nprob pointers (D1h, D2h, A_out; A_out[p]
+// filled with leading dimension m[p]) or device tensors in element strides (D1, D2, A_dev).
+struct KnnBatchIn {
+  const double* const* D1h = nullptr; const double* const* D2h = nullptr; int32_t* const* A_out = nullptr;
+  const double* D1 = nullptr; const int64_t* s1 = nullptr;
+  const double* D2 = nullptr; const int64_t* s2 = nullptr;
+  int32_t* A_dev = nullptr; const int64_t* sa = nullptr;
+};
+
+// clp_batch_correspondences(_dev).  Everything is checked on the host first; the device work is one upload (the table,
+// and the clouds of the host call), one staging launch (device call), the launches of clp_knn.cuh's batch section and
+// one readback of the counts.  Nothing of the batch but knn_buf, knn_pinned, its stream and its error string is touched.
+int batch_correspondences(clp_batch b, bool on_device, int32_t nprob, int32_t d, const KnnBatchIn& in, const int64_t* n1,
+                          const int64_t* n2, int32_t knn, double radius, int enforce_1to1, int64_t capacity, int64_t* m_out) {
+  if (!b) return CLP_ERR_INVALID;
+  const std::string who = "batch correspondences: ";
+  auto tag = [&](int p) { return who + "problem " + std::to_string(p) + ": "; };
+  if (!m_out || !n1 || !n2) return fail(b, CLP_ERR_INVALID, who + "n1, n2 and m are required");
+  if (nprob < 1) return fail(b, CLP_ERR_INVALID, who + "nprob must be >= 1");
+  std::fill(m_out, m_out + nprob, (int64_t)0);
+  if (on_device ? (!in.s1 || !in.s2 || !in.sa) : (!in.D1h || !in.D2h || !in.A_out))
+    return fail(b, CLP_ERR_INVALID, who + "NULL pointer arrays or strides");
+  if (knn < 1) return fail(b, CLP_ERR_INVALID, who + "knn must be >= 1");
+  if (d < 1) return fail(b, CLP_ERR_INVALID, who + "d must be >= 1");
+  for (int p = 0; p < nprob; ++p) {
+    if (n1[p] < 0 || n2[p] < 0) return fail(b, CLP_ERR_INVALID, tag(p) + "negative n1 or n2");
+    if ((n1[p] > 0 && !(on_device ? in.D1 : in.D1h[p])) || (n2[p] > 0 && !(on_device ? in.D2 : in.D2h[p])))
+      return fail(b, CLP_ERR_INVALID, tag(p) + "NULL point cloud");
+  }
+  if (on_device) {
+    auto ok = [](const int64_t* s) { return s[0] >= 0 && s[1] >= 1 && s[2] >= 1; };
+    if (!ok(in.s1) || !ok(in.s2) || !ok(in.sa))
+      return fail(b, CLP_ERR_INVALID, who + "bad strides (coordinate, point, row and column strides must be >= 1, batch "
+                                            "strides >= 0)");
+  }
+  if (knn > kKnnMaxK)
+    return fail(b, CLP_ERR_UNSUPPORTED, who + "knn = " + std::to_string(knn) + " exceeds CLP_KNN_MAX_K = " + std::to_string(kKnnMaxK));
+  if (d > kKnnMaxD)
+    return fail(b, CLP_ERR_UNSUPPORTED, who + "d = " + std::to_string(d) + " exceeds CLP_KNN_MAX_D = " + std::to_string(kKnnMaxD));
+  for (int p = 0; p < nprob; ++p)
+    if (n1[p] >= kKnnNone || n2[p] >= kKnnNone)
+      return fail(b, CLP_ERR_UNSUPPORTED, tag(p) + "n1 and n2 must be below 2^31 - 1 (int32 indices)");
+  for (int p = 0; p < nprob; ++p) {
+    const long long rows = (long long)n1[p] * std::min<int64_t>(knn, n2[p]);
+    if (capacity < rows || (rows > 0 && (on_device ? !in.A_dev : !in.A_out[p])))
+      return fail(b, CLP_ERR_INVALID, tag(p) + "A holds " + std::to_string(capacity) + " rows, n1 * min(knn, n2) = " +
+                                          std::to_string(rows) + " are required");
+  }
+  // the plan: a problem without rows (n1 = 0 or n2 = 0) takes no queries and no candidates
+  const int D = d <= 3 ? d : 0;
+  const int T = D > 0 ? kKnnTileReg : kKnnTileGen;
+  std::vector<KnnProb> tab((size_t)nprob);
+  long long nq = 0, nc = 0, ctas = 0, lsz = 0, rows_all = 0, max_nc = 0, most = 1;
+  int kmax = 1;
+  for (int p = 0; p < nprob; ++p) {
+    KnnProb& P = tab[(size_t)p];
+    std::memset(&P, 0, sizeof(P));
+    const int kk = (int)std::min<int64_t>(knn, n2[p]);
+    const bool live = (long long)n1[p] * kk > 0;
+    P.bp.n1 = live ? (int)n1[p] : 0; P.bp.n2 = live ? (int)n2[p] : 0; P.kk = live ? kk : 0;
+    P.bp.d1_off = (long long)d * nq; P.bp.d2_off = (long long)d * nc; P.bp.a_off = -1;
+    P.q_off = nq; P.c_off = nc; P.cta0 = ctas; P.m_off = lsz;
+    nq += P.bp.n1; nc += P.bp.n2; ctas += (P.bp.n1 + kKnnThreads - 1) / kKnnThreads; lsz += (long long)P.kk * P.bp.n1;
+    rows_all += (long long)P.kk * P.bp.n1;
+    max_nc = std::max<long long>(max_nc, P.bp.n2);
+    most = std::max<long long>(most, (long long)d * std::max(P.bp.n1, P.bp.n2));
+    kmax = std::max(kmax, P.kk);
+  }
+  if (rows_all == 0) return CLP_OK;
+  // candidate slices, as the single call cuts them but for the whole batch's query CTAs; bounds relative to each n2
+  const long long want = (4LL * b->sm_count + ctas - 1) / ctas;
+  const int nsplit = (int)std::max<long long>(1, std::min<long long>({want, (max_nc + 1023) / 1024, 1024}));
+  for (KnnProb& P : tab) {
+    P.chunk = round_up((P.bp.n2 + nsplit - 1) / nsplit, T);
+    P.l_off = (long long)nsplit * P.m_off;
+  }
+  int K = 1;
+  while (K < kmax) K *= 2;
+  // scratch layout, every region 256-byte aligned; the prefix table | d1 | d2 is uploaded from knn_pinned as it lies
+  const long long nscan = std::max(nq, nc), nb = (nscan + kKnnScanItems - 1) / kKnnScanItems;
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t o = at; at = (at + bytes + 255) & ~(size_t)255; return o; };
+  const size_t o_tab = take((size_t)nprob * sizeof(KnnProb));
+  const size_t o_d1 = take((size_t)d * nq * 8), o_d2 = take((size_t)d * nc * 8);
+  const size_t up = on_device ? (size_t)nprob * sizeof(KnnProb) : o_d2 + (size_t)d * nc * 8;
+  const size_t o_psd = take((size_t)nsplit * lsz * 8), o_pj = take((size_t)nsplit * lsz * 4);
+  const size_t o_lsd = nsplit > 1 ? take((size_t)lsz * 8) : o_psd, o_lj = nsplit > 1 ? take((size_t)lsz * 4) : o_pj;
+  const size_t o_cnt = take((size_t)nscan * 4), o_off = take((size_t)nscan * 8), o_bsum = take((size_t)nb * 8), o_tot = take(8);
+  const size_t o_m = take((size_t)nprob * 8), o_rb = take((size_t)nprob * 8);
+  const size_t o_best = enforce_1to1 ? take((size_t)nc * 8) : 0, o_c0 = enforce_1to1 ? take((size_t)nc * 4) : 0;
+  const size_t o_a = on_device ? 0 : take((size_t)2 * rows_all * 4);
+  CLP_CUDA(b, cudaSetDevice(b->device));
+  if (at > b->knn_buf.cap) {
+    size_t free_b = 0, total_b = 0;
+    CLP_CUDA(b, cudaMemGetInfo(&free_b, &total_b));
+    if (at > free_b + b->knn_buf.cap)
+      return fail(b, CLP_ERR_ALLOC, who + "the scratch (" + std::to_string(at) + " bytes) does not fit the free device memory (" +
+                                        std::to_string(free_b + b->knn_buf.cap) + " bytes)");
+  }
+  CLP_CUDA(b, b->knn_buf.ensure(at));
+  const size_t o_hm = (up + 255) & ~(size_t)255;  // the counts come back here
+  CLP_CUDA(b, b->knn_pinned.ensure(o_hm + (size_t)nprob * 8));
+  char* hp = b->knn_pinned.as<char>();
+  std::memcpy(hp + o_tab, tab.data(), (size_t)nprob * sizeof(KnnProb));
+  if (!on_device)
+    for (int p = 0; p < nprob; ++p) {
+      const KnnProb& P = tab[(size_t)p];
+      if (P.bp.n1) std::memcpy(hp + o_d1 + (size_t)P.bp.d1_off * 8, in.D1h[p], (size_t)d * P.bp.n1 * 8);
+      if (P.bp.n2) std::memcpy(hp + o_d2 + (size_t)P.bp.d2_off * 8, in.D2h[p], (size_t)d * P.bp.n2 * 8);
+    }
+  const cudaStream_t st = b->stream;
+  char* base = b->knn_buf.as<char>();
+  CLP_CUDA(b, cudaMemcpyAsync(base, hp, up, cudaMemcpyHostToDevice, st));
+  KnnBatchArgs a;
+  std::memset(&a, 0, sizeof(a));
+  a.prob = reinterpret_cast<const KnnProb*>(base + o_tab); a.nprob = nprob; a.d = d; a.nsplit = nsplit;
+  a.D1 = reinterpret_cast<const double*>(base + o_d1); a.D2 = reinterpret_cast<const double*>(base + o_d2);
+  a.part_sd = reinterpret_cast<double*>(base + o_psd); a.part_j = reinterpret_cast<int*>(base + o_pj);
+  a.lsd = reinterpret_cast<double*>(base + o_lsd); a.lj = reinterpret_cast<int*>(base + o_lj);
+  a.r2 = radius * radius;  // bm_utils.cpp:192: NaN keeps nothing, inf keeps every neighbour
+  a.cnt = reinterpret_cast<int*>(base + o_cnt); a.off = reinterpret_cast<long long*>(base + o_off);
+  a.bsum = reinterpret_cast<long long*>(base + o_bsum); a.total = reinterpret_cast<long long*>(base + o_tot);
+  a.mcount = reinterpret_cast<long long*>(base + o_m); a.rbase = reinterpret_cast<long long*>(base + o_rb);
+  a.best = reinterpret_cast<unsigned long long*>(base + o_best); a.c0best = reinterpret_cast<unsigned int*>(base + o_c0);
+  if (on_device) {
+    a.A = in.A_dev;
+    for (int k = 0; k < 3; ++k) a.as[k] = in.sa[k];
+    BatchStageArgs g;
+    std::memset(&g, 0, sizeof(g));
+    g.prob = reinterpret_cast<const unsigned char*>(base + o_tab); g.prob_stride = sizeof(KnnProb);
+    g.nprob = nprob; g.dd = d;
+    g.D1 = in.D1; g.D2 = in.D2;
+    for (int k = 0; k < 3; ++k) { g.s1[k] = in.s1[k]; g.s2[k] = in.s2[k]; }
+    g.d1 = reinterpret_cast<double*>(base + o_d1); g.d2 = reinterpret_cast<double*>(base + o_d2);
+    g.bad = &b->sync.as<SyncBlock>()->counts[1];  // never written: the table holds no associations
+    const dim3 grid((unsigned)std::min<long long>(64, (most + kBatchThreads - 1) / kBatchThreads), (unsigned)std::min(nprob, 65535));
+    batch_stage_points_kernel<<<grid, kBatchThreads, 0, st>>>(g);
+    CLP_CUDA(b, cudaGetLastError());
+  } else {
+    a.A = reinterpret_cast<int*>(base + o_a);
+    a.packed = 1;
+  }
+  const dim3 pgrid((unsigned)ctas, (unsigned)nsplit);
+  const size_t smem = knn_partial_smem(D, d);
+  cudaError_t e;
+  switch (D) {
+    case 1: e = knn_batch_partial_k<1>(K, pgrid, smem, st, a); break;
+    case 2: e = knn_batch_partial_k<2>(K, pgrid, smem, st, a); break;
+    case 3: e = knn_batch_partial_k<3>(K, pgrid, smem, st, a); break;
+    default: e = knn_batch_partial_k<0>(K, pgrid, smem, st, a); break;
+  }
+  CLP_CUDA(b, e);
+  CLP_CUDA(b, knn_batch_merge(K, (unsigned)ctas, st, a));
+  const unsigned bp = (unsigned)((nprob + 255) / 256);
+  if (!enforce_1to1) {
+    a.nscan = nq;
+    knn_scan_blocks_kernel<<<(unsigned)((nq + kKnnScanItems - 1) / kKnnScanItems), 256, 0, st>>>(a.cnt, nq, a.off, a.bsum);
+    knn_scan_top_kernel<<<1, 1024, 0, st>>>(a.bsum, (nq + kKnnScanItems - 1) / kKnnScanItems, a.total);
+    knn_batch_rows_kernel<<<bp, 256, 0, st>>>(a, 0);
+    knn_batch_write_kernel<<<(unsigned)ctas, kKnnThreads, 0, st>>>(a);
+  } else {
+    CLP_CUDA(b, cudaMemsetAsync(a.best, 0xff, (size_t)nc * 8, st));
+    CLP_CUDA(b, cudaMemsetAsync(a.c0best, 0xff, (size_t)nc * 4, st));
+    knn_batch_best_sd_kernel<<<(unsigned)ctas, kKnnThreads, 0, st>>>(a);
+    knn_batch_best_c0_kernel<<<(unsigned)ctas, kKnnThreads, 0, st>>>(a);
+    const unsigned b2 = (unsigned)((nc + 255) / 256);
+    knn_flag_kernel<<<b2, 256, 0, st>>>(a.c0best, nc, a.cnt);
+    a.nscan = nc;
+    knn_scan_blocks_kernel<<<(unsigned)((nc + kKnnScanItems - 1) / kKnnScanItems), 256, 0, st>>>(a.cnt, nc, a.off, a.bsum);
+    knn_scan_top_kernel<<<1, 1024, 0, st>>>(a.bsum, (nc + kKnnScanItems - 1) / kKnnScanItems, a.total);
+    knn_batch_rows_kernel<<<bp, 256, 0, st>>>(a, 1);
+    knn_batch_write_1to1_kernel<<<b2, 256, 0, st>>>(a);
+  }
+  CLP_CUDA(b, cudaGetLastError());
+  long long* h_m = reinterpret_cast<long long*>(hp + o_hm);
+  CLP_CUDA(b, cudaMemcpyAsync(h_m, a.mcount, (size_t)nprob * 8, cudaMemcpyDeviceToHost, st));
+  CLP_CUDA(b, cudaStreamSynchronize(st));
+  const std::vector<long long> ms(h_m, h_m + nprob);
+  long long M = 0;
+  for (long long x : ms) M += x;
+  if (!on_device && M > 0) {  // the staged rows of problem p start at 2 (m[0] + .. + m[p - 1])
+    CLP_CUDA(b, b->knn_pinned.ensure((size_t)2 * M * 4));
+    int32_t* h_a = b->knn_pinned.as<int32_t>();
+    CLP_CUDA(b, cudaMemcpyAsync(h_a, a.A, (size_t)2 * M * 4, cudaMemcpyDeviceToHost, st));
+    CLP_CUDA(b, cudaStreamSynchronize(st));
+    long long r0 = 0;
+    for (int p = 0; p < nprob; ++p) {
+      if (ms[(size_t)p] > 0) std::memcpy(in.A_out[p], h_a + 2 * r0, (size_t)2 * ms[(size_t)p] * 4);
+      r0 += ms[(size_t)p];
+    }
+  }
+  std::copy(ms.begin(), ms.end(), m_out);
+  return CLP_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -3324,9 +3557,10 @@ int clp_batch_destroy(clp_batch b) {
   cudaSetDevice(b->device);
   for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in, &b->custom_in,
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
-                    &b->mc_pscratch, &b->mc_sscratch, &b->sdp_out})
+                    &b->mc_pscratch, &b->mc_sscratch, &b->sdp_out, &b->knn_buf})
     d->release();
   b->pinned.release();
+  b->knn_pinned.release();
   b->pinned_points.release();
   if (b->ev0) cudaEventDestroy(b->ev0);
   if (b->ev1) cudaEventDestroy(b->ev1);
@@ -3529,6 +3763,23 @@ int clp_batch_max_clique_custom_dev(clp_batch b, const char* source, const doubl
     in.inv = &inv;
     return batch_max_clique(b, kBatchKindCustom, d, nprob, in, method, time_limit_s, infos, nodes_out, core_out);
   });
+}
+
+int clp_batch_correspondences(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                              const double* const* D2, const int64_t* n2, int32_t knn, double radius, int enforce_1to1,
+                              int32_t* const* A_out, int64_t capacity, int64_t* m) {
+  KnnBatchIn in;
+  in.D1h = D1; in.D2h = D2; in.A_out = A_out;
+  return guarded(b, [&] { return batch_correspondences(b, false, nprob, d, in, n1, n2, knn, radius, enforce_1to1, capacity, m); });
+}
+
+int clp_batch_correspondences_dev(clp_batch b, int32_t nprob, int32_t d, const double* D1_dev, const int64_t d1_strides[3],
+                                  const int64_t* n1, const double* D2_dev, const int64_t d2_strides[3], const int64_t* n2,
+                                  int32_t knn, double radius, int enforce_1to1, int32_t* A_dev, const int64_t a_strides[3],
+                                  int64_t capacity, int64_t* m) {
+  KnnBatchIn in;
+  in.D1 = D1_dev; in.s1 = d1_strides; in.D2 = D2_dev; in.s2 = d2_strides; in.A_dev = A_dev; in.sa = a_strides;
+  return guarded(b, [&] { return batch_correspondences(b, true, nprob, d, in, n1, n2, knn, radius, enforce_1to1, capacity, m); });
 }
 
 }  // extern "C"

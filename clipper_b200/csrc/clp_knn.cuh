@@ -70,30 +70,29 @@ __device__ __forceinline__ void knn_clear(double (&sd)[K], int (&jj)[K]) {
   for (int t = 0; t < K; ++t) { sd[t] = __longlong_as_double(0x7ff0000000000000LL); jj[t] = kKnnNone; }
 }
 
+// The running top-K (sd, jj) of query i of D1 over the candidates [lo, hi) of D2 (indices relative to D2), tiles of D2
+// staged in shared memory.  Every thread of the CTA calls it with the same lo, hi and d (the barriers are the CTA's);
+// live: i is a query (a thread past the last one stages tiles and keeps an empty list).
 template <int D, int K>
-__global__ void __launch_bounds__(kKnnThreads) knn_partial_kernel(KnnArgs a) {
+__device__ __forceinline__ void knn_scan_candidates(const double* D1, const double* D2, int d_rt, long long i, bool live,
+                                                    long long lo, long long hi, double (&sd)[K], int (&jj)[K]) {
   extern __shared__ double knn_smem[];
   constexpr int T = D > 0 ? kKnnTileReg : kKnnTileGen;
-  const int d = D > 0 ? D : a.d;
+  const int d = D > 0 ? D : d_rt;
   double* tile = knn_smem;                   // T candidates x d, as they lie in D2
   double* qs = knn_smem + (size_t)T * d;     // D = 0: the queries, coordinate-major (d x kKnnThreads)
-  const long long i = (long long)blockIdx.x * kKnnThreads + threadIdx.x;
-  const bool live = i < a.n1;
   double q[D > 0 ? D : 1];
   if constexpr (D > 0) {
 #pragma unroll
-    for (int k = 0; k < D; ++k) q[k] = live ? a.D1[i * D + k] : 0.0;
+    for (int k = 0; k < D; ++k) q[k] = live ? D1[i * D + k] : 0.0;
   } else {
-    for (int k = 0; k < d; ++k) qs[k * kKnnThreads + threadIdx.x] = live ? a.D1[i * d + k] : 0.0;
+    for (int k = 0; k < d; ++k) qs[k * kKnnThreads + threadIdx.x] = live ? D1[i * d + k] : 0.0;
   }
-  double sd[K]; int jj[K];
   knn_clear<K>(sd, jj);
-  const long long lo = (long long)blockIdx.y * a.chunk;
-  const long long hi = lo + a.chunk < a.n2 ? lo + a.chunk : a.n2;
   for (long long c0 = lo; c0 < hi; c0 += T) {
     const int cnt = (int)(hi - c0 < T ? hi - c0 : T);
     __syncthreads();  // the previous tile is consumed
-    const double* src = a.D2 + c0 * d;
+    const double* src = D2 + c0 * d;
     for (int e = threadIdx.x; e < cnt * d; e += kKnnThreads) tile[e] = src[e];
     __syncthreads();
     if (!live) continue;
@@ -116,6 +115,16 @@ __global__ void __launch_bounds__(kKnnThreads) knn_partial_kernel(KnnArgs a) {
       knn_insert<K>(sd, jj, s, (int)(c0 + c));
     }
   }
+}
+
+template <int D, int K>
+__global__ void __launch_bounds__(kKnnThreads) knn_partial_kernel(KnnArgs a) {
+  const long long i = (long long)blockIdx.x * kKnnThreads + threadIdx.x;
+  const bool live = i < a.n1;
+  const long long lo = (long long)blockIdx.y * a.chunk;
+  const long long hi = lo + a.chunk < a.n2 ? lo + a.chunk : a.n2;
+  double sd[K]; int jj[K];
+  knn_scan_candidates<D, K>(a.D1, a.D2, a.d, i, live, lo, hi, sd, jj);
   if (!live) return;
 #pragma unroll
   for (int t = 0; t < K; ++t)
@@ -254,6 +263,192 @@ __global__ void __launch_bounds__(256) knn_write_1to1_kernel(const unsigned int*
   const long long m = *total;
   const long long row = off[j] + bsum[j / kKnnScanItems];
   A[row] = (int)c0best[j]; A[m + row] = (int)j;
+}
+
+// ---- batches of cloud pairs (clp_batch_correspondences(_dev)) -------------------------------------------------------
+// Problem p is the single call on (D1_p, D2_p), bit for bit.  The clouds are concatenated: query i of p is q_off + i of
+// one query index space, candidate j of p is c_off + j of one candidate index space (the staged clouds at d * q_off
+// and d * c_off).  The steps are those of the single call, each one launch for the whole batch:
+//   1. knn_batch_partial_kernel<D, K>: the query CTAs of all problems one after the other along x (problem p owns
+//      CTAs [cta0, cta0 + ceil(n1 / kKnnThreads))), a candidate slice along y; slice s of p is [s * chunk, (s + 1) *
+//      chunk) of its own candidates, chunk = round_up(ceil(n2 / nsplit), tile).  K covers the largest kk of the batch;
+//      each problem writes its own kk entries per query and slice.
+//   2. knn_batch_merge_kernel<K>: the slices' lists of every query merged, cnt[q_off + i] = its kept pairs.
+//   3. one exclusive scan of cnt over the whole query space (knn_scan_blocks_kernel + knn_scan_top_kernel).
+//   4. knn_batch_rows_kernel: m[p] = scan(end of p) - scan(start of p) and rbase[p] = scan(start of p).
+//   5. knn_batch_write_kernel: row off[q] - rbase[p] of problem p.
+//   1-to-1: the atomicMin passes on the concatenated candidate space (64-bit offsets), the flags, the scan, the counts
+//   and the rows the same way, by c1.
+// A problem's result depends on nothing but its own clouds: the order of the lists is total, so neither the slicing
+// nor the batch around a problem changes it.
+struct KnnProb {
+  BatchProblem bp;          // d1_off = d q_off, d2_off = d c_off, n1, n2 (0 for a problem with no rows), a_off = -1:
+                            // the entry batch_stage_points_kernel reads
+  long long q_off, c_off;   // first query / candidate in the concatenated index spaces
+  long long cta0;           // first query CTA
+  long long l_off, m_off;   // partial lists [nsplit][kk][n1] at l_off, merged lists [kk][n1] at m_off
+  long long chunk;          // candidates per slice
+  int kk, pad_;
+};
+
+struct KnnBatchArgs {
+  const KnnProb* prob; int nprob;
+  int d, nsplit;
+  const double* D1; const double* D2;   // staged clouds
+  double* part_sd; int* part_j;         // partial lists
+  double* lsd; int* lj;                 // merged lists (the partial ones when nsplit = 1)
+  double r2;
+  int* cnt; long long* off; long long* bsum; long long* total; long long nscan;  // the scan and its length
+  long long* mcount; long long* rbase;  // per problem: m and the scan at its first query (candidate for 1-to-1)
+  unsigned long long* best; unsigned int* c0best;  // 1-to-1, per concatenated candidate
+  int* A; long long as[3];              // entry (r, c) of problem p at A[p as[0] + r as[1] + c as[2]]
+  int packed;                           // 1: at A[2 rbase[p] + r + c m[p]] instead (the host call's staging)
+};
+
+// the problem whose range [start, next start) holds x, for starts cta0 (F = 0), q_off (F = 1) or c_off (F = 2): the
+// last one whose start is <= x (problems with empty ranges share their start with the next one)
+template <int F>
+__device__ __forceinline__ int knn_problem(const KnnProb* t, int nprob, long long x) {
+  int lo = 0, hi = nprob - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    const long long s = F == 0 ? t[mid].cta0 : F == 1 ? t[mid].q_off : t[mid].c_off;
+    if (s <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+template <int D, int K>
+__global__ void __launch_bounds__(kKnnThreads, 4) knn_batch_partial_kernel(KnnBatchArgs a) {
+  const KnnProb* P = a.prob + knn_problem<0>(a.prob, a.nprob, blockIdx.x);
+  const long long n1 = P->bp.n1, n2 = P->bp.n2;
+  const long long i = ((long long)blockIdx.x - P->cta0) * kKnnThreads + threadIdx.x;
+  const bool live = i < n1;
+  const long long lo = (long long)blockIdx.y * P->chunk;
+  const long long hi = lo + P->chunk < n2 ? lo + P->chunk : n2;
+  double sd[K]; int jj[K];
+  knn_scan_candidates<D, K>(a.D1 + P->q_off * (D > 0 ? D : a.d), a.D2 + P->c_off * (D > 0 ? D : a.d), a.d, i, live, lo,
+                            hi, sd, jj);
+  if (!live) return;
+  const long long l_off = P->l_off;  // read after the scan: fewer registers live across it
+  const int kk = P->kk;
+#pragma unroll
+  for (int t = 0; t < K; ++t)
+    if (t < kk) {
+      const size_t o = l_off + ((size_t)blockIdx.y * kk + t) * n1 + i;
+      a.part_sd[o] = sd[t]; a.part_j[o] = jj[t];
+    }
+}
+
+// the query of this thread in the grid of knn_batch_partial_kernel (x only): its problem (returned; -1 past the
+// problem's last query), the problem's entry and the local index
+__device__ __forceinline__ int knn_batch_query(const KnnBatchArgs& a, KnnProb& P, long long& i) {
+  const int p = knn_problem<0>(a.prob, a.nprob, blockIdx.x);
+  P = a.prob[p];
+  i = ((long long)blockIdx.x - P.cta0) * kKnnThreads + threadIdx.x;
+  return i < P.bp.n1 ? p : -1;
+}
+
+template <int K>
+__global__ void __launch_bounds__(kKnnThreads) knn_batch_merge_kernel(KnnBatchArgs a) {
+  KnnProb P; long long i;
+  if (knn_batch_query(a, P, i) < 0) return;
+  const long long n1 = P.bp.n1;
+  const int kk = P.kk;
+  if (a.nsplit == 1) {
+    int c = 0;
+    for (int t = 0; t < kk; ++t) {
+      const size_t o = P.m_off + (size_t)t * n1 + i;
+      if (a.lj[o] == kKnnNone || !(a.lsd[o] <= a.r2)) break;
+      ++c;
+    }
+    a.cnt[P.q_off + i] = c;
+    return;
+  }
+  double sd[K]; int jj[K];
+  knn_clear<K>(sd, jj);
+  for (int s = 0; s < a.nsplit; ++s)
+    for (int t = 0; t < kk; ++t) {
+      const size_t o = P.l_off + ((size_t)s * kk + t) * n1 + i;
+      if (!knn_insert<K>(sd, jj, a.part_sd[o], a.part_j[o])) break;  // the rest of this sorted list is worse
+    }
+  int c = 0;
+#pragma unroll
+  for (int t = 0; t < K; ++t)
+    if (t < kk) {
+      const size_t o = P.m_off + (size_t)t * n1 + i;
+      a.lsd[o] = sd[t]; a.lj[o] = jj[t];
+      c += (jj[t] != kKnnNone && sd[t] <= a.r2) ? 1 : 0;
+    }
+  a.cnt[P.q_off + i] = c;
+}
+
+// the exclusive scan at x of the scanned space (its total at the end)
+__device__ __forceinline__ long long knn_scan_at(const KnnBatchArgs& a, long long x) {
+  return x < a.nscan ? a.off[x] + a.bsum[x / kKnnScanItems] : *a.total;
+}
+
+// one thread per problem: m[p] and the scan at its first query (by_c1 = 0) or candidate (by_c1 = 1)
+__global__ void __launch_bounds__(256) knn_batch_rows_kernel(KnnBatchArgs a, int by_c1) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.nprob) return;
+  const KnnProb& P = a.prob[p];
+  const long long x0 = by_c1 ? P.c_off : P.q_off, x1 = x0 + (by_c1 ? P.bp.n2 : P.bp.n1);
+  const long long r0 = knn_scan_at(a, x0);
+  a.rbase[p] = r0;
+  a.mcount[p] = knn_scan_at(a, x1) - r0;
+}
+
+// the address of entry (r, c) of problem p
+__device__ __forceinline__ long long knn_batch_at(const KnnBatchArgs& a, int p, long long r, int c) {
+  return a.packed ? 2 * a.rbase[p] + r + c * a.mcount[p] : p * a.as[0] + r * a.as[1] + c * a.as[2];
+}
+
+__global__ void __launch_bounds__(kKnnThreads) knn_batch_write_kernel(KnnBatchArgs a) {
+  KnnProb P; long long i;
+  const int p = knn_batch_query(a, P, i);
+  if (p < 0) return;
+  const long long q = P.q_off + i;
+  const long long row = knn_scan_at(a, q) - a.rbase[p];
+  const int c = a.cnt[q];
+  for (int r = 0; r < c; ++r) {
+    a.A[knn_batch_at(a, p, row + r, 0)] = (int)i;
+    a.A[knn_batch_at(a, p, row + r, 1)] = a.lj[P.m_off + (size_t)r * P.bp.n1 + i];
+  }
+}
+
+// 1-to-1, first pass: the least sd (as bits) of the kept pairs of every c1 of the concatenated candidate space
+__global__ void __launch_bounds__(kKnnThreads) knn_batch_best_sd_kernel(KnnBatchArgs a) {
+  KnnProb P; long long i;
+  if (knn_batch_query(a, P, i) < 0) return;
+  const int c = a.cnt[P.q_off + i];
+  for (int r = 0; r < c; ++r) {
+    const size_t o = P.m_off + (size_t)r * P.bp.n1 + i;
+    atomicMin(&a.best[P.c_off + a.lj[o]], (unsigned long long)__double_as_longlong(a.lsd[o]));
+  }
+}
+
+// second pass: the least c0 among the kept pairs of c1 whose sd equals that least one
+__global__ void __launch_bounds__(kKnnThreads) knn_batch_best_c0_kernel(KnnBatchArgs a) {
+  KnnProb P; long long i;
+  if (knn_batch_query(a, P, i) < 0) return;
+  const int c = a.cnt[P.q_off + i];
+  for (int r = 0; r < c; ++r) {
+    const size_t o = P.m_off + (size_t)r * P.bp.n1 + i;
+    const long long g = P.c_off + a.lj[o];
+    if ((unsigned long long)__double_as_longlong(a.lsd[o]) == a.best[g]) atomicMin(&a.c0best[g], (unsigned int)i);
+  }
+}
+
+// one row for every c1 that has a kept pair: the flags over the concatenated candidates (knn_flag_kernel), the scan,
+// knn_batch_rows_kernel(by_c1 = 1), then the rows
+__global__ void __launch_bounds__(256) knn_batch_write_1to1_kernel(KnnBatchArgs a) {
+  const long long g = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= a.nscan || a.c0best[g] == 0xffffffffu) return;
+  const int p = knn_problem<2>(a.prob, a.nprob, g);
+  const long long row = knn_scan_at(a, g) - a.rbase[p];
+  a.A[knn_batch_at(a, p, row, 0)] = (int)a.c0best[g];
+  a.A[knn_batch_at(a, p, row, 1)] = (int)(g - a.prob[p].c_off);
 }
 
 }  // namespace clp

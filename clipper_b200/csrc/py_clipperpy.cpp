@@ -166,6 +166,20 @@ void pybind_correspondences(py::module& m)
         },
         "D1"_a, "D2"_a, "knn"_a, "radius"_a, "enforce_1to1"_a,
         "Associations (m, 2) int32: every column of D1 (d x n1) to its knn nearest columns of D2 within radius, on the GPU.");
+  m.def("distance_based_correspondences_many",
+        [](const std::vector<py::array>& D1s, const std::vector<py::array>& D2s, size_t knn, double radius,
+           bool enforce_1to1) {
+          std::vector<clipper::invariants::Data> M1, M2;
+          for (const py::array& a : D1s) M1.push_back(to_matrix(a, "D1s"));
+          for (const py::array& a : D2s) M2.push_back(to_matrix(a, "D2s"));
+          py::list out;
+          for (const clipper::Association& A : clipper::utils::distanceBasedCorrespondencesBatch(M1, M2, knn, radius, enforce_1to1))
+            out.append(from_assoc(A));
+          return out;
+        },
+        "D1s"_a, "D2s"_a, "knn"_a, "radius"_a, "enforce_1to1"_a,
+        "distance_based_correspondences of every pair (D1s[p], D2s[p]) in one batched call on the GPU: a list of (m, 2) "
+        "int32 arrays.");
 }
 
 void pybind_dsd(py::module& m)

@@ -48,6 +48,16 @@ namespace utils {
   Association distanceBasedCorrespondences(const invariants::Data& D1, const invariants::Data& D2, size_t knn,
                                            double radius, bool enforce1to1);
 
+  /**
+   * @brief distanceBasedCorrespondences of many cloud pairs in one batched call on the GPU (device 0, a temporary
+   * clp_batch; clp_batch_correspondences).  Entry p of the result is exactly distanceBasedCorrespondences(D1s[p],
+   * D2s[p], knn, radius, enforce1to1).  D1s and D2s have the same length and every cloud the same number of rows; an
+   * empty list gives an empty result.
+   */
+  std::vector<Association> distanceBasedCorrespondencesBatch(const std::vector<invariants::Data>& D1s,
+                                                             const std::vector<invariants::Data>& D2s, size_t knn,
+                                                             double radius, bool enforce1to1);
+
   /// simple named profiling timer (utils.h:107-163)
   class Timer
   {

@@ -468,6 +468,36 @@ int clp_batch_max_clique_custom_dev(clp_batch b, const char* source, const doubl
                                     int32_t d, const clp_points_dev* pts, int method, double time_limit_s,
                                     clp_mc_info* infos, int32_t* const* nodes_out, int32_t* const* core_out);
 
+/* ---- putative associations for a batch of cloud pairs (the batched form of clp_correspondences) --------------------
+ * Problem p gets exactly what clp_correspondences gives for (D1_p, n1[p], D2_p, n2[p]) with the call's d, knn, radius
+ * and enforce_1to1: the same m[p], the same rows in the same order, bit for bit.  A problem's result depends on nothing
+ * else: not on the other problems, nprob or p, and not on anything past n1[p] and n2[p] (NaN or garbage included).
+ * n1[p] = 0 or n2[p] = 0 gives m[p] = 0.  n1, n2 and m are host arrays of nprob; the call returns when m is on the host.
+ * clp_batch_correspondences: D1[p] (d x n1[p]) and D2[p] (d x n2[p]) are column-major host arrays; A_out[p] holds
+ *   capacity rows and receives problem p's as clp_correspondences fills it (c0 in A_out[p][0 .. m[p]), c1 in
+ *   A_out[p][m[p] .. 2 m[p])); A_out[p] may be NULL when n1[p] * min(knn, n2[p]) = 0.
+ * clp_batch_correspondences_dev: the clouds on the batch's device in the element strides of clp_points_dev (coordinate
+ *   k of point j of problem p at D1_dev[p d1_strides[0] + k d1_strides[1] + j d1_strides[2]], D2 alike; a batch stride
+ *   may be 0: one cloud for every problem); entry (r, c) of problem p is written at A_dev[p a_strides[0] +
+ *   r a_strides[1] + c a_strides[2]] for r < m[p] (rows m[p] .. capacity - 1 are left as they were).  With strides
+ *   (2 cap, 1, cap) this is a (nprob, cap, 2) tensor that clp_batch_*_dev take as their associations.
+ * The batch's device, stream (clp_batch_set_stream) and error string are used, and its own kNN scratch; its other state
+ * stays as it was.  The device work is a fixed number of launches whatever nprob, and one synchronisation.
+ * Errors, checked on the host before anything is uploaded, in this order, naming the first failing problem:
+ *   CLP_ERR_INVALID for NULL pointers (a cloud may be NULL when every problem's size for it is 0), nprob < 1, knn < 1, d < 1, a negative size or bad strides (coordinate, point,
+ *   row and column strides >= 1, batch strides >= 0); CLP_ERR_UNSUPPORTED for knn > CLP_KNN_MAX_K, d > CLP_KNN_MAX_D or
+ *   a size >= 2^31 - 1; CLP_ERR_INVALID for capacity < n1[p] * min(knn, n2[p]); CLP_ERR_ALLOC when the scratch does not
+ *   fit the free device memory.  m is all zero after an error; the batch stays usable.
+ * Handing A and m to clp_batch_*_dev: there m[p] = 0 means the all-to-all hypothesis, so a problem without rows must be
+ * left out, and m[p] > 4096 is refused. */
+int clp_batch_correspondences(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                              const double* const* D2, const int64_t* n2, int32_t knn, double radius, int enforce_1to1,
+                              int32_t* const* A_out, int64_t capacity, int64_t* m);
+int clp_batch_correspondences_dev(clp_batch b, int32_t nprob, int32_t d, const double* D1_dev, const int64_t d1_strides[3],
+                                  const int64_t* n1, const double* D2_dev, const int64_t d2_strides[3], const int64_t* n2,
+                                  int32_t knn, double radius, int enforce_1to1, int32_t* A_dev, const int64_t a_strides[3],
+                                  int64_t capacity, int64_t* m);
+
 /* ---- semidefinite relaxation (solveAsMSRCSDR / sdp::solve, ref clipper.cpp:101-113, sdp.cpp:88-296) ---------------
  * Solves  maximise <M, X>  subject to  X PSD, tr X = 1, X_ij = 0 where C_ij = 0, X_ij >= 0 where C_ij != 0  on the
  * device by two-block ADMM (X in the spectraplex, Z in the polyhedral set), with a Jacobi eigensolver in shared memory
