@@ -26,6 +26,7 @@ SYMBOLS = [
     "clp_k2ij", "clp_create_all_to_all", "clp_find_k_largest", "clp_find_above", "clp_dsd_dense",
     "clp_shard_config", "clp_shard_rows", "clp_shard_export", "clp_shard_import", "clp_shard_blob_bytes",
     "clp_set_ctas_per_sm", "clp_set_grid_cap", "clp_set_dense_mode", "clp_get_dense_mode", "clp_sparse_info",
+    "clp_last_solve_sweeps",
     "clp_batch_create", "clp_batch_destroy", "clp_batch_last_error", "clp_batch_set_params",
     "clp_batch_solve_euclidean", "clp_batch_solve_pointnormal", "clp_batch_info",
     "clp_max_clique", "clp_core_numbers",
@@ -168,6 +169,7 @@ def load():
     L.clp_set_dense_mode.argtypes = [vp, C.c_int]
     L.clp_get_dense_mode.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.clp_sparse_info.argtypes = [vp, lp, lp]
+    L.clp_last_solve_sweeps.argtypes = [vp, lp]
     # batches of small problems: arrays of host pointers (void**) and sizes
     pp = C.POINTER(C.c_void_p)
     L.clp_batch_create.argtypes = [C.c_int, C.POINTER(vp)]

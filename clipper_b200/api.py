@@ -651,6 +651,14 @@ class CLIPPER:
         _capi.check(self._h, self._lib.clp_sparse_info(self._h, C.byref(a), C.byref(b)))
         return int(a.value), int(b.value)
 
+    def last_solve_sweeps(self):
+        """how the line-search evaluations of the last solve read the matrix (clp_last_solve_sweeps): evaluations that
+        swept the whole compact copy, rebuilt the restricted copy, swept only the restricted copy; entries and padding
+        entries the restricted sweeps read; full sweeps after the first rebuild"""
+        a = (C.c_int64 * 6)()
+        _capi.check(self._h, self._lib.clp_last_solve_sweeps(self._h, a))
+        return dict(zip(("full", "rebuild", "restricted", "entries", "padding", "fallback"), (int(x) for x in a)))
+
     def _sync_params(self):
         _capi.check(self._h, self._lib.clp_set_params(self._h, C.byref(self._params._pod())))
 

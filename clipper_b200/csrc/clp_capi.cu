@@ -132,6 +132,7 @@ struct clp_handle_s {
   int res_G = 0;                                    // CTAs of the resident kernels for the current matrix
   int res_NI = 0;
   int smem_optin = 0;                               // cudaDevAttrMaxSharedMemoryPerBlockOptin
+  int l2_bytes = 0;                                 // cudaDevAttrL2CacheSize
   int pack = env_int("CLP_PACK", 1);              // resident layout of plain fp32 matrices with 4-byte entries (0: always 6 bytes)
 
   // solver workspace
@@ -158,6 +159,11 @@ struct clp_handle_s {
   DevBuf sp_val, sp_col, sp_ptr4, sp_part, sp_item, sp_rowid;  // sp_ptr4: kept entries per (segment, row)
   DevBuf sp_hist, sp_bsum;  // compact build: class histograms of the row tiles | block sums of the scans
   DevBuf sp_win, res_wcol;  // packed layout: occupied 16-column windows per row | members' columns where every warp starts
+  // packed layout on one GPU: the resident solver's restricted copy (values | columns | slot offsets | row lengths | S' of
+  // every CTA | row products), sized once per build for the largest S' that can be taken
+  DevBuf res_rval, res_rcol, res_roff, res_rlen, res_rbits, res_rprod;
+  bool res_restrict = false;
+  ResSweeps last_sweeps{};  // sweep counters of the last solve
   unsigned long long sp_nnz = 0, sp_nnz_real = 0;
   CompactShape sp_shape{};  // layout of the last compact copy built
   SparseView sp{};
@@ -359,7 +365,8 @@ ResKernels res_kernels(clp_handle h) {
   using S = ResShape<T, false>;
   if constexpr (sizeof(T) == 4)
     if (h->sp.packed)
-      return {(const void*)solver_resident_kernel<T, false, true>, (const void*)matvec_resident_kernel<T, S, true>, S::NT};
+      return {h->res_restrict ? (const void*)solver_resident_kernel<T, false, true, true> : (const void*)solver_resident_kernel<T, false, true>,
+              (const void*)matvec_resident_kernel<T, S, true>, S::NT};
   return {(const void*)solver_resident_kernel<T, false>, (const void*)matvec_resident_kernel<T, S>, S::NT};
 }
 int res_warps(clp_handle h) {
@@ -402,9 +409,9 @@ CompactShape compact_shape(clp_handle h) {
 
 template <typename T>
 cudaError_t res_set_attrs(clp_handle h) {
-  // [storage][sharded][packed][device]: set once per process (handles may live on different host threads)
-  static std::atomic<bool> done[2][2][2][8];
-  std::atomic<bool>& flag = done[sizeof(T) == 8 ? 1 : 0][h->world > 1 ? 1 : 0][h->sp.packed ? 1 : 0][h->device & 7];
+  // [storage][sharded][packed][restricted][device]: set once per process (handles may live on different host threads)
+  static std::atomic<bool> done[2][2][2][2][8];
+  std::atomic<bool>& flag = done[sizeof(T) == 8 ? 1 : 0][h->world > 1 ? 1 : 0][h->sp.packed ? 1 : 0][h->res_restrict ? 1 : 0][h->device & 7];
   if (flag.load(std::memory_order_acquire)) return cudaSuccess;
   // the attribute is a per-function PERMISSION shared by every handle of the process (two shards in one process ask
   // for different sizes): always the device maximum; the carve-out follows what each launch actually requests
@@ -414,6 +421,10 @@ cudaError_t res_set_attrs(clp_handle h) {
   if (rc == cudaSuccess) flag.store(true, std::memory_order_release);
   return rc;
 }
+
+// the result buffer's 256-byte header: SolverOut, then the resident solver's sweep counters
+constexpr size_t kSweepsAt = 128;
+static_assert(sizeof(SolverOut) <= kSweepsAt && kSweepsAt + sizeof(ResSweeps) <= 256, "result header layout");
 
 ResArgs res_args(clp_handle h) {
   ResArgs a;
@@ -439,6 +450,11 @@ ResArgs res_args(clp_handle h) {
   a.prof_cta = h->prof_ctas ? h->prof_buf.as<double>() : nullptr;
   a.prof_laps = (h->prof_ctas || h->prof_laps) ? 1 : 0;
   a.wcol = h->res_wcol.as<int>();
+  if (h->res_restrict) {
+    a.rval = h->res_rval.as<float>(); a.rcol = h->res_rcol.as<unsigned short>(); a.roff = h->res_roff.as<unsigned int>();
+    a.rlen = h->res_rlen.as<unsigned int>(); a.rbits = h->res_rbits.as<unsigned int>(); a.rprod = h->res_rprod.as<double>();
+  }
+  a.sweeps = reinterpret_cast<ResSweeps*>(reinterpret_cast<char*>(h->result.p) + kSweepsAt);
   return a;
 }
 
@@ -493,6 +509,7 @@ template <typename T>
 int build_sparse(clp_handle h, bool force, const CompactShape& s, ScoreHandoff ho) {
   const int nseg = s.nseg;
   const long long nptr = (long long)nseg * (h->rows_pad + 1);
+  h->res_restrict = false;  // decided below with the layout; a build that keeps the dense sweep leaves it off
   if (!ho.after_score) { if (int rc = reset_sync(h)) return rc; }
   SyncBlock* sb = h->sync.as<SyncBlock>();
   const T* M = h->Mbuf.as<T>();
@@ -594,6 +611,10 @@ int build_sparse(clp_handle h, bool force, const CompactShape& s, ScoreHandoff h
     G = (int)std::max<long long>(1, std::min<long long>(std::min<long long>(h->grid_cap > 0 ? std::min(h->grid_cap, h->sm_count) : h->sm_count, NI / 2),
                                                         std::max<long long>(1, by_bytes)));
     h->res_G = G;
+    // sweeps over the support of the trial vector (the restricted copy, allocated below): packed copy on one GPU,
+    // only when it does not fit L2 -- a copy that does is served from L2 after the first pass anyway, and there the
+    // streamed full sweep beat the per-row restricted one (config 1: 3.3 against 4.0 ms per solve, DESIGN.md section 6)
+    h->res_restrict = h->sp.packed && h->world == 1 && (double)h->sp_nnz * sizeof(T) > (double)h->l2_bytes;
     CLP_CUDA(h, res_set_attrs<T>(h));
     const int NW = res_warps(h);
     CLP_CUDA(h, h->res_vecs.ensure((size_t)R_SLOTS * h->mpad * sizeof(double)));
@@ -610,6 +631,20 @@ int build_sparse(clp_handle h, bool force, const CompactShape& s, ScoreHandoff h
     CLP_CUDA(h, h->res_wcol.ensure((size_t)G * NW * 4 * sizeof(int)));
     res_warp_cols_kernel<<<(unsigned)((G * NW * 32 + 255) / 256), 256, 0, h->stream>>>(h->sp, G, NW, h->res_wcol.as<int>());
     CLP_CUDA(h, cudaGetLastError());
+  }
+  // the restricted copy: every row slot sized for the largest S' a rebuild takes
+  if (h->res_restrict) {
+    const unsigned long long ent = std::max<unsigned long long>(
+        4, std::min<unsigned long long>(h->sp_nnz, (unsigned long long)h->rows_pad * res_restrict_cap(~0u, (int)h->m)));
+    CLP_CUDA(h, h->res_rval.ensure((size_t)ent * sizeof(float)));
+    CLP_CUDA(h, h->res_rcol.ensure((size_t)ent * sizeof(unsigned short)));
+    CLP_CUDA(h, h->res_roff.ensure(((size_t)NI + 1) * sizeof(unsigned int)));
+    CLP_CUDA(h, h->res_rlen.ensure((size_t)h->rows_pad * sizeof(unsigned int)));
+    CLP_CUDA(h, h->res_rbits.ensure((size_t)G * ((h->m + 31) / 32) * sizeof(unsigned int)));
+    CLP_CUDA(h, h->res_rprod.ensure((size_t)h->rows_pad * 2 * sizeof(double)));
+    res_restrict_caps_kernel<<<(unsigned)((NI + 1 + 255) / 256), 256, 0, h->stream>>>(h->sp.itemptr, NI, (int)h->m, h->res_roff.as<unsigned int>());
+    CLP_CUDA(h, cudaGetLastError());
+    if (int rc = scan(h->res_roff.as<unsigned int>(), (long long)NI + 1, nullptr)) return rc;
   }
   h->sp_shape = s;
   return CLP_OK;
@@ -1023,6 +1058,9 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
 
   const SolverOut so = *h->pinned.as<const SolverOut>();
   h->seq = so.seq_end;
+  h->last_sweeps = ResSweeps{so.n_evals, 0, 0, 0ull, 0ull, 0};
+  if (h->dense_mode_eff == 6 && h->res_restrict)
+    h->last_sweeps = *reinterpret_cast<const ResSweeps*>(h->pinned.as<const char>() + kSweepsAt);
   if (h->prof_ctas && h->dense_mode_eff == 6) {  // diagnostics: spread of the per-CTA phase times
     std::vector<double> pc((size_t)h->res_G * 8);
     CLP_CUDA(h, cudaMemcpy(pc.data(), h->prof_buf.p, pc.size() * sizeof(double), cudaMemcpyDeviceToHost));
@@ -1662,6 +1700,8 @@ int clp_create(int device, int storage, clp_handle* out) {
   if (e != cudaSuccess || occ < 1 || occ3 < 1) return bail("occupancy query (is the sm_90a image loadable?)", e);
   h->ctas_per_sm = std::min(occ, 2);
   h->ctas_sparse = std::min(occ3, 3);
+  if ((e = cudaDeviceGetAttribute(&h->l2_bytes, cudaDevAttrL2CacheSize, device)) != cudaSuccess)
+    return bail("cudaDeviceGetAttribute", e);
   if ((e = cudaDeviceGetAttribute(&h->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device)) != cudaSuccess)
     return bail("cudaDeviceGetAttribute", e);
 
@@ -1677,6 +1717,7 @@ int clp_destroy(clp_handle h) {
   h->comm.release();
   for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->inv_prm, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
+                    &h->res_rval, &h->res_rcol, &h->res_roff, &h->res_rlen, &h->res_rbits, &h->res_rprod,
                     &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf, &h->knn_buf})
     b->release();
   h->pinned.release();
@@ -2138,6 +2179,14 @@ int clp_sparse_info(clp_handle h, int64_t* nnz_kept, int64_t* bytes_per_pass) {
   if (bytes_per_pass)
     *bytes_per_pass = (int64_t)(h->sp_nnz * h->entry_bytes() +
                                 (unsigned long long)(h->rows_pad / 4) * (h->sp_shape.resident ? 1 : h->plan.NSEG) * 20);
+  return CLP_OK;
+}
+
+int clp_last_solve_sweeps(clp_handle h, int64_t* counts) {
+  if (!h || !counts) return CLP_ERR_INVALID;
+  const ResSweeps& r = h->last_sweeps;
+  counts[0] = r.full; counts[1] = r.rebuild; counts[2] = r.restricted;
+  counts[3] = (int64_t)r.entries; counts[4] = (int64_t)r.padding; counts[5] = r.fallback;
   return CLP_OK;
 }
 

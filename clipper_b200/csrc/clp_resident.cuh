@@ -53,6 +53,13 @@ template <typename T, bool SHARDED> using ResShape = typename ResShapeOf<T, SHAR
 enum ResVec : int { R_U0 = 0, R_U1, R_G0, R_G1, R_MV0, R_MV1, R_CV0, R_CV1, R_SLOTS };
 enum ResStage : int { RS_RAW = 0, RS_DIV = 1, RS_STEP = 2 };
 
+// line-search evaluations by sweep kind and what the restricted sweeps read, over one solve
+struct ResSweeps {
+  long long full, rebuild, restricted;
+  unsigned long long entries, padding;  // restricted sweeps: entries read, padding entries read
+  long long fallback;                   // full sweeps after the first rebuild (the support grew past m / kSupportDiv)
+};
+
 struct ResArgs {
   SparseView sp;           // full-row compact copy: off16 holds column indices, itemptr [NI + 1], rowid [rows_pad]
   int m, row0, rows, rows_pad, NI;
@@ -78,7 +85,23 @@ struct ResArgs {
   double* prof_cta;        // nullable: [G][8] per-CTA phase times in ns (sweeps, epilogues, exchanges, staging), items, chunks
   int prof_laps;           // thread 0 of every CTA reads %globaltimer four times per evaluation (phase split in clp_solution)
   const int* wcol;         // packed layout: [G][warps][4] column of each member's last entry before the warp's stream (-1: none)
+  // packed layout on one GPU: the restricted copy (res_restrict_build; null rval: every sweep reads the whole copy)
+  float* rval;             // entries of every row whose column lies in S', in column order, padded to a multiple of 4
+  unsigned short* rcol;    //   with (0, column m); row slot of member s of item it: roff[it] + s * (roff[it + 1] - roff[it]) / 4
+  const unsigned int* roff;  // [NI + 1]
+  unsigned int* rlen;      // [rows_pad] entries of every row slot (stream position 4 it + s), without the padding
+  unsigned int* rbits;     // [G][ceil(m / 32)] S' as a column bitmap, one copy per CTA
+  double* rprod;           // [rows_pad][2] M w, C w of every row from the last restricted sweep
+  ResSweeps* sweeps;       // counters of the last solve (written by CTA 0)
 };
+
+// S' is rebuilt when the candidate's support holds at most m / kSupportDiv columns
+constexpr int kSupportDiv = 4;
+// entries a row slot must hold: the row's stored entries, at most one per support column, rounded up to whole chunks
+__host__ __device__ inline unsigned int res_restrict_cap(unsigned int row_entries, int m) {
+  const unsigned int t = ((unsigned int)(m / kSupportDiv) + 3u) & ~3u;
+  return row_entries < t ? row_entries : t;
+}
 
 // ---------------------------------------------------------------------------------------------------------------
 // mbarrier / bulk-copy primitives (SASS: SYNCS.*, UBLKCP)
@@ -586,6 +609,200 @@ __device__ __forceinline__ void res_gather_pieces(const double* ptab, unsigned i
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// sweeps over the support of the trial vector (packed layout, one GPU)
+// After the first penalty steps almost every entry of a projected candidate is an exact zero, and M_ij w_j with w_j = 0
+// adds nothing to row i's sums.  So once the support of the staged candidate w holds at most m / kSupportDiv columns,
+// every CTA copies those of its rows' entries whose column is in supp(w) -- S' -- into its own part of a restricted
+// copy, and the following evaluations read only that copy as long as supp(w) stays inside S'.  A row is still summed by
+// the CTA that owns it, from its own entries: only the terms multiplied by a zero of w are left out, so the sums are
+// the same exact products with a different grouping of the terms.  Every CTA stages the same w and so takes the same
+// decision without an exchange.
+// ---------------------------------------------------------------------------------------------------------------
+enum ResSweepKind : int { SW_FULL = 0, SW_REBUILD = 1, SW_RESTRICTED = 2 };
+
+// The staged candidate w (vs, raw) against S' (the CTA's bitmap; have: the restricted copy is valid): restricted if
+// supp(w) lies in S', else rebuild if |supp(w)| <= m / kSupportDiv, else full.  A rebuild stores supp(w) as the new S'.
+template <int NT>
+__device__ int res_support_kind(const ResArgs& a, int bid, const double* vs, bool have, double* red_s, double* fin) {
+  constexpr int NW = NT / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int m = a.m, nwords = (m + 31) >> 5;
+  unsigned int* bits = a.rbits + (size_t)bid * nwords;
+  int nsup = 0;
+  unsigned int outside = 0u;
+  for (int g = warp * 32; g < nwords; g += NW * 32) {  // lane l holds word g + l of S'
+    const unsigned int mine = (have && g + lane < nwords) ? bits[g + lane] : 0u;
+    const int ng = min(32, nwords - g);
+#pragma unroll 4
+    for (int k = 0; k < ng; ++k) {
+      const int j = (g + k) * 32 + lane;
+      const unsigned int b = __ballot_sync(0xffffffffu, j < m && vs[j] != 0.0);
+      nsup += __popc(b);
+      outside |= b & ~__shfl_sync(0xffffffffu, mine, k);
+    }
+  }
+  const double n = res_block_sum<NT>(lane == 0 ? (double)nsup : 0.0, red_s, fin);
+  const bool out = __syncthreads_or(outside != 0u) != 0;
+  if (have && !out) return SW_RESTRICTED;
+  if (!((double)kSupportDiv * n <= (double)m)) return SW_FULL;
+  for (int g = warp * 32; g < nwords; g += NW * 32) {
+    unsigned int mine = 0u;
+    const int ng = min(32, nwords - g);
+    for (int k = 0; k < ng; ++k) {
+      const int j = (g + k) * 32 + lane;
+      const unsigned int b = __ballot_sync(0xffffffffu, j < m && vs[j] != 0.0);
+      if (lane == k) mine = b;
+    }
+    if (g + lane < nwords) bits[g + lane] = mine;
+  }
+  return SW_REBUILD;
+}
+
+// Rebuild: one warp per item of the CTA reads the item's packed entries (columns from the deltas, as in
+// res_apply_packed) and appends every entry whose column holds a non-zero of w to its row's slot, in column order; the
+// slot is then padded to a whole chunk with (0, column m).  A slot holds at most min(row entries, m / kSupportDiv)
+// entries, which res_restrict_cap rounds up to a chunk: it never overflows.
+template <int NT>
+__device__ void res_restrict_build(const ResArgs& a, int bid, const double* vs) {
+  constexpr int NW = NT / 32, RB = 4;  // rounds of 32 chunks in flight per warp
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int it0 = a.sp.cta_first[bid], it1 = a.sp.cta_first[bid + 1];
+  const unsigned int* pw = reinterpret_cast<const unsigned int*>(a.sp.val);
+  for (unsigned int it = it0 + warp; it < it1; it += NW) {
+    const unsigned int b = a.sp.itemptr[it], e = a.sp.itemptr[it + 1];
+    const unsigned int r0 = a.roff[it], slot = r0 + (unsigned int)(lane & 3) * ((a.roff[it + 1] - r0) >> 2);
+    int carry = -1;
+    unsigned int cnt = 0u;  // entries of the member's row written so far (the same on its 8 lanes)
+    for (unsigned int c0 = b; c0 < e; c0 += 32u * RB) {
+      Packed4 E[RB];
+#pragma unroll
+      for (int u = 0; u < RB; ++u) {
+        const unsigned int c = c0 + 32u * u + (unsigned int)lane;
+        if (c < e) E[u].load(pw, 4ull * c); else E[u].neutral();
+      }
+#pragma unroll
+      for (int u = 0; u < RB; ++u) {
+        if (c0 + 32u * u >= e) break;  // warp-uniform
+        const unsigned int w4[4] = {E[u].w.x, E[u].w.y, E[u].w.z, E[u].w.w};
+        const unsigned int own = pack_delta(w4[0]) + pack_delta(w4[1]) + pack_delta(w4[2]) + pack_delta(w4[3]);
+        unsigned int inc = own;
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+        int col = carry + (int)(inc - own);
+        carry += (int)__shfl_sync(0xffffffffu, inc, 28 + (lane & 3));
+        unsigned int keep = 0u;
+        int cols[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          col += (int)pack_delta(w4[q]);
+          cols[q] = col;
+          if ((w4[q] & 0x07800000u) && vs[col] != 0.0) keep |= 1u << q;
+        }
+        const unsigned int nk = (unsigned int)__popc(keep);
+        unsigned int kin = nk;
+#pragma unroll
+        for (int o = 4; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, kin, o); if (lane >= o) kin += y; }
+        unsigned int at = slot + cnt + (kin - nk);
+        cnt += __shfl_sync(0xffffffffu, kin, 28 + (lane & 3));
+#pragma unroll
+        for (int q = 0; q < 4; ++q)
+          if (keep & (1u << q)) {
+            a.rval[at] = __uint_as_float((w4[q] & 0x07ffffffu) + a.sp.ebias);
+            a.rcol[at] = (unsigned short)cols[q];
+            ++at;
+          }
+      }
+    }
+    if (lane < 4) {  // lane s: member s
+      for (unsigned int k = cnt; k & 3u; ++k) { a.rval[slot + k] = 0.0f; a.rcol[slot + k] = (unsigned short)a.m; }
+      a.rlen[4u * it + (unsigned int)lane] = cnt;
+    }
+  }
+}
+
+// The restricted sweep: warp w sums the CTA's rows w, w + NW, ... from their slots into rprod.  Lane l takes chunks
+// l, l + 32, ... of a row; RD rounds of RU chunks per lane are in flight, carried on from one row to the next.  The
+// copy was written by this CTA in this launch: plain loads, no ld.global.nc.
+template <int NT>
+__device__ void res_sweep_restricted(const ResArgs& a, int bid, const double* vs) {
+  constexpr int NW = NT / 32, RU = 2, RD = 2;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const unsigned int it0 = a.sp.cta_first[bid];
+  const int nrow = (int)(a.sp.cta_first[bid + 1] - it0) * 4;
+  for (int rb = warp; rb < nrow; rb += 32 * NW) {
+    // lane i: slot and padded length of the warp's row rb + NW i
+    const int nb = min(32, (nrow - rb + NW - 1) / NW);
+    unsigned int slot = 0u, len = 0u;
+    if (lane < nb) {
+      const unsigned int t = 4u * it0 + (unsigned int)(rb + NW * lane), it = t >> 2;
+      const unsigned int r0 = a.roff[it];
+      slot = r0 + (t & 3u) * ((a.roff[it + 1] - r0) >> 2);
+      len = (a.rlen[t] + 3u) & ~3u;
+    }
+    int ci = 0;             // producer cursor: row of the batch, first entry of its next round
+    unsigned int ck = 0u;
+    float4 X[RD][RU];
+    uint2 K[RD][RU];
+    int srow[RD];
+    bool slast[RD], sval[RD];
+    auto produce = [&](int s) {
+      sval[s] = ci < nb;
+      if (!sval[s]) return;
+      const unsigned int s0 = __shfl_sync(0xffffffffu, slot, ci), n0 = __shfl_sync(0xffffffffu, len, ci);
+#pragma unroll
+      for (int u = 0; u < RU; ++u) {
+        const unsigned int k = ck + 4u * (unsigned int)lane + 128u * u;
+        if (k < n0) {
+          X[s][u] = *reinterpret_cast<const float4*>(a.rval + s0 + k);
+          K[s][u] = *reinterpret_cast<const uint2*>(a.rcol + s0 + k);
+        } else {
+          X[s][u] = make_float4(0.f, 0.f, 0.f, 0.f);
+          K[s][u] = make_uint2((unsigned int)a.m * 0x10001u, (unsigned int)a.m * 0x10001u);  // column m holds 0.0
+        }
+      }
+      srow[s] = ci;
+      slast[s] = ck + 128u * RU >= n0;
+      if (slast[s]) { ++ci; ck = 0u; } else ck += 128u * RU;
+    };
+    double aM[2] = {0.0, 0.0}, aC[2] = {0.0, 0.0};
+#pragma unroll
+    for (int s = 0; s < RD; ++s) produce(s);
+    for (;;) {
+      bool done = false;
+#pragma unroll
+      for (int s = 0; s < RD; ++s) {
+        if (!sval[s]) { done = true; break; }
+#pragma unroll
+        for (int u = 0; u < RU; ++u) {
+          const float x4[4] = {X[s][u].x, X[s][u].y, X[s][u].z, X[s][u].w};
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {
+            const double v = vs[off_of(K[s][u], q)];
+            aM[u & 1] = fma((double)x4[q], v, aM[u & 1]);
+            aC[u & 1] += v;
+          }
+        }
+        if (slast[s]) {
+          double accM = aM[0] + aM[1], accC = aC[0] + aC[1];
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) {
+            accM += __shfl_xor_sync(0xffffffffu, accM, o);
+            accC += __shfl_xor_sync(0xffffffffu, accC, o);
+          }
+          if (lane == 0) {
+            double* p = a.rprod + 2 * (4ull * it0 + (unsigned long long)(rb + NW * srow[s]));
+            p[0] = accM; p[1] = accC;
+          }
+          aM[0] = aM[1] = aC[0] = aC[1] = 0.0;
+        }
+        produce(s);
+      }
+      if (done) break;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // device-wide exchange of 8 partial sums: one arrival counter, every CTA reduces the table itself
 // ---------------------------------------------------------------------------------------------------------------
 template <int NT, bool SHARDED, bool SOLO>
@@ -719,7 +936,7 @@ __device__ bool res_exchange(const ResArgs& a, const int bid, const double (&loc
 // ---------------------------------------------------------------------------------------------------------------
 // the solver body (shared by solver_resident_kernel and the batched kernel)
 // ---------------------------------------------------------------------------------------------------------------
-template <typename T, int NT, int U, int D, bool SHARDED, bool SOLO, bool COH = false, bool PACK = false>
+template <typename T, int NT, int U, int D, bool SHARDED, bool SOLO, bool COH = false, bool PACK = false, bool RESTRICT = false>
 __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   constexpr int NW = NT / 32;
   const int bid = SOLO ? 0 : (int)blockIdx.x;  // CTA index within the problem (batched: one CTA per problem)
@@ -747,6 +964,8 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   constexpr bool stage_bulk = !SHARDED && !SOLO;
   // candidate staged as it is, 1/|w| applied to the row results: whenever a CTA owns fewer rows than the vector has entries
   constexpr bool stage_raw = !SOLO;
+  // sweeps over the support of the trial vector: packed copy, one GPU (res_support_kind)
+  constexpr bool restrict_ok = RESTRICT && PACK && !SHARDED && !SOLO;
   if constexpr (!SHARDED && !SOLO) {
     if (threadIdx.x < kStageBlocks) mbar_init(&sbars[threadIdx.x], 1);
     fence_mbar_init();
@@ -809,6 +1028,11 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
 
   double vals[kRedVals], loc[kRedVals];
   long long n_evals = 0, n_inner = 0, n_matvec = 0;
+  long long n_sweep[3] = {0, 0, 0};  // line-search evaluations by ResSweepKind
+  long long n_fallback = 0;
+  double r_entries = 0.0, r_padding = 0.0;
+  bool rhave = false;                // the restricted copy holds S'
+  int skind = SW_FULL;               // sweep of the current evaluation
   int cur = 0, cpar = 0, red_par = 0, status = 0, i_outer = 0;
   double d = 0.0, F = 0.0, sum_cur = 0.0, z = 0.0, sw = 0.0;  // z, sw: |w|^2 and sum(w) of the candidate the next evaluation stages
   unsigned long long round = 0, seq = a.seq0;
@@ -920,7 +1144,24 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
                                         vs, red_s, fin, errp, a.spin_limit, bid * 416);
         }
         RES_LAP(ns_st);
-        RES_SWEEP();
+        skind = SW_FULL;
+        if constexpr (restrict_ok)
+          if (a.rval) skind = res_support_kind<NT>(a, bid, vs, rhave, red_s, fin);
+        if (skind == SW_FULL) {
+          RES_SWEEP();
+        } else {
+          if (skind == SW_REBUILD) {
+            res_restrict_build<NT>(a, bid, vs);
+            rhave = true;
+            __syncthreads();
+          }
+          res_sweep_restricted<NT>(a, bid, vs);
+          ++n_matvec;
+          __syncthreads();
+          RES_LAP(ns_mv);
+        }
+        ++n_sweep[skind];
+        if (skind == SW_FULL && rhave) ++n_fallback;
         ++n_evals;
         // per-row epilogue: gradFnew, Fnew, |unew - u|^2 and BOTH possible next trial points
         const double alpha_rej = __dmul_rn(alpha, P.beta);
@@ -928,7 +1169,13 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         const unsigned int tag = (unsigned int)(seq + 1);
         RES_FOR_ROWS(i, itx, sx) {
           double Mv, Cv;
-          res_gather_pieces(ptab, isub, ptab_sh, wmask, itx, sx, w0_, w1_, Mv, Cv);
+          if (skind != SW_FULL) {
+            const unsigned int t = 4u * itx + (unsigned int)sx, n = a.rlen[t];
+            Mv = a.rprod[2ull * t]; Cv = a.rprod[2ull * t + 1];
+            loc[6] += (double)n; loc[7] += (double)((0u - n) & 3u);
+          } else {
+            res_gather_pieces(ptab, isub, ptab_sh, wmask, itx, sx, w0_, w1_, Mv, Cv);
+          }
           double un = vs[i];
           if (lzs) {
             un = div_by_invariant(un, nrm_l, rinv_l);
@@ -952,6 +1199,7 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         cpar ^= 1; ctag = tag;
         // the line-search decision (clipper.cpp:242-251), identical on every CTA / rank
         Fnew = vals[0]; du2 = vals[1]; zB = vals[3]; swB = vals[4];
+        r_entries += vals[6]; r_padding += vals[7];
         deltaF = Fnew - F;
         sum_trial = sumv;
         if (deltaF < -P.eps) {
@@ -1007,6 +1255,11 @@ finish:
     a.out->F = F; a.out->d = d; a.out->ifinal = i_outer; a.out->cur = cur; a.out->status = status;
     a.out->n_evals = n_evals; a.out->n_inner = n_inner; a.out->n_matvec = n_matvec; a.out->seq_end = seq;
     a.out->ns_matvec = ns_mv + ns_st; a.out->ns_combine = ns_cb; a.out->ns_exchange = ns_ex;
+    if (restrict_ok && a.sweeps) {
+      a.sweeps->full = n_sweep[SW_FULL]; a.sweeps->rebuild = n_sweep[SW_REBUILD]; a.sweeps->restricted = n_sweep[SW_RESTRICTED];
+      a.sweeps->entries = (unsigned long long)r_entries; a.sweeps->padding = (unsigned long long)r_padding;
+      a.sweeps->fallback = n_fallback;
+    }
   }
 #undef RES_LAP
 #undef RES_ZERO
@@ -1015,11 +1268,13 @@ finish:
 #undef RES_SWEEP
 }
 
-template <typename T, bool SHARDED, bool PACK = false>
+// RESTRICT: the instance with sweeps over the support (packed copy on one GPU, larger than L2).  Its own instance
+// because the new path costs the kernel registers (spills) that the solves without it should not pay.
+template <typename T, bool SHARDED, bool PACK = false, bool RESTRICT = false>
 __global__ void __launch_bounds__(ResShape<T, SHARDED>::NT, 1) solver_resident_kernel(ResArgs a) {
   extern __shared__ __align__(128) unsigned char clp_res_smem[];
   using S = ResShape<T, SHARDED>;
-  res_solve_body<T, S::NT, S::U, S::D, SHARDED, false, false, PACK>(a, clp_res_smem);
+  res_solve_body<T, S::NT, S::U, S::D, SHARDED, false, false, PACK, RESTRICT>(a, clp_res_smem);
 }
 
 // stand-alone mat-vec on the resident layout: stage v, sweep, per-row epilogue -- one launch, no device-wide barrier.
@@ -1090,6 +1345,14 @@ __global__ void res_warp_cols_kernel(SparseView sp, int G, int NW, int* wcol) {
 #pragma unroll
   for (int o = 4; o < 32; o <<= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
   if (lane < 4) wcol[gw * 4 + lane] = (int)sum - 1;
+}
+
+// packed layout on one GPU, once per build: roff[it] = entries of item it's four row slots in the restricted copy
+// (res_restrict_cap), roff[NI] = 0; the exclusive scan of clp_sparse.cuh then turns them into slot offsets
+__global__ void res_restrict_caps_kernel(const unsigned int* itemptr, int NI, int m, unsigned int* roff) {
+  const int it = blockIdx.x * blockDim.x + threadIdx.x;
+  if (it < NI) roff[it] = 4u * res_restrict_cap(itemptr[it + 1] - itemptr[it], m);  // a member's entries = the item's chunks
+  else if (it == NI) roff[it] = 0u;
 }
 
 }  // namespace clp

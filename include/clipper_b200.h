@@ -268,6 +268,13 @@ int clp_set_dense_mode(clp_handle h, int mode);
 int clp_get_dense_mode(clp_handle h, int* requested, int* effective);
 /* entries kept by the compact copy (all local rows) and the algorithmic bytes one sparse pass reads */
 int clp_sparse_info(clp_handle h, int64_t* nnz_kept, int64_t* bytes_per_pass);
+/* How the line-search evaluations of the last solve read the matrix.  counts[0..5]: evaluations that swept the whole
+ * compact copy, that rebuilt the restricted copy (the entries of every row in the support S' of the trial vector, once
+ * |S'| <= m / 4) and swept it, that swept the restricted copy only (the support stayed inside S'); the entries and the
+ * padding entries those restricted sweeps read, summed over the solve; and how many of the full sweeps came after the
+ * first rebuild.  Only the resident solver on a packed copy larger than the L2 cache, on one GPU, takes restricted
+ * sweeps; every other solve reports all its evaluations as full. */
+int clp_last_solve_sweeps(clp_handle h, int64_t* counts);
 
 /* ---- maximum clique of the constraint graph (solveAsMaximumClique, clipper.cpp:82-97, maxclique.cpp:89-140) --------
  * The graph is C without its diagonal: {i,j} is an edge iff C_ij = 1 (the sign bit of the stored element is clear),
