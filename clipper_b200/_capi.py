@@ -39,11 +39,14 @@ SYMBOLS = [
     "clp_sdp_default_params", "clp_sdp_solve", "clp_batch_sdp_matrices",
     "clp_correspondences", "clp_correspondences_dev",
     "clp_batch_correspondences", "clp_batch_correspondences_dev",
+    "clp_estimate_transform", "clp_estimate_transform_dev",
+    "clp_batch_estimate_transform", "clp_batch_estimate_transform_dev",
 ]
 INV_MAX_PARAMS = 16
 MC_EXACT, MC_HEU, MC_KCORE = 0, 1, 2
 SDP_MAX_M = 128
 KNN_MAX_K, KNN_MAX_D = 32, 64
+TF_OK, TF_EMPTY, TF_DEGENERATE, TF_NONFINITE = 0, 1, 2, 3
 
 
 class ClpParams(C.Structure):
@@ -99,6 +102,14 @@ class ClpPointsDev(C.Structure):
         ("D1", C.c_void_p), ("d1_strides", C.c_int64 * 3), ("D2", C.c_void_p), ("d2_strides", C.c_int64 * 3),
         ("A", C.c_void_p), ("a_strides", C.c_int64 * 3),
         ("n1", C.POINTER(C.c_int64)), ("n2", C.POINTER(C.c_int64)), ("m", C.POINTER(C.c_int64)),
+    ]
+
+
+class ClpTfInfo(C.Structure):
+    """clp_tf_info: outcome of one rigid-transform estimate."""
+    _fields_ = [
+        ("status", C.c_int32), ("k", C.c_int64), ("rmse", C.c_double), ("sv", C.c_double * 3), ("gap", C.c_double),
+        ("t", C.c_double), ("kernel_ms", C.c_double),
     ]
 
 
@@ -213,6 +224,11 @@ def load():
     L.clp_correspondences_dev.argtypes = [vp, vp, i32, i64, vp, i64, i32, dbl, C.c_int, vp, i64, lp]
     L.clp_batch_correspondences.argtypes = [vp, i32, i32, pp, lp, pp, lp, i32, dbl, C.c_int, pp, i64, lp]
     L.clp_batch_correspondences_dev.argtypes = [vp, i32, i32, vp, lp, lp, vp, lp, lp, i32, dbl, C.c_int, vp, lp, i64, lp]
+    tip = C.POINTER(ClpTfInfo)
+    L.clp_estimate_transform.argtypes = [vp, vp, i32, i64, vp, i64, vp, i64, vp, i64, vp, tip]
+    L.clp_estimate_transform_dev.argtypes = [vp, vp, i32, i64, vp, i64, vp, i64, vp, i64, vp, tip]
+    L.clp_batch_estimate_transform.argtypes = [vp, i32, i32, pp, lp, pp, lp, pp, lp, pp, lp, pp, tip]
+    L.clp_batch_estimate_transform_dev.argtypes = [vp, i32, i32, ptp, pp, lp, vp, lp, tip]
     _lib = L
     return L
 

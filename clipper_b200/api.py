@@ -6,6 +6,7 @@ Names, argument meaning and defaults follow reference bindings/python/py_clipper
   utils.{create_all_to_all, k2ij}      dsd.{solve, create_all_to_all, k2ij}
   utils.distance_based_correspondences(_dev) (additive: putative associations by exact kNN on the GPU)
   utils.distance_based_correspondences_many(_dev) (additive: the same for a batch of cloud pairs in one call)
+  utils.estimate_rigid_transform(_many)(_dev) (additive: the rigid transform of selected associations on the GPU)
   Rounding, Params, Solution, MCParams, SDPParams, CLIPPER (11 methods)
 
 Differences that are deliberate and additive:
@@ -419,6 +420,173 @@ def distance_based_correspondences_many_dev(D1, D2, knn, radius, enforce_1to1, n
     return A, [int(x) for x in m]
 
 
+class TransformInfo:
+    """outcome of one rigid-transform estimate (clp_tf_info): status (TF_OK, TF_EMPTY, TF_DEGENERATE, TF_NONFINITE),
+    k (pairs used), rmse, sv (singular values of H, descending, 3 entries), gap, t (wall-clock seconds), kernel_ms"""
+    __slots__ = ("status", "k", "rmse", "sv", "gap", "t", "kernel_ms")
+
+    def __init__(self, ci):
+        self.status, self.k, self.rmse = int(ci.status), int(ci.k), float(ci.rmse)
+        self.sv, self.gap = np.array(ci.sv[:], dtype=np.float64), float(ci.gap)
+        self.t, self.kernel_ms = float(ci.t), float(ci.kernel_ms)
+
+    def __repr__(self):
+        return "<TransformInfo status=%d k=%d rmse=%g gap=%g>" % (self.status, self.k, self.rmse, self.gap)
+
+
+def _tf_rows(rows, name):
+    """(int32 array or None, k) of a rows argument: None is every row"""
+    if rows is None:
+        return None, 0
+    r = np.ascontiguousarray(np.asarray(rows).reshape(-1))
+    if r.size and not np.issubdtype(r.dtype, np.integer):
+        raise TypeError("%s must hold integer row indices" % name)
+    if r.size and (r.min() < -2 ** 31 or r.max() >= 2 ** 31):
+        raise ValueError("%s holds row indices outside int32" % name)
+    return np.ascontiguousarray(r, dtype=np.int32), int(r.size)
+
+
+def _tf_host_problem(D1, D2, A, rows):
+    """checked host arrays of one problem: (D1, D2, A or None, m, rows, k); an A without rows and rows None take
+    k = 0 rows (empty, not all-to-all)"""
+    D1 = np.asfortranarray(_check_f64(D1, "D1"))
+    D2 = np.asfortranarray(_check_f64(D2, "D2"))
+    if D1.ndim != 2 or D2.ndim != 2 or D1.shape[0] != D2.shape[0]:
+        raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+    m = 0
+    if A is not None:
+        if not isinstance(A, np.ndarray) or A.dtype != np.int32:
+            raise TypeError("A must be a numpy int32 array (m, 2)")
+        if A.ndim != 2 or A.shape[1] != 2:
+            raise ValueError("A must be (m, 2)")
+        m = A.shape[0]
+        A = np.asfortranarray(A)
+    r, kk = _tf_rows(rows, "rows")
+    if A is not None and m == 0 and r is None:
+        r, kk = np.zeros(1, np.int32), 0   # an empty A is no pairs, not the all-to-all hypothesis
+    return D1, D2, A, m, r, kk
+
+
+def _tf_T(buf, d):
+    """row-major (d+1, d+1) from the column-major buffer the C-ABI fills"""
+    return np.ascontiguousarray(buf.reshape(d + 1, d + 1).T)
+
+
+def estimate_rigid_transform(D1, D2, A, rows=None):
+    """the proper rigid transform T ((d+1, d+1) float64, row-major, b ~ R a + t) that aligns the pairs (D1[:, A[r, 0]],
+    D2[:, A[r, 1]]) of the rows r of A (device 0; clp_estimate_transform).  D1 (d, n1), D2 (d, n2) float64 with d 2 or
+    3; A (m, 2) int32, e.g. CLIPPER.get_selected_associations(), or None for the all-to-all hypothesis (row r = (r //
+    n2, r % n2)); rows: row indices of A (each counted once per listing) or None for every row.  An A without rows
+    gives status TF_EMPTY.  Returns (T, TransformInfo)."""
+    D1, D2, A, m, r, k = _tf_host_problem(D1, D2, A, rows)
+    d = D1.shape[0]
+    T = np.zeros((d + 1) ** 2 if d >= 1 else 1)
+    info = _capi.ClpTfInfo()
+    h = _knn_handle(0, False)   # the utils' kept handle: only its device, stream and error string are used
+    _capi.check(h, _capi.load().clp_estimate_transform(
+        h, D1.ctypes.data, d, D1.shape[1], D2.ctypes.data, D2.shape[1], A.ctypes.data if A is not None else None, m,
+        r.ctypes.data if r is not None else None, k, T.ctypes.data, C.byref(info)))
+    return _tf_T(T, d), TransformInfo(info)
+
+
+def estimate_rigid_transform_many(D1s, D2s, As, rows=None):
+    """estimate_rigid_transform of every problem (D1s[p], D2s[p], As[p], rows[p]) in one batched call on the GPU
+    (device 0; clp_batch_estimate_transform), one d for all; rows None or a list whose entries may be None.  Problem p
+    is bit for bit the single call.  Returns (list of T, list of TransformInfo)."""
+    D1s, D2s, As = list(D1s), list(D2s), list(As)
+    nb = len(D1s)
+    if len(D2s) != nb or len(As) != nb:
+        raise ValueError("D1s, D2s and As must have the same length, got %d, %d and %d" % (nb, len(D2s), len(As)))
+    rows = [None] * nb if rows is None else list(rows)
+    if len(rows) != nb:
+        raise ValueError("rows must hold one entry per problem")
+    if nb == 0:
+        return [], []
+    probs = [_tf_host_problem(X, Y, A, r) for X, Y, A, r in zip(D1s, D2s, As, rows)]
+    d = probs[0][0].shape[0]
+    if any(q[0].shape[0] != d for q in probs):
+        raise ValueError("every problem must have the same d")
+    Ts = [np.zeros((d + 1) ** 2 if d >= 1 else 1) for _ in range(nb)]
+    infos = (_capi.ClpTfInfo * nb)()
+    vp, i64 = C.c_void_p, C.c_int64
+    ptr = lambda x: x.ctypes.data if x is not None else None  # noqa: E731
+    kb = _knn_batch(0, False)   # the utils' kept batch: only its device, stream and error string are used
+    kb.check(_capi.load().clp_batch_estimate_transform(
+        kb.b, nb, d, (vp * nb)(*[q[0].ctypes.data for q in probs]), (i64 * nb)(*[q[0].shape[1] for q in probs]),
+        (vp * nb)(*[q[1].ctypes.data for q in probs]), (i64 * nb)(*[q[1].shape[1] for q in probs]),
+        (vp * nb)(*[ptr(q[2]) for q in probs]), (i64 * nb)(*[q[3] for q in probs]),
+        (vp * nb)(*[ptr(q[4]) for q in probs]), (i64 * nb)(*[q[5] for q in probs]), (vp * nb)(*[T.ctypes.data for T in Ts]),
+        infos))
+    return [_tf_T(T, d) for T in Ts], [TransformInfo(infos[p]) for p in range(nb)]
+
+
+def estimate_rigid_transform_dev(D1, D2, A, rows=None):
+    """estimate_rigid_transform of CUDA tensors on their device and torch's current stream (clp_estimate_transform_dev):
+    D1 (d, n1), D2 (d, n2) float64, A (m, 2) int32 CUDA tensor or None (all-to-all); rows a host sequence or None.
+    Tensors of another layout than column-major are copied on the device first.  Returns (T, TransformInfo), T a (d+1,
+    d+1) float64 CUDA tensor; bit for bit the host call's T."""
+    import torch
+    for name, X in (("D1", D1), ("D2", D2)):
+        if not isinstance(X, torch.Tensor) or X.dtype != torch.float64:
+            raise TypeError("%s must be a torch.float64 tensor" % name)
+    if A is not None and (not isinstance(A, torch.Tensor) or A.dtype != torch.int32):
+        raise TypeError("A must be a torch.int32 tensor or None")
+    if D1.dim() != 2 or D2.dim() != 2 or D1.shape[0] != D2.shape[0]:
+        raise ValueError("D1 and D2 must be (d, n1) and (d, n2)")
+    if A is not None and (A.dim() != 2 or A.shape[1] != 2):
+        raise ValueError("A must be (m, 2)")
+    r, k = _tf_rows(rows, "rows")
+    m = 0 if A is None else int(A.shape[0])
+    if A is not None and m == 0 and r is None:
+        r, k = np.zeros(1, np.int32), 0   # an empty A is no pairs, not the all-to-all hypothesis
+    for name, X in (("D1", D1), ("D2", D2)) + ((("A", A),) if A is not None else ()):
+        if not X.is_cuda or X.device != D1.device:
+            raise ValueError("%s must be a CUDA tensor on D1's device, got one on %s" % (name, X.device))
+    (d, n1), n2 = D1.shape, D2.shape[1]
+    P1, P2 = D1.t().contiguous(), D2.t().contiguous()   # column-major (d, n) is row-major (n, d)
+    PA = A.t().contiguous() if A is not None else None
+    T = torch.empty((d + 1, d + 1), dtype=torch.float64, device=D1.device)
+    h = _knn_handle(D1.device.index, True)
+    lib = _capi.load()
+    # as in distance_based_correspondences_dev: torch's default stream is named as the legacy default stream
+    stream = torch.cuda.current_stream(D1.device).cuda_stream or _CUDA_STREAM_LEGACY
+    _capi.check(h, lib.clp_set_stream(h, C.c_void_p(stream)))
+    info = _capi.ClpTfInfo()
+    # the C-ABI writes T column-major: T.t() of a row-major tensor
+    _capi.check(h, lib.clp_estimate_transform_dev(
+        h, P1.data_ptr() or None, d, n1, P2.data_ptr() or None, n2, PA.data_ptr() if PA is not None else None, m,
+        r.ctypes.data if r is not None else None, k, T.data_ptr(), C.byref(info)))
+    return T.t(), TransformInfo(info)
+
+
+def estimate_rigid_transform_many_dev(D1, D2, A, rows=None, n1=None, n2=None, m=None):
+    """estimate_rigid_transform of a batch in GPU memory, in one call on torch's current stream
+    (clp_batch_estimate_transform_dev).  D1, D2, A, n1, n2 and m exactly as BatchCLIPPER.solve_many_dev takes them
+    (A None or m[p] = 0: all-to-all); rows: None (every row) or B entries, each None or host row indices, e.g. [s.nodes
+    for s in sols].  Returns (T, infos): T a (B, d+1, d+1) float64 CUDA tensor, row-major per problem, and B
+    TransformInfo; problem p is bit for bit the single call."""
+    import torch
+    from .batch import _dev_points
+    if not isinstance(D1, torch.Tensor) or not D1.is_cuda:
+        raise ValueError("D1 must be a CUDA tensor")
+    d, nb, pts, ms, keep = _dev_points(D1.device.index, D1, D2, A, n1, n2, m)  # keep: the host size arrays of pts
+    rows = [None] * nb if rows is None else list(rows)
+    if len(rows) != nb:
+        raise ValueError("rows must hold one entry per problem")
+    rk = [_tf_rows(r, "rows[%d]" % p) for p, r in enumerate(rows)]
+    T = torch.empty((nb, d + 1, d + 1), dtype=torch.float64, device=D1.device)
+    kb = _knn_batch(D1.device.index, True)
+    lib = _capi.load()
+    stream = torch.cuda.current_stream(D1.device).cuda_stream or _CUDA_STREAM_LEGACY
+    kb.check(lib.clp_batch_set_stream(kb.b, C.c_void_p(stream)))
+    infos = (_capi.ClpTfInfo * nb)()
+    vp, i64 = C.c_void_p, C.c_int64
+    kb.check(lib.clp_batch_estimate_transform_dev(
+        kb.b, nb, d, C.byref(pts), (vp * nb)(*[r.ctypes.data if r is not None else None for r, _ in rk]),
+        (i64 * nb)(*[k for _, k in rk]), T.data_ptr(), (i64 * 3)(*T.stride()), infos))
+    return T, [TransformInfo(infos[p]) for p in range(nb)]
+
+
 def k2ij(k, n):
     """reference utils.cpp:87-97"""
     i, j = C.c_uint64(), C.c_uint64()
@@ -461,7 +629,13 @@ utils = types.SimpleNamespace(create_all_to_all=create_all_to_all, k2ij=k2ij,
                               distance_based_correspondences=distance_based_correspondences,
                               distance_based_correspondences_dev=distance_based_correspondences_dev,
                               distance_based_correspondences_many=distance_based_correspondences_many,
-                              distance_based_correspondences_many_dev=distance_based_correspondences_many_dev)
+                              distance_based_correspondences_many_dev=distance_based_correspondences_many_dev,
+                              estimate_rigid_transform=estimate_rigid_transform,
+                              estimate_rigid_transform_many=estimate_rigid_transform_many,
+                              estimate_rigid_transform_dev=estimate_rigid_transform_dev,
+                              estimate_rigid_transform_many_dev=estimate_rigid_transform_many_dev,
+                              TransformInfo=TransformInfo, TF_OK=_capi.TF_OK, TF_EMPTY=_capi.TF_EMPTY,
+                              TF_DEGENERATE=_capi.TF_DEGENERATE, TF_NONFINITE=_capi.TF_NONFINITE)
 dsd = types.SimpleNamespace(solve=dsd_solve, create_all_to_all=create_all_to_all, k2ij=k2ij)
 
 

@@ -437,6 +437,82 @@ std::vector<Association> distanceBasedCorrespondencesBatch(const std::vector<inv
   return As;
 }
 
+// T (column-major from the C-ABI, the layout of Eigen::MatrixXd) and info of one estimate
+static RigidTransformEstimate transform_estimate(const std::vector<double>& T, int d, const clp_tf_info& f)
+{
+  RigidTransformEstimate r;
+  r.T.resize(d + 1, d + 1);
+  std::memcpy(r.T.data(), T.data(), sizeof(double) * (size_t)((d + 1) * (d + 1)));
+  r.status = f.status; r.k = (int)f.k; r.rmse = f.rmse; r.gap = f.gap;
+  r.sv.resize(3);
+  for (int i = 0; i < 3; ++i) r.sv(i) = f.sv[i];
+  return r;
+}
+
+// every row of A (rows = {0, .., m-1} given explicitly, so an empty A is k = 0 rather than all-to-all), with a
+// temporary handle on device 0
+RigidTransformEstimate estimateRigidTransform(const invariants::Data& D1, const invariants::Data& D2, const Association& A)
+{
+  if (D1.rows() != D2.rows())
+    throw std::runtime_error("clipper_b200: estimateRigidTransform expects D1 and D2 with the same number of rows");
+  const int d = (int)D1.rows();
+  const int64_t m = (int64_t)A.rows();
+  std::vector<int32_t> rows((size_t)std::max<int64_t>(m, 1));
+  for (int64_t i = 0; i < m; ++i) rows[(size_t)i] = (int32_t)i;
+  clp_handle h = nullptr;
+  if (clp_create(0, CLP_STORE_F32, &h) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_create: ") + clp_last_error(nullptr));
+  std::shared_ptr<void> guard(h, [](void* p) { clp_destroy(static_cast<clp_handle>(p)); });
+  std::vector<double> T((size_t)std::max(1, (d + 1) * (d + 1)));
+  clp_tf_info f;
+  check(h, clp_estimate_transform(h, D1.data(), d, (int64_t)D1.cols(), D2.data(), (int64_t)D2.cols(),
+                                  reinterpret_cast<const int32_t*>(A.data()), m, rows.data(), m, T.data(), &f),
+        "clp_estimate_transform");
+  return transform_estimate(T, d, f);
+}
+
+// every problem in one clp_batch_estimate_transform call with a temporary batch on device 0
+std::vector<RigidTransformEstimate> estimateRigidTransformBatch(const std::vector<invariants::Data>& D1s,
+                                                                const std::vector<invariants::Data>& D2s,
+                                                                const std::vector<Association>& As)
+{
+  if (D1s.size() != D2s.size() || D1s.size() != As.size())
+    throw std::runtime_error("clipper_b200: estimateRigidTransformBatch expects as many D1s, D2s and As");
+  const size_t nprob = D1s.size();
+  if (nprob == 0) return {};
+  if (nprob > (size_t)INT32_MAX) throw std::runtime_error("clipper_b200: estimateRigidTransformBatch: too many problems");
+  const int d = (int)D1s[0].rows();
+  for (size_t p = 0; p < nprob; ++p)
+    if (D1s[p].rows() != d || D2s[p].rows() != d)
+      throw std::runtime_error("clipper_b200: estimateRigidTransformBatch expects every cloud with the same number of rows");
+  int64_t most = 1;
+  for (const Association& A : As) most = std::max<int64_t>(most, (int64_t)A.rows());
+  std::vector<int32_t> iota((size_t)most);
+  for (int64_t i = 0; i < most; ++i) iota[(size_t)i] = (int32_t)i;
+  std::vector<int64_t> n1(nprob), n2(nprob), m(nprob);
+  std::vector<const double*> p1(nprob), p2(nprob);
+  std::vector<const int32_t*> pa(nprob), rows(nprob, iota.data());
+  std::vector<std::vector<double>> Ts(nprob, std::vector<double>((size_t)std::max(1, (d + 1) * (d + 1))));
+  std::vector<double*> pt(nprob);
+  for (size_t p = 0; p < nprob; ++p) {
+    n1[p] = (int64_t)D1s[p].cols(); n2[p] = (int64_t)D2s[p].cols(); m[p] = (int64_t)As[p].rows();
+    p1[p] = D1s[p].data(); p2[p] = D2s[p].data(); pa[p] = reinterpret_cast<const int32_t*>(As[p].data());
+    pt[p] = Ts[p].data();
+  }
+  clp_batch b = nullptr;
+  if (clp_batch_create(0, &b) != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_batch_create: ") + clp_batch_last_error(nullptr));
+  std::shared_ptr<void> guard(b, [](void* q) { clp_batch_destroy(static_cast<clp_batch>(q)); });
+  std::vector<clp_tf_info> f(nprob);
+  const int rc = clp_batch_estimate_transform(b, (int32_t)nprob, d, p1.data(), n1.data(), p2.data(), n2.data(), pa.data(),
+                                              m.data(), rows.data(), m.data(), pt.data(), f.data());
+  if (rc != CLP_OK)
+    throw std::runtime_error(std::string("clipper_b200: clp_batch_estimate_transform: ") + clp_batch_last_error(b));
+  std::vector<RigidTransformEstimate> out;
+  for (size_t p = 0; p < nprob; ++p) out.push_back(transform_estimate(Ts[p], d, f[p]));
+  return out;
+}
+
 Eigen::VectorXd selectFromIndicator(const Eigen::VectorXd& x, const Eigen::VectorXi& ind)
 {
   long cnt = 0;

@@ -9,6 +9,7 @@
 #include "clp_batch_matrix.cuh"
 #include "clp_sdp.cuh"
 #include "clp_knn.cuh"
+#include "clp_transform.cuh"
 #include "clp_host_utils.h"
 #include "clp_jit.h"
 #include "../../include/clipper_b200.h"
@@ -177,6 +178,9 @@ struct clp_handle_s {
   DevBuf sdp_buf;
   // putative associations (clp_knn.cuh): staged clouds | partial lists | merged lists | counts and scans | staged A
   DevBuf knn_buf;
+  // rigid transform (clp_transform.cuh): bad key | problem table | rows | packed pairs | results; its pinned staging
+  DevBuf tf_buf;
+  PinnedBuf tf_pinned;
 
   size_t esize() const { return storage == CLP_STORE_F64 ? 8 : 4; }
   int entry_bytes() const { return sp.packed ? 4 : (int)esize() + 2; }  // compact copy: bytes per stored entry
@@ -1718,9 +1722,10 @@ int clp_destroy(clp_handle h) {
   for (DevBuf* b : {&h->Mbuf, &h->A_dev, &h->E1, &h->E2, &h->F12, &h->inv_prm, &h->D1dev, &h->D2dev, &h->vecs, &h->llbuf, &h->d2buf, &h->plan2buf, &h->sp_val, &h->sp_col, &h->sp_ptr4, &h->sp_part, &h->sp_item, &h->sp_rowid, &h->parts, &h->small,
                     &h->result, &h->u0dev, &h->ybuf, &h->sync, &h->panel, &h->cscbuf, &h->res_vecs, &h->res_cand, &h->res_pieces, &h->res_redll, &h->prof_buf,
                     &h->res_rval, &h->res_rcol, &h->res_roff, &h->res_rlen, &h->res_rbits, &h->res_rprod,
-                    &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf, &h->knn_buf})
+                    &h->mc_adj, &h->mc_work, &h->mc_scratch, &h->sdp_buf, &h->knn_buf, &h->tf_buf})
     b->release();
   h->pinned.release();
+  h->tf_pinned.release();
   if (h->ev0) cudaEventDestroy(h->ev0);
   if (h->ev1) cudaEventDestroy(h->ev1);
   if (h->stream && h->own_stream) cudaStreamDestroy(h->stream);
@@ -2229,6 +2234,8 @@ struct clp_batch_s {
   // putative associations (clp_knn.cuh): problem table | staged clouds | lists | scan | counts | 1-to-1 | staged A
   DevBuf knn_buf;
   PinnedBuf knn_pinned;     // the table and host clouds going up, the counts and host A coming back
+  DevBuf tf_buf;            // rigid transform (clp_transform.cuh), as clp_handle_s::tf_buf
+  PinnedBuf tf_pinned;
   int prof_on = env_int("CLP_PROF_BATCH", 0);
   PinnedBuf pinned;         // the caller's other inputs, then the results
   PinnedBuf pinned_points;  // D1 | D2 | A of scored problems (stage_points)
@@ -3572,6 +3579,164 @@ int batch_correspondences(clp_batch b, bool on_device, int32_t nprob, int32_t d,
   std::copy(ms.begin(), ms.end(), m_out);
   return CLP_OK;
 }
+
+// ---- rigid transform of selected associations (clp_transform.cuh) -------------------------------------------------
+// The inputs of the four clp_*estimate_transform* entries; a single call is a batch of one.  Host inputs: D1h, D2h, Ah
+// (column-major m x 2, NULL or m = 0: all-to-all) per problem; device inputs: pts (clp_points_dev).  rows and k are
+// host arrays.  Outputs: T_out[p] on the host (column-major), or T_dev at element strides ts.
+struct TfIn {
+  const double* const* D1h = nullptr; const double* const* D2h = nullptr; const int32_t* const* Ah = nullptr;
+  const int64_t* n1 = nullptr; const int64_t* n2 = nullptr; const int64_t* m = nullptr;
+  const clp_points_dev* pts = nullptr;
+  const int32_t* const* rows = nullptr; const int64_t* k = nullptr;
+  double* const* T_out = nullptr;
+  double* T_dev = nullptr; const int64_t* ts = nullptr;
+};
+
+// One host path for the handle (H = clp_handle_s) and the batch (clp_batch_s): only o's device, stream, events and error
+// string are used, and the transform's own scratch (buf, pin).  Everything is checked on the host first; the device
+// work is one upload (the pairs gathered on the host, or the rows for the device gather), a gather launch (device
+// inputs), the estimate launch and one readback.
+template <typename H>
+int estimate_transform(H* o, DevBuf& buf, PinnedBuf& pin, int32_t nprob, int32_t d, const TfIn& in, clp_tf_info* infos) {
+  const auto t_begin = std::chrono::steady_clock::now();
+  const bool dev = in.pts != nullptr;
+  const std::string who = "estimate transform: ";
+  auto tag = [&](int p) { return who + "problem " + std::to_string(p) + ": "; };
+  if (!infos || !in.n1 || !in.n2 || !in.k || nprob < 1)
+    return fail(o, CLP_ERR_INVALID, who + "n1, n2, k and infos are required, and nprob >= 1");
+  if (dev ? (!in.T_dev || !in.ts) : (!in.D1h || !in.D2h || !in.T_out))
+    return fail(o, CLP_ERR_INVALID, who + "NULL pointer arrays or output");
+  if (d < 1) return fail(o, CLP_ERR_INVALID, who + "d must be >= 1");
+  if (dev) {
+    auto ok = [](const int64_t* s) { return s[0] >= 0 && s[1] >= 1 && s[2] >= 1; };
+    if (!ok(in.pts->d1_strides) || !ok(in.pts->d2_strides) || (in.pts->A && !ok(in.pts->a_strides)) || !ok(in.ts))
+      return fail(o, CLP_ERR_INVALID, who + "bad strides (coordinate, point, row and column strides must be >= 1, batch "
+                                            "strides >= 0)");
+  }
+  // the problem table: sizes, rows and, for host inputs, every used association index
+  std::vector<TfProb> tab((size_t)nprob);
+  long long npairs = 0, nrows = 0, most = 1;
+  for (int p = 0; p < nprob; ++p) {
+    TfProb& P = tab[(size_t)p];
+    const int64_t n1 = in.n1[p], n2 = in.n2[p], m = in.m ? in.m[p] : 0;
+    if (n1 < 0 || n2 < 0 || m < 0) return fail(o, CLP_ERR_INVALID, tag(p) + "negative n1, n2 or m");
+    const double* D1 = dev ? in.pts->D1 : in.D1h[p];
+    const double* D2 = dev ? in.pts->D2 : in.D2h[p];
+    if ((n1 > 0 && !D1) || (n2 > 0 && !D2)) return fail(o, CLP_ERR_INVALID, tag(p) + "NULL point cloud");
+    if (!dev && !in.T_out[p]) return fail(o, CLP_ERR_INVALID, tag(p) + "NULL T_out");
+    const int32_t* A = dev ? in.pts->A : (in.Ah ? in.Ah[p] : nullptr);
+    const bool a2a = !A || m == 0;
+    const long long rows_of = a2a ? (long long)n1 * n2 : (long long)m;
+    const int32_t* rows = in.rows ? in.rows[p] : nullptr;
+    if (rows && in.k[p] < 0) return fail(o, CLP_ERR_INVALID, tag(p) + "k must be >= 0");
+    const long long k = rows ? (long long)in.k[p] : rows_of;
+    for (long long i = 0; i < ((rows || (!a2a && !dev)) ? k : 0); ++i) {  // every row 0 .. k-1 is in range
+      const long long r = rows ? (long long)rows[i] : i;
+      if (r < 0 || r >= rows_of)
+        return fail(o, CLP_ERR_INVALID, tag(p) + "row " + std::to_string(r) + " outside [0, " + std::to_string(rows_of) + ")");
+      if (!a2a && !dev && (A[r] < 0 || A[r] >= n1 || A[m + r] < 0 || A[m + r] >= n2))
+        return fail(o, CLP_ERR_INVALID, tag(p) + "association index out of range of D1/D2");
+    }
+    P.off = npairs; P.k = k; P.rows_off = (dev && rows) ? nrows : -1;
+    P.n1 = n1; P.n2 = n2; P.m = a2a ? 0 : m;
+    npairs += 2LL * d * k;
+    if (dev && rows) nrows += k;
+    most = std::max(most, k);
+  }
+  if (d != 2 && d != 3) return fail(o, CLP_ERR_UNSUPPORTED, who + "d = " + std::to_string(d) + ", only 2 and 3 are supported");
+  // scratch, every region 256-byte aligned; bad key | table | rows | pairs (host inputs) go up from pin as they lie
+  size_t at = 0;
+  auto take = [&](size_t bytes) { const size_t q = at; at = (at + bytes + 255) & ~(size_t)255; return q; };
+  const size_t o_bad = take(8), o_tab = take((size_t)nprob * sizeof(TfProb)), o_rows = take((size_t)nrows * 4);
+  const size_t o_pairs = take((size_t)npairs * 8);
+  const size_t up = dev ? o_pairs : at;
+  const size_t o_out = take((size_t)nprob * sizeof(TfOut));
+  CLP_CUDA(o, cudaSetDevice(o->device));
+  if (at > buf.cap) {
+    size_t free_b = 0, total_b = 0;
+    CLP_CUDA(o, cudaMemGetInfo(&free_b, &total_b));
+    if (at > free_b + buf.cap)
+      return fail(o, CLP_ERR_ALLOC, who + "the scratch (" + std::to_string(at) + " bytes) does not fit the free device memory (" +
+                                        std::to_string(free_b + buf.cap) + " bytes)");
+  }
+  CLP_CUDA(o, buf.ensure(at));
+  CLP_CUDA(o, pin.ensure(std::max(up, (size_t)nprob * sizeof(TfOut) + 256)));
+  char* hp = pin.as<char>();
+  std::memset(hp + o_bad, 0, 8);
+  std::memcpy(hp + o_tab, tab.data(), (size_t)nprob * sizeof(TfProb));
+  for (int p = 0; p < nprob; ++p) {
+    const TfProb& P = tab[(size_t)p];
+    const int32_t* rows = in.rows ? in.rows[p] : nullptr;
+    if (dev) {
+      if (P.rows_off >= 0 && P.k > 0) std::memcpy(hp + o_rows + (size_t)P.rows_off * 4, rows, (size_t)P.k * 4);
+      continue;
+    }
+    double* q = reinterpret_cast<double*>(hp + o_pairs) + P.off;
+    const double* D1 = in.D1h[p];
+    const double* D2 = in.D2h[p];
+    const int32_t* A = in.Ah ? in.Ah[p] : nullptr;
+    for (long long i = 0; i < P.k; ++i) {
+      const long long r = rows ? (long long)rows[i] : i;
+      const long long i1 = P.m == 0 ? r / P.n2 : A[r], i2 = P.m == 0 ? r % P.n2 : A[P.m + r];
+      for (int c = 0; c < d; ++c) {
+        q[c * P.k + i] = D1[i1 * d + c];
+        q[(d + c) * P.k + i] = D2[i2 * d + c];
+      }
+    }
+  }
+  const cudaStream_t st = o->stream;
+  char* base = buf.as<char>();
+  CLP_CUDA(o, cudaMemcpyAsync(base, hp, up, cudaMemcpyHostToDevice, st));
+  unsigned long long* bad = reinterpret_cast<unsigned long long*>(base + o_bad);
+  const TfProb* dtab = reinterpret_cast<const TfProb*>(base + o_tab);
+  double* pairs = reinterpret_cast<double*>(base + o_pairs);
+  TfOut* outs = reinterpret_cast<TfOut*>(base + o_out);
+  CLP_CUDA(o, cudaEventRecord(o->ev0, st));
+  if (dev) {
+    const clp_points_dev& s = *in.pts;
+    TfGatherArgs g;
+    std::memset(&g, 0, sizeof(g));
+    g.prob = dtab; g.nprob = nprob; g.d = d;
+    g.D1 = s.D1; g.D2 = s.D2; g.A = s.A;
+    for (int c = 0; c < 3; ++c) { g.s1[c] = s.d1_strides[c]; g.s2[c] = s.d2_strides[c]; g.sa[c] = s.a_strides[c]; }
+    g.rows = reinterpret_cast<const int*>(base + o_rows); g.pairs = pairs; g.bad = bad;
+    const dim3 grid((unsigned)std::min<long long>(64, (most + kTfThreads - 1) / kTfThreads), (unsigned)std::min(nprob, 65535));
+    tf_gather_kernel<<<grid, kTfThreads, 0, st>>>(g);
+    CLP_CUDA(o, cudaGetLastError());
+  }
+  TfEstimateArgs e;
+  std::memset(&e, 0, sizeof(e));
+  e.prob = dtab; e.nprob = nprob; e.pairs = pairs; e.out = outs; e.bad = bad;
+  if (dev) { e.T_dev = in.T_dev; for (int c = 0; c < 3; ++c) e.ts[c] = in.ts[c]; }
+  const unsigned grid = (unsigned)std::min(nprob, 1 << 20);
+  if (d == 2) tf_estimate_kernel<2><<<grid, kTfThreads, 0, st>>>(e);
+  else tf_estimate_kernel<3><<<grid, kTfThreads, 0, st>>>(e);
+  CLP_CUDA(o, cudaGetLastError());
+  CLP_CUDA(o, cudaEventRecord(o->ev1, st));
+  unsigned long long* h_bad = reinterpret_cast<unsigned long long*>(hp);
+  TfOut* h_out = reinterpret_cast<TfOut*>(hp + 256);
+  CLP_CUDA(o, cudaMemcpyAsync(h_bad, bad, 8, cudaMemcpyDeviceToHost, st));
+  CLP_CUDA(o, cudaMemcpyAsync(h_out, outs, (size_t)nprob * sizeof(TfOut), cudaMemcpyDeviceToHost, st));
+  CLP_CUDA(o, cudaStreamSynchronize(st));
+  if (const unsigned long long key = *h_bad)
+    return fail(o, CLP_ERR_INVALID, tag((int)(0xffffffffu - (unsigned int)(key & 0xffffffffu))) +
+                                        "association index out of range of D1/D2");
+  float ms = 0.f;
+  CLP_CUDA(o, cudaEventElapsedTime(&ms, o->ev0, o->ev1));
+  const double t = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count() / nprob;
+  const int E = d + 1;
+  for (int p = 0; p < nprob; ++p) {
+    const TfOut& r = h_out[p];
+    clp_tf_info& f = infos[p];
+    std::memset(&f, 0, sizeof(f));
+    f.status = r.status; f.k = tab[(size_t)p].k; f.rmse = r.rmse;
+    f.sv[0] = r.sv[0]; f.sv[1] = r.sv[1]; f.sv[2] = r.sv[2]; f.gap = r.gap;
+    f.t = t; f.kernel_ms = ms;
+    if (!dev) std::memcpy(in.T_out[p], r.T, (size_t)E * E * 8);
+  }
+  return CLP_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -3606,9 +3771,10 @@ int clp_batch_destroy(clp_batch b) {
   cudaSetDevice(b->device);
   for (DevBuf* d : {&b->in_d1, &b->in_d2, &b->in_a, &b->in_u0, &b->out_u, &b->probs, &b->outs, &b->nnz, &b->sync, &b->scratch, &b->prof, &b->mat_in, &b->custom_in,
                     &b->mc_probs, &b->mc_edges, &b->mc_adj, &b->mc_vint, &b->mc_tpre, &b->mc_out, &b->mc_state, &b->mc_rounds,
-                    &b->mc_pscratch, &b->mc_sscratch, &b->sdp_out, &b->knn_buf})
+                    &b->mc_pscratch, &b->mc_sscratch, &b->sdp_out, &b->knn_buf, &b->tf_buf})
     d->release();
   b->pinned.release();
+  b->tf_pinned.release();
   b->knn_pinned.release();
   b->pinned_points.release();
   if (b->ev0) cudaEventDestroy(b->ev0);
@@ -3829,6 +3995,52 @@ int clp_batch_correspondences_dev(clp_batch b, int32_t nprob, int32_t d, const d
   KnnBatchIn in;
   in.D1 = D1_dev; in.s1 = d1_strides; in.D2 = D2_dev; in.s2 = d2_strides; in.A_dev = A_dev; in.sa = a_strides;
   return guarded(b, [&] { return batch_correspondences(b, true, nprob, d, in, n1, n2, knn, radius, enforce_1to1, capacity, m); });
+}
+
+// a single call is a batch of one: the clp_score_*_dev layouts are the strides (0, 1, d) of the clouds, (0, 1, m) of A
+// and (0, 1, d + 1) of T
+int clp_estimate_transform(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2,
+                           const int32_t* A, int64_t m, const int32_t* rows, int64_t k, double* T_out, clp_tf_info* info) {
+  if (!h) return CLP_ERR_INVALID;
+  TfIn in;
+  in.D1h = &D1; in.D2h = &D2; in.Ah = &A; in.n1 = &n1; in.n2 = &n2; in.m = &m; in.rows = &rows; in.k = &k;
+  in.T_out = &T_out;
+  return guarded(h, [&] { return estimate_transform(h, h->tf_buf, h->tf_pinned, 1, d, in, info); });
+}
+
+int clp_estimate_transform_dev(clp_handle h, const double* D1_dev, int32_t d, int64_t n1, const double* D2_dev, int64_t n2,
+                               const int32_t* A_dev, int64_t m, const int32_t* rows, int64_t k, double* T_dev,
+                               clp_tf_info* info) {
+  if (!h) return CLP_ERR_INVALID;
+  clp_points_dev pts;
+  std::memset(&pts, 0, sizeof(pts));
+  pts.D1 = D1_dev; pts.D2 = D2_dev; pts.A = A_dev;
+  const int64_t dd = std::max<int64_t>(d, 1), ts[3] = {0, 1, dd + 1};
+  pts.d1_strides[1] = pts.d2_strides[1] = 1; pts.d1_strides[2] = pts.d2_strides[2] = dd;
+  pts.a_strides[1] = 1; pts.a_strides[2] = std::max<int64_t>(m, 1);
+  TfIn in;
+  in.pts = &pts; in.n1 = &n1; in.n2 = &n2; in.m = &m; in.rows = &rows; in.k = &k; in.T_dev = T_dev; in.ts = ts;
+  return guarded(h, [&] { return estimate_transform(h, h->tf_buf, h->tf_pinned, 1, d, in, info); });
+}
+
+int clp_batch_estimate_transform(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                                 const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                 const int32_t* const* rows, const int64_t* k, double* const* T_out, clp_tf_info* infos) {
+  if (!b) return CLP_ERR_INVALID;
+  TfIn in;
+  in.D1h = D1; in.D2h = D2; in.Ah = A; in.n1 = n1; in.n2 = n2; in.m = m; in.rows = rows; in.k = k; in.T_out = T_out;
+  return guarded(b, [&] { return estimate_transform(b, b->tf_buf, b->tf_pinned, nprob, d, in, infos); });
+}
+
+int clp_batch_estimate_transform_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts,
+                                     const int32_t* const* rows, const int64_t* k, double* T_dev, const int64_t t_strides[3],
+                                     clp_tf_info* infos) {
+  if (!b) return CLP_ERR_INVALID;
+  if (!pts) return fail(b, CLP_ERR_INVALID, "estimate transform: pts is required");
+  TfIn in;
+  in.pts = pts; in.n1 = pts->n1; in.n2 = pts->n2; in.m = pts->m; in.rows = rows; in.k = k; in.T_dev = T_dev;
+  in.ts = t_strides;
+  return guarded(b, [&] { return estimate_transform(b, b->tf_buf, b->tf_pinned, nprob, d, in, infos); });
 }
 
 }  // extern "C"

@@ -180,6 +180,33 @@ void pybind_correspondences(py::module& m)
         "D1s"_a, "D2s"_a, "knn"_a, "radius"_a, "enforce_1to1"_a,
         "distance_based_correspondences of every pair (D1s[p], D2s[p]) in one batched call on the GPU: a list of (m, 2) "
         "int32 arrays.");
+  auto tf_info = [](const clipper::utils::RigidTransformEstimate& r) {
+    return py::dict("status"_a = r.status, "k"_a = r.k, "rmse"_a = r.rmse, "gap"_a = r.gap, "sv"_a = from_vector(r.sv));
+  };
+  m.def("estimate_rigid_transform",
+        [tf_info](const py::array& D1, const py::array& D2, const py::array& A) {
+          const auto r = clipper::utils::estimateRigidTransform(to_matrix(D1, "D1"), to_matrix(D2, "D2"), to_assoc(A, "A"));
+          return py::make_tuple(from_matrix(r.T), tf_info(r));
+        },
+        "D1"_a, "D2"_a, "A"_a,
+        "(T, info): the proper rigid transform ((d+1, d+1), b ~ R a + t) aligning the pairs of every row of A, on the GPU; "
+        "info holds status, k, rmse, gap and sv.");
+  m.def("estimate_rigid_transform_many",
+        [tf_info](const std::vector<py::array>& D1s, const std::vector<py::array>& D2s, const std::vector<py::array>& As) {
+          std::vector<clipper::invariants::Data> M1, M2;
+          std::vector<clipper::Association> AA;
+          for (const py::array& a : D1s) M1.push_back(to_matrix(a, "D1s"));
+          for (const py::array& a : D2s) M2.push_back(to_matrix(a, "D2s"));
+          for (const py::array& a : As) AA.push_back(to_assoc(a, "As"));
+          py::list Ts, infos;
+          for (const auto& r : clipper::utils::estimateRigidTransformBatch(M1, M2, AA)) {
+            Ts.append(from_matrix(r.T));
+            infos.append(tf_info(r));
+          }
+          return py::make_tuple(Ts, infos);
+        },
+        "D1s"_a, "D2s"_a, "As"_a,
+        "estimate_rigid_transform of every problem in one batched call on the GPU: (list of T, list of info).");
 }
 
 void pybind_dsd(py::module& m)

@@ -58,6 +58,33 @@ namespace utils {
                                                              const std::vector<invariants::Data>& D2s, size_t knn,
                                                              double radius, bool enforce1to1);
 
+  /// the rigid transform that aligns associated points, and how well it is determined (clp_tf_info)
+  struct RigidTransformEstimate {
+    Eigen::MatrixXd T;   ///< (d+1) x (d+1), last row [0 .. 0 1]: b ~ R a + t maps the frame of D1 into that of D2
+    int status = 0;      ///< CLP_TF_OK, CLP_TF_EMPTY, CLP_TF_DEGENERATE or CLP_TF_NONFINITE
+    int k = 0;           ///< pairs used
+    double rmse = 0.0;   ///< sqrt(sum |R a_i + t - b_i|^2 / k)
+    double gap = 0.0;    ///< sv[d-2] + sign(det H) sv[d-1]: R is unique exactly when gap > 0
+    Eigen::VectorXd sv;  ///< the 3 singular values of H = sum (b_i - mu_b)(a_i - mu_a)', descending
+  };
+
+  /**
+   * @brief The proper rigid transform that aligns the pairs (D1.col(A(i,0)), D2.col(A(i,1))) of every row of A, e.g.
+   * getSelectedAssociations(), on the GPU (device 0, a temporary handle; clp_estimate_transform).  d is 2 or 3.  An empty
+   * A gives CLP_TF_EMPTY (no pairs; not the all-to-all hypothesis).  Semantics in full: include/clipper_b200.h.
+   */
+  RigidTransformEstimate estimateRigidTransform(const invariants::Data& D1, const invariants::Data& D2,
+                                                const Association& A);
+
+  /**
+   * @brief estimateRigidTransform of many problems in one batched call on the GPU (device 0, a temporary clp_batch;
+   * clp_batch_estimate_transform).  Entry p is bit for bit estimateRigidTransform(D1s[p], D2s[p], As[p]).  The three
+   * lists have the same length and every cloud the same number of rows; an empty list gives an empty result.
+   */
+  std::vector<RigidTransformEstimate> estimateRigidTransformBatch(const std::vector<invariants::Data>& D1s,
+                                                                  const std::vector<invariants::Data>& D2s,
+                                                                  const std::vector<Association>& As);
+
   /// simple named profiling timer (utils.h:107-163)
   class Timer
   {

@@ -505,6 +505,73 @@ int clp_batch_correspondences_dev(clp_batch b, int32_t nprob, int32_t d, const d
                                   int32_t knn, double radius, int enforce_1to1, int32_t* A_dev, const int64_t a_strides[3],
                                   int64_t capacity, int64_t* m);
 
+/* ---- rigid transform of selected associations (the last step of a registration) ---------------------------------------
+ * The proper rigid transform that aligns the pairs a set of rows of A names, on the device (clp_transform.cuh).  D1
+ * (d x n1) and D2 (d x n2) are fp64 and A (m x 2) int32 in the layouts of the scoring calls, read as they read them:
+ * A == NULL or m == 0 is the all-to-all hypothesis, row r = (r / n2, r mod n2) as clp_create_all_to_all orders it, so the
+ * nodes of a solve on all-to-all index the right pairs.
+ * Rows: rows (host, int32) lists k row indices of A, each counted once per listing, in the given order; rows == NULL
+ *   means every row 0 .. m-1 (k is then ignored).  Only the listed rows of A and the points they name are read.
+ * Estimate: pair i is a_i = D1[:, A(r_i, 0)], b_i = D2[:, A(r_i, 1)].  All arithmetic is fp64 in two passes: the means
+ *   mu_a, mu_b, then H = sum (b_i - mu_b)(a_i - mu_a)' on the centred points.  R is a proper rotation (det R = +1)
+ *   minimising sum |R a_i + t - b_i|^2 (Umeyama's correction of the SVD solution, no scale) and t = mu_b - R mu_a, so
+ *   b ~ R a + t: T maps the frame of D1 into the frame of D2.
+ * Outputs: T (d+1) x (d+1), column-major, last row [0 .. 0 1].  info.rmse = sqrt(sum |r_i|^2 / k) with the residual
+ *   r_i = R (a_i - mu_a) - (b_i - mu_b) (= R a_i + t - b_i).  info.sv: the singular values of H, descending (sv[2] = 0
+ *   for d = 2).  info.gap = sv[d-2] + sign(det H) sv[d-1], the sign +1 when det H = 0: R is unique exactly when gap > 0,
+ *   and its sensitivity to rounding is about sv[0] / gap.  info.k: the number of pairs used.
+ * Status (info.status):
+ *   CLP_TF_EMPTY       k = 0: T = I, rmse = 0, sv = gap = 0.
+ *   CLP_TF_NONFINITE   a used coordinate is not finite (or a sum overflows): R, t, rmse, sv and gap are NaN.
+ *   CLP_TF_DEGENERATE  sv[0] = 0 or gap <= 1e-12 sv[0] (one pair, collinear points in 3-D, all points equal): R is still
+ *                      a proper rotation and a minimiser (R = I when H = 0), but not the only one.
+ *   CLP_TF_OK          otherwise (coplanar points in 3-D included: the determinant fixes the third axis).
+ * Determinism: a repeated call is bit-identical; problem p of a batch is bit for bit the single call on the same inputs,
+ *   and a host call the device call; a problem's result depends on nothing it does not read (not on nprob, p or the
+ *   other problems).  info.t is the wall-clock seconds of the call (batches: divided by nprob), info.kernel_ms the device
+ *   time of its kernels.
+ * clp_estimate_transform: host D1, D2, A; T_out host.  clp_estimate_transform_dev: D1, D2 and A on the handle's device in
+ *   the clp_score_*_dev layouts (column-major, contiguous), T_out on the device.
+ * clp_batch_estimate_transform: host arrays of nprob pointers (A may be NULL, or A[p] NULL: all-to-all for problem p;
+ *   m may be NULL: all zero); T_out[p] host.  clp_batch_estimate_transform_dev: pts as clp_batch_*_dev take it (pts->A
+ *   == NULL: all-to-all everywhere, m[p] == 0: for problem p); entry (r, c) of problem p's T goes to T_dev[p t_strides[0]
+ *   + r t_strides[1] + c t_strides[2]] (element strides, so a torch (nprob, d+1, d+1) float64 tensor is written in place).
+ * rows and k are host arrays of nprob (rows itself or rows[p] may be NULL: all rows).  Only the handle's or batch's
+ * device, stream (clp_set_stream, clp_batch_set_stream) and error string are used, and a scratch of the transform's own:
+ * its matrix, solve state and kNN scratch stay as they were.  Every call returns when infos (and host T) are on the host.
+ * Errors, in this order, naming the first failing problem; the handle or batch stays usable:
+ *   CLP_ERR_INVALID for NULL pointers, nprob < 1, d < 1, negative sizes, bad strides (coordinate, point, row, column and T
+ *     row and column strides >= 1, batch strides >= 0), k < 0, a row outside [0, m) (m = n1 n2 for all-to-all) or a
+ *     host association index out of range;
+ *   CLP_ERR_UNSUPPORTED for d other than 2 and 3;
+ *   CLP_ERR_ALLOC when the scratch (2 d k doubles per problem, plus the rows) does not fit the free device memory;
+ *   CLP_ERR_INVALID, found on the device, for a device association index out of range, naming the lowest such problem;
+ *     nothing is written to T_dev then. */
+#define CLP_TF_OK 0
+#define CLP_TF_EMPTY 1
+#define CLP_TF_DEGENERATE 2
+#define CLP_TF_NONFINITE 3
+typedef struct clp_tf_info {
+  int32_t status;   /* CLP_TF_*                                                                 */
+  int64_t k;        /* pairs used                                                               */
+  double rmse;      /* sqrt(sum |R a_i + t - b_i|^2 / k)                                        */
+  double sv[3];     /* singular values of H, descending                                        */
+  double gap;       /* sv[d-2] + sign(det H) sv[d-1]                                            */
+  double t;         /* wall-clock seconds of the call (batches: divided by nprob)              */
+  double kernel_ms; /* device time of the call's kernels (CUDA events; batches: the whole call) */
+} clp_tf_info;
+int clp_estimate_transform(clp_handle h, const double* D1, int32_t d, int64_t n1, const double* D2, int64_t n2,
+                           const int32_t* A, int64_t m, const int32_t* rows, int64_t k, double* T_out, clp_tf_info* info);
+int clp_estimate_transform_dev(clp_handle h, const double* D1_dev, int32_t d, int64_t n1, const double* D2_dev, int64_t n2,
+                               const int32_t* A_dev, int64_t m, const int32_t* rows, int64_t k, double* T_dev,
+                               clp_tf_info* info);
+int clp_batch_estimate_transform(clp_batch b, int32_t nprob, int32_t d, const double* const* D1, const int64_t* n1,
+                                 const double* const* D2, const int64_t* n2, const int32_t* const* A, const int64_t* m,
+                                 const int32_t* const* rows, const int64_t* k, double* const* T_out, clp_tf_info* infos);
+int clp_batch_estimate_transform_dev(clp_batch b, int32_t nprob, int32_t d, const clp_points_dev* pts,
+                                     const int32_t* const* rows, const int64_t* k, double* T_dev, const int64_t t_strides[3],
+                                     clp_tf_info* infos);
+
 /* ---- semidefinite relaxation (solveAsMSRCSDR / sdp::solve, ref clipper.cpp:101-113, sdp.cpp:88-296) ---------------
  * Solves  maximise <M, X>  subject to  X PSD, tr X = 1, X_ij = 0 where C_ij = 0, X_ij >= 0 where C_ij != 0  on the
  * device by two-block ADMM (X in the spectraplex, Z in the polyhedral set), with a Jacobi eigensolver in shared memory
