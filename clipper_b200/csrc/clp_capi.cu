@@ -456,7 +456,7 @@ ResArgs res_args(clp_handle h) {
   a.wcol = h->res_wcol.as<int>();
   if (h->res_restrict) {
     a.rval = h->res_rval.as<float>(); a.rcol = h->res_rcol.as<unsigned short>(); a.roff = h->res_roff.as<unsigned int>();
-    a.rlen = h->res_rlen.as<unsigned int>(); a.rbits = h->res_rbits.as<unsigned int>(); a.rprod = h->res_rprod.as<double>();
+    a.rlen = h->res_rlen.as<unsigned int>(); a.rbits = h->res_rbits.as<unsigned int>(); a.rprod = h->res_rprod.as<uint4>();
   }
   a.sweeps = reinterpret_cast<ResSweeps*>(reinterpret_cast<char*>(h->result.p) + kSweepsAt);
   return a;
@@ -645,7 +645,7 @@ int build_sparse(clp_handle h, bool force, const CompactShape& s, ScoreHandoff h
     CLP_CUDA(h, h->res_roff.ensure(((size_t)NI + 1) * sizeof(unsigned int)));
     CLP_CUDA(h, h->res_rlen.ensure((size_t)h->rows_pad * sizeof(unsigned int)));
     CLP_CUDA(h, h->res_rbits.ensure((size_t)G * ((h->m + 31) / 32) * sizeof(unsigned int)));
-    CLP_CUDA(h, h->res_rprod.ensure((size_t)h->rows_pad * 2 * sizeof(double)));
+    CLP_CUDA(h, h->res_rprod.ensure((size_t)h->rows_pad * 2 * sizeof(uint4)));
     res_restrict_caps_kernel<<<(unsigned)((NI + 1 + 255) / 256), 256, 0, h->stream>>>(h->sp.itemptr, NI, (int)h->m, h->res_roff.as<unsigned int>());
     CLP_CUDA(h, cudaGetLastError());
     if (int rc = scan(h->res_roff.as<unsigned int>(), (long long)NI + 1, nullptr)) return rc;
@@ -1044,6 +1044,8 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
     if (h->prof_ctas) CLP_CUDA(h, h->prof_buf.ensure((size_t)h->res_G * 8 * sizeof(double)));
     // the per-CTA partial sums travel as LL cells tagged with the launch-local round number: start from tag 0
     CLP_CUDA(h, cudaMemsetAsync(h->res_redll.p, 0, (size_t)2 * h->res_G * kRedVals * sizeof(uint4), h->stream));
+    // so are the row products of the restricted sweeps
+    if (h->res_restrict) CLP_CUDA(h, cudaMemsetAsync(h->res_rprod.p, 0, (size_t)h->rows_pad * 2 * sizeof(uint4), h->stream));
     ResArgs ra = res_args(h);
     le = with_storage(h, [&](auto t) { return launch_resident_solver<decltype(t)>(h, ra); });
   } else {
@@ -1069,9 +1071,23 @@ int solve_core(clp_handle h, clp_solution* out, double* u_out_host, double* u_ou
     std::vector<double> pc((size_t)h->res_G * 8);
     CLP_CUDA(h, cudaMemcpy(pc.data(), h->prof_buf.p, pc.size() * sizeof(double), cudaMemcpyDeviceToHost));
     if (h->prof_ctas >= 2) {  // one line per CTA: index, ms in sweeps / epilogues / exchanges / staging, items, chunks
-      for (int b = 0; b < h->res_G; ++b)
-        std::fprintf(stderr, "[clp cta] %d %.4f %.4f %.4f %.4f %.0f %.0f\n", b, 1e-6 * pc[(size_t)b * 8], 1e-6 * pc[(size_t)b * 8 + 1],
+                              // (+ restricted entries swept and how far the costliest warp range of the restricted split lies above
+                              // its share, in costliest slots: below 1)
+      for (int b = 0; b < h->res_G; ++b) {
+        std::fprintf(stderr, "[clp cta] %d %.4f %.4f %.4f %.4f %.0f %.0f", b, 1e-6 * pc[(size_t)b * 8], 1e-6 * pc[(size_t)b * 8 + 1],
                      1e-6 * pc[(size_t)b * 8 + 2], 1e-6 * pc[(size_t)b * 8 + 3], pc[(size_t)b * 8 + 4], pc[(size_t)b * 8 + 5]);
+        if (h->res_restrict) std::fprintf(stderr, " %.0f %.4f", pc[(size_t)b * 8 + 6], pc[(size_t)b * 8 + 7]);
+        std::fprintf(stderr, "\n");
+      }
+    }
+    if (h->res_restrict) {  // the restricted entries each CTA swept (the split of res_restrict_split balances them)
+      double lo = 1e300, hi = 0, sum = 0, over = -1;
+      for (int b = 0; b < h->res_G; ++b) {
+        const double x = pc[(size_t)b * 8 + 6];
+        lo = std::min(lo, x); hi = std::max(hi, x); sum += x; over = std::max(over, pc[(size_t)b * 8 + 7]);
+      }
+      std::fprintf(stderr, "[clp prof] restricted entries per solve: min %.0f  mean %.1f  max %.0f over %d CTAs (split: costliest warp range "
+                   "above its share by %.3f costliest slots)\n", lo, sum / h->res_G, hi, h->res_G, over);
     }
     const char* nm[4] = {"sweeps", "epilogues", "exchanges", "staging"};
     for (int q = 0; q < 4; ++q) {

@@ -82,7 +82,8 @@ struct ResArgs {
   long long spin_limit;    // clock64 ticks a wait may last before it raises the time-out flag
   unsigned int pieces_cap, state_cap;  // on-chip piece table (entries) / row state (rows) per CTA, 0: keep them in HBM
   uint4* redll;            // [2][G][8] per-CTA partial sums as self-validating LL cells (zeroed before the launch)
-  double* prof_cta;        // nullable: [G][8] per-CTA phase times in ns (sweeps, epilogues, exchanges, staging), items, chunks
+  double* prof_cta;        // nullable: [G][8] per-CTA phase times in ns (sweeps, epilogues, exchanges, staging), items, chunks,
+                           //   restricted entries swept (rebuild and restricted evaluations), the split's largest overshoot (res_prof_split)
   int prof_laps;           // thread 0 of every CTA reads %globaltimer four times per evaluation (phase split in clp_solution)
   const int* wcol;         // packed layout: [G][warps][4] column of each member's last entry before the warp's stream (-1: none)
   // packed layout on one GPU: the restricted copy (res_restrict_build; null rval: every sweep reads the whole copy)
@@ -91,7 +92,8 @@ struct ResArgs {
   const unsigned int* roff;  // [NI + 1]
   unsigned int* rlen;      // [rows_pad] entries of every row slot (stream position 4 it + s), without the padding
   unsigned int* rbits;     // [G][ceil(m / 32)] S' as a column bitmap, one copy per CTA
-  double* rprod;           // [rows_pad][2] M w, C w of every row from the last restricted sweep
+  uint4* rprod;            // [rows_pad][2] M w, C w of every row slot from the last restricted sweep as LL cells tagged
+                           //   with the evaluation's round (zeroed before the launch)
   ResSweeps* sweeps;       // counters of the last solve (written by CTA 0)
 };
 
@@ -102,6 +104,11 @@ __host__ __device__ inline unsigned int res_restrict_cap(unsigned int row_entrie
   const unsigned int t = ((unsigned int)(m / kSupportDiv) + 3u) & ~3u;
   return row_entries < t ? row_entries : t;
 }
+// fixed charge of a row slot, in chunks, in the split of the restricted sweeps (res_restrict_split): the row's
+// reduction, shuffles and store, and the rest of its last, partly filled round (32 was faster than 8 and 64 at c2,
+// DESIGN.md section 6)
+constexpr unsigned int kRowCost = 32;
+static_assert(kRowCost >= 1, "every slot must cost something: the last range then ends at the last slot");
 
 // ---------------------------------------------------------------------------------------------------------------
 // mbarrier / bulk-copy primitives (SASS: SYNCS.*, UBLKCP)
@@ -720,24 +727,114 @@ __device__ void res_restrict_build(const ResArgs& a, int bid, const double* vs) 
   }
 }
 
-// The restricted sweep: warp w sums the CTA's rows w, w + NW, ... from their slots into rprod.  Lane l takes chunks
-// l, l + 32, ... of a row; RD rounds of RU chunks per lane are in flight, carried on from one row to the next.  The
-// copy was written by this CTA in this launch: plain loads, no ld.global.nc.
+// The split of the restricted sweeps, chosen at the first restricted evaluation after a rebuild: the row slots are cut
+// into G x NW contiguous ranges of equal cost, one per warp of the grid, a slot costing its chunks plus kRowCost; range
+// k = b NW + w goes to warp w of CTA b and is [t_k, t_{k+1}), t_k = the first slot whose prefix cost reaches k / (G NW)
+// of the total.  The rows' owners wrote rlen before the rebuild evaluation's exchange; every CTA reads all of it (L2
+// loads: this SM's L1 may still hold an older S') and adds the same integers in the same order, so all CTAs agree on
+// every bound without an exchange.  Thread t covers the items [t K, (t + 1) K), four slots each (one 16-byte load).
+// Writes the bounds of the CTA's warps to bnd[0..NW].
 template <int NT>
-__device__ void res_sweep_restricted(const ResArgs& a, int bid, const double* vs) {
-  constexpr int NW = NT / 32, RU = 2, RD = 2;
+__device__ void res_restrict_split(const ResArgs& a, int bid, unsigned int* bnd, unsigned int* red_u) {
+  constexpr int NW = NT / 32;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const unsigned int it0 = a.sp.cta_first[bid];
-  const int nrow = (int)(a.sp.cta_first[bid + 1] - it0) * 4;
-  for (int rb = warp; rb < nrow; rb += 32 * NW) {
-    // lane i: slot and padded length of the warp's row rb + NW i
-    const int nb = min(32, (nrow - rb + NW - 1) / NW);
+  const unsigned int NI = (unsigned int)a.NI, K = (NI + NT - 1) / NT;
+  const unsigned int s = min(NI, threadIdx.x * K), e = min(NI, s + K);
+  const uint4* len4 = reinterpret_cast<const uint4*>(a.rlen);
+  auto cost = [](unsigned int n) { return ((n + 3u) >> 2) + kRowCost; };
+  unsigned int own = 0u;
+#pragma unroll 4
+  for (unsigned int it = s; it < e; ++it) { const uint4 n = __ldcg(len4 + it); own += cost(n.x) + cost(n.y) + cost(n.z) + cost(n.w); }
+  unsigned int inc = own;  // inclusive scan over the warp, then over the warps' totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const unsigned int y = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += y; }
+  __syncthreads();
+  if (lane == 31) red_u[warp] = inc;
+  for (int k = threadIdx.x; k <= NW; k += NT) bnd[k] = (bid == 0 && k == 0) ? 0u : 4u * NI;  // t_0 = 0; no slot: past the end
+  __syncthreads();
+  unsigned int before = 0u;
+  unsigned long long T = 0ull;
+  for (int w = 0; w < NW; ++w) { const unsigned int x = red_u[w]; T += x; if (w < warp) before += x; }
+  // slot t is t_k for every k >= 1 with Q(t - 1) GW < k T <= Q(t) GW, Q(t) = the cost of slots 0..t (all positive)
+  const unsigned long long GW = (unsigned long long)a.G * NW, k0 = (unsigned long long)bid * NW;
+  unsigned long long Q = before + inc - own;
+  unsigned long long k = Q * GW / T + 1;  // the first target not reached before this thread's slots
+#pragma unroll 4
+  for (unsigned int it = s; it < e; ++it) {
+    const uint4 n = __ldcg(len4 + it);
+    const unsigned int n4[4] = {n.x, n.y, n.z, n.w};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      Q += cost(n4[q]);
+      for (; k * T <= Q * GW; ++k)
+        if (k >= k0 && k <= k0 + NW) bnd[k - k0] = 4u * it + (unsigned int)q + 1u;
+    }
+  }
+  __syncthreads();
+}
+
+// profile: the entries of the row slots [lo, hi) (returned to thread 0)
+template <int NT>
+__device__ unsigned int res_prof_slots(const ResArgs& a, unsigned int lo, unsigned int hi, unsigned int* red_u) {
+  constexpr int NW = NT / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  unsigned int sum = 0u;
+  for (unsigned int t = lo + threadIdx.x; t < hi; t += NT) sum += __ldcg(a.rlen + t);
+  sum = __reduce_add_sync(0xffffffffu, sum);
+  __syncthreads();
+  if (lane == 0) red_u[warp] = sum;
+  __syncthreads();
+  unsigned int s = 0u;
+  if (threadIdx.x == 0)
+    for (int w = 0; w < NW; ++w) s += red_u[w];
+  __syncthreads();
+  return s;
+}
+
+// profile: what res_restrict_split balances, recomputed from rlen and the bounds it wrote.  The costliest range of this
+// CTA's warps exceeds the share total / (G NW) by x times the costliest slot; the split keeps x < 1 (a range ends at
+// the first slot whose prefix cost reaches the next target).  Raises the CTA's slot 7 to x.
+template <int NT>
+__device__ void res_prof_split(const ResArgs& a, int bid, const unsigned int* bnd, unsigned int* red_u) {
+  constexpr int NW = NT / 32;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  auto cost = [&](unsigned int t) { return ((__ldcg(a.rlen + t) + 3u) >> 2) + kRowCost; };
+  unsigned int tot = 0u, cmax = 0u, mine = 0u;
+  for (unsigned int t = threadIdx.x; t < 4u * (unsigned int)a.NI; t += NT) { const unsigned int c = cost(t); tot += c; cmax = max(cmax, c); }
+  for (unsigned int t = bnd[warp] + (unsigned int)lane; t < bnd[warp + 1]; t += 32u) mine += cost(t);  // the warp's range
+  tot = __reduce_add_sync(0xffffffffu, tot);
+  cmax = __reduce_max_sync(0xffffffffu, cmax);
+  mine = __reduce_add_sync(0xffffffffu, mine);
+  __syncthreads();
+  if (lane == 0) { red_u[3 * warp] = tot; red_u[3 * warp + 1] = cmax; red_u[3 * warp + 2] = mine; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double T = 0.0, cm = 0.0, wm = 0.0;
+    for (int w = 0; w < NW; ++w) { T += (double)red_u[3 * w]; cm = fmax(cm, (double)red_u[3 * w + 1]); wm = fmax(wm, (double)red_u[3 * w + 2]); }
+    const double GW = (double)a.G * NW;
+    a.prof_cta[(size_t)bid * 8 + 7] = fmax(a.prof_cta[(size_t)bid * 8 + 7], (wm * GW - T) / (cm * GW));
+  }
+  __syncthreads();
+}
+
+// The restricted sweep: the calling warp sums the row slots lo, lo + step, ... < hi into their LL cells in rprod, tagged
+// ptag.  Lane l takes chunks l, l + 32, ... of a row; RD rounds of RU chunks per lane are in flight, carried on from one
+// row to the next.  A row's sums depend on its slot alone, not on which CTA or warp sweeps it.  The slots may have been
+// written by another CTA earlier in this launch: L2 loads (ld.global.cg), no ld.global.nc and no L1.
+__device__ void res_sweep_restricted(const ResArgs& a, unsigned int lo, unsigned int hi, unsigned int step, const double* vs,
+                                     unsigned int ptag) {
+  constexpr int RU = 2, RD = 2;
+  const int lane = threadIdx.x & 31;
+  const int nrow = hi > lo ? (int)((hi - lo + step - 1) / step) : 0;
+  for (int rb = 0; rb < nrow; rb += 32) {
+    // lane i: slot and padded length of the warp's row rb + i
+    const int nb = min(32, nrow - rb);
     unsigned int slot = 0u, len = 0u;
     if (lane < nb) {
-      const unsigned int t = 4u * it0 + (unsigned int)(rb + NW * lane), it = t >> 2;
+      const unsigned int t = lo + step * (unsigned int)(rb + lane), it = t >> 2;
       const unsigned int r0 = a.roff[it];
       slot = r0 + (t & 3u) * ((a.roff[it + 1] - r0) >> 2);
-      len = (a.rlen[t] + 3u) & ~3u;
+      len = (__ldcg(a.rlen + t) + 3u) & ~3u;
     }
     int ci = 0;             // producer cursor: row of the batch, first entry of its next round
     unsigned int ck = 0u;
@@ -753,8 +850,8 @@ __device__ void res_sweep_restricted(const ResArgs& a, int bid, const double* vs
       for (int u = 0; u < RU; ++u) {
         const unsigned int k = ck + 4u * (unsigned int)lane + 128u * u;
         if (k < n0) {
-          X[s][u] = *reinterpret_cast<const float4*>(a.rval + s0 + k);
-          K[s][u] = *reinterpret_cast<const uint2*>(a.rcol + s0 + k);
+          X[s][u] = __ldcg(reinterpret_cast<const float4*>(a.rval + s0 + k));
+          K[s][u] = __ldcg(reinterpret_cast<const uint2*>(a.rcol + s0 + k));
         } else {
           X[s][u] = make_float4(0.f, 0.f, 0.f, 0.f);
           K[s][u] = make_uint2((unsigned int)a.m * 0x10001u, (unsigned int)a.m * 0x10001u);  // column m holds 0.0
@@ -789,10 +886,7 @@ __device__ void res_sweep_restricted(const ResArgs& a, int bid, const double* vs
             accM += __shfl_xor_sync(0xffffffffu, accM, o);
             accC += __shfl_xor_sync(0xffffffffu, accC, o);
           }
-          if (lane == 0) {
-            double* p = a.rprod + 2 * (4ull * it0 + (unsigned long long)(rb + NW * srow[s]));
-            p[0] = accM; p[1] = accC;
-          }
+          if (lane < 2) ll_store(a.rprod + 2ull * (lo + step * (unsigned int)(rb + srow[s])) + lane, lane ? accC : accM, ptag);
           aM[0] = aM[1] = aC[0] = aC[1] = 0.0;
         }
         produce(s);
@@ -800,6 +894,26 @@ __device__ void res_sweep_restricted(const ResArgs& a, int bid, const double* vs
       if (done) break;
     }
   }
+}
+
+// M w, C w of one row slot from its two LL cells (res_sweep_restricted): a cell whose tag is not ptag yet is re-polled;
+// one that does not arrive within spin_limit raises the error flag
+__device__ __forceinline__ void res_rprod_take(const uint4* p, unsigned int ptag, long long spin_limit, int* errp,
+                                               double& Mv, double& Cv) {
+  unsigned int lo[2], t1[2], hi[2], t2[2];
+#pragma unroll
+  for (int e = 0; e < 2; ++e) ll_ld4<false>(p + e, lo[e], t1[e], hi[e], t2[e]);
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    long long t0 = 0;
+    while (!(t1[e] == ptag && t2[e] == ptag)) {
+      if (t0 == 0) t0 = clock64();
+      else if (clock64() - t0 > spin_limit) { atomicExch(errp, 1); break; }
+      ll_ld4<false>(p + e, lo[e], t1[e], hi[e], t2[e]);
+    }
+  }
+  Mv = __hiloint2double((int)hi[0], (int)lo[0]);
+  Cv = __hiloint2double((int)hi[1], (int)lo[1]);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -970,6 +1084,12 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
     if (threadIdx.x < kStageBlocks) mbar_init(&sbars[threadIdx.x], 1);
     fence_mbar_init();
   }
+  // the row slots of this CTA's warps in the restricted sweeps, warp w: [rbnd[w], rbnd[w + 1]) (res_restrict_split), and
+  // their entries (rbnd[NW + 1]): in the part of fin that only the sharded exchange uses
+  static_assert(kMaxPeers * kRedVals * 2 >= kResWarps + 2, "fin holds the restricted split");
+  unsigned int* const rbnd = reinterpret_cast<unsigned int*>(fin + 2 * kRedVals);
+  if constexpr (restrict_ok)
+    if (a.prof_cta && threadIdx.x == 0) { a.prof_cta[(size_t)bid * 8 + 6] = 0.0; a.prof_cta[(size_t)bid * 8 + 7] = -1.0; }
   __syncthreads();
 
   // piece table and per-row state (u, gradF, Mhat u, Chat u of the current and the next iterate): on chip when the
@@ -1032,6 +1152,7 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
   long long n_fallback = 0;
   double r_entries = 0.0, r_padding = 0.0;
   bool rhave = false;                // the restricted copy holds S'
+  bool rsplit = false;               // rbnd holds the split of the current S'
   int skind = SW_FULL;               // sweep of the current evaluation
   int cur = 0, cpar = 0, red_par = 0, status = 0, i_outer = 0;
   double d = 0.0, F = 0.0, sum_cur = 0.0, z = 0.0, sw = 0.0;  // z, sw: |w|^2 and sum(w) of the candidate the next evaluation stages
@@ -1150,12 +1271,32 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         if (skind == SW_FULL) {
           RES_SWEEP();
         } else {
+          // a rebuild evaluation is swept by the rows' owners; the restricted evaluations that follow it by the split
+          // of the new S', which the owners' rlen gives once the rebuild evaluation's exchange has published it
+          unsigned int* const red_u = reinterpret_cast<unsigned int*>(red_s);
+          const int warp = threadIdx.x >> 5;
           if (skind == SW_REBUILD) {
             res_restrict_build<NT>(a, bid, vs);
-            rhave = true;
+            rhave = true; rsplit = false;
             __syncthreads();
+            if (a.prof_cta) {
+              const unsigned int n = res_prof_slots<NT>(a, 4u * it0, 4u * it1, red_u);
+              if (threadIdx.x == 0) a.prof_cta[(size_t)bid * 8 + 6] += (double)n;
+            }
+            res_sweep_restricted(a, 4u * it0 + (unsigned int)warp, 4u * it1, (unsigned int)NW, vs, (unsigned int)(round + 1));
+          } else {
+            if (!rsplit) {
+              res_restrict_split<NT>(a, bid, rbnd, red_u);
+              rsplit = true;
+              if (a.prof_cta) {
+                const unsigned int n = res_prof_slots<NT>(a, rbnd[0], rbnd[NW], red_u);
+                if (threadIdx.x == 0) rbnd[NW + 1] = n;
+                res_prof_split<NT>(a, bid, rbnd, red_u);
+              }
+            }
+            if (a.prof_cta && threadIdx.x == 0) a.prof_cta[(size_t)bid * 8 + 6] += (double)rbnd[NW + 1];
+            res_sweep_restricted(a, rbnd[warp], rbnd[warp + 1], 1u, vs, (unsigned int)(round + 1));
           }
-          res_sweep_restricted<NT>(a, bid, vs);
           ++n_matvec;
           __syncthreads();
           RES_LAP(ns_mv);
@@ -1170,8 +1311,9 @@ __device__ void res_solve_body(const ResArgs& a, unsigned char* smem) {
         RES_FOR_ROWS(i, itx, sx) {
           double Mv, Cv;
           if (skind != SW_FULL) {
+            // the row's sums, from whichever CTA swept its slot in this evaluation
             const unsigned int t = 4u * itx + (unsigned int)sx, n = a.rlen[t];
-            Mv = a.rprod[2ull * t]; Cv = a.rprod[2ull * t + 1];
+            res_rprod_take(a.rprod + 2ull * t, (unsigned int)(round + 1), a.spin_limit, errp, Mv, Cv);
             loc[6] += (double)n; loc[7] += (double)((0u - n) & 3u);
           } else {
             res_gather_pieces(ptab, isub, ptab_sh, wmask, itx, sx, w0_, w1_, Mv, Cv);

@@ -10,14 +10,17 @@ from clp_last_solve_sweeps and clp_sparse_info:
                     (the power step and the first normalisation always sweep the whole copy)
   rebuilds          one pass of the compact copy read + 6 bytes written per kept entry (not counted: a few %)
   restricted sweeps 6 bytes (fp32 value + 16-bit column) per entry and padding entry read
-"dense_equivalent" is what the same evaluations would read with one full pass each, as bench.py assumes.  Prints ONE
-JSON line per workload.
+"dense_equivalent" is what the same evaluations would read with one full pass each, as bench.py assumes.  One more solve
+on a handle made with CLP_PROF_CTAS=1 gives the spread over the CTAs (min / mean / max) of the sweep time and of the
+restricted entries each CTA swept; the phase times above come from solves without it.  Prints ONE JSON line per workload.
 """
 import argparse
 import json
 import os
+import re
 import subprocess
 import sys
+import tempfile
 
 import numpy as np
 
@@ -35,11 +38,46 @@ def card():
         return {"name": None, "error": str(e)}
 
 
-def profile(clp, datagen, name, solves):
-    prob = datagen.config_problem(name); cfg = prob["cfg"]
+def scored(clp, prob):
+    cfg = prob["cfg"]
     ip = clp.invariants.EuclideanDistanceParams(); ip.sigma, ip.epsilon = cfg["sigma"], cfg["epsilon"]
     c = clp.CLIPPER(clp.invariants.EuclideanDistance(ip), clp.Params())
     c.score_pairwise_consistency(prob["D1"], prob["D2"], prob["A"])
+    return c
+
+
+def cta_spread(clp, prob):
+    """one solve with the per-CTA timers (CLP_PROF_CTAS=1, read when a handle is made): the library's "[clp prof]" lines,
+    which it writes to stderr, as {quantity: {min, mean, max}}"""
+    os.environ["CLP_PROF_CTAS"] = "1"
+    try:
+        c = scored(clp, prob)
+    finally:
+        del os.environ["CLP_PROF_CTAS"]
+    with tempfile.TemporaryFile(mode="w+") as tmp:
+        sys.stderr.flush()
+        saved = os.dup(2)
+        os.dup2(tmp.fileno(), 2)
+        try:
+            c.solve(prob["u0"])
+        finally:
+            os.dup2(saved, 2)
+            os.close(saved)
+        tmp.seek(0)
+        text = tmp.read()
+    out = {}
+    for ln in text.splitlines():
+        m = re.match(r"\[clp prof\] (.+?) per solve: min (\S+)\s+mean (\S+)\s+max (\S+)", ln)
+        if m:
+            key = m.group(1).strip().replace(" ", "_") + ("_ms" if "entries" not in m.group(1) else "")
+            lo, mean, hi = (float(x) for x in m.group(2, 3, 4))
+            out[key] = {"min": lo, "mean": mean, "max": hi, "max_over_mean": hi / mean if mean else None}
+    return out
+
+
+def profile(clp, datagen, name, solves):
+    prob = datagen.config_problem(name); cfg = prob["cfg"]
+    c = scored(clp, prob)
     _, pass_bytes = c.sparse_info()
     c.solve(prob["u0"])
     rows = []
@@ -61,6 +99,7 @@ def profile(clp, datagen, name, solves):
         "kernel_ms": {"median": float(np.median(k[:, 0])), "min": float(k[:, 0].min()), "max": float(k[:, 0].max())},
         "phase_ms_cta0": {"sweeps_and_staging": float(np.median(k[:, 1])), "epilogues": float(np.median(k[:, 2])),
                           "exchanges": float(np.median(k[:, 3]))},
+        "per_cta": cta_spread(clp, prob),
         "card": card(),
     }
 
